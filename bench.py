@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- IAF-transform throughput on B200 (BASELINE.json metric).
+"""bench.py -- IAF-transform throughput on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload c2a|c2b|...]
+                    [--dump-outputs DIR]
 
 A "step" is one fused IAF step (masked-AR conv stack -> mu, s -> z' = (z - .1 mu)/exp(.1 s),
 per-element arw_logsd, per-sample logdet) over one GLOBAL batch of 256 synthetic samples of
@@ -14,7 +15,9 @@ n_z=32, 16x16 (SURVEY 8d).  Metric: latent elements/s = 256*n_z*H*W / t_step, wh
                overlaps the next group's kernels.  CUDA events around the whole region, max over ranks.
                The steps rotate through NSETS input/output sets whose footprint exceeds L2.
 * roofline   : the step kernel(s) alone: one CUDA graph of K back-to-back launches, CUDA events;
-               bound = whichever of algorithmic-bytes/HBM-peak and algorithmic-flops/bf16-peak is larger.
+               bound = whichever of algorithmic-bytes/HBM-peak and algorithmic-flops/fp16-peak is larger
+               (data-sheet peaks of the card's model, e.g. H100 SXM 3.35 TB/s HBM3, 989 dense fp16 TFLOP/s at 700 W;
+               the card's power limit is recorded in config).
 * e2e        : same metric through the public host-buffer entry (IAFOperator.submit_host ->
                iaf_step_submit_host): pinned host inputs H2D, step, results D2H, every step,
                pipelined over three device staging slots; timed until wait_host() returns.
@@ -26,6 +29,11 @@ n_z=32, 16x16 (SURVEY 8d).  Metric: latent elements/s = 256*n_z*H*W / t_step, wh
                serves both: per thread-count candidate 3 warm-up + 5 timed calls (median), the best
                candidate then runs the timed steps; the b200 arm runs it in a fresh subprocess so that
                both arms measure under the same conditions.
+
+--dump-outputs DIR: after the timed steps, the arrays the last timed step of the headline workload computed
+(z', per-element arw_logsd, per-sample logdet; float32 .npy) and the ELBO scalars of the timed region (float64).  The
+inputs are seeded, so two builds can be compared output for output.  At N > 1 rank 0 writes its shard of the batch
+(the ELBO scalars are the all-reduced, global ones).
 
 N>1: launched by torchrun, one rank per GPU; the GLOBAL batch of 256 is sharded (256/N samples per rank:
 strong scaling, north_star / SURVEY 8e), weights replicated, no data-path collective.
@@ -62,13 +70,28 @@ METRIC = "IAF latents/sec (z',logdet) @ n_z=32,16x16,bs256"
 UNIT = "latent elements/s"
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), "measured (MEASURED_PEAKS.json, burst)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
+L2_BYTES = 50 * 2 ** 20  # H100
+
+
+def peaks(device):
+    """HBM GB/s and dense fp16 tensor TFLOP/s from NVIDIA's data sheet of the card's model (H100 SXM: 700 W; H100 PCIe:
+    350 W); a card with a lower power limit than the sheet's reaches less, so the limit goes into the line beside them."""
+    name = torch.cuda.get_device_name(device)
+    if "H100" in name and "PCIe" in name:
+        return 2000.0, 756.0, "H100 PCIe data sheet (350 W)"
+    if "H100" in name:
+        return 3350.0, 989.0, "H100 SXM data sheet (700 W)"
+    raise SystemExit("bench.py: no data-sheet peaks for %s" % name)
+
+
+def power_limit_w(index):
+    """The card's enforced power limit in watts (NVML), or None when NVML is not available."""
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        return pynvml.nvmlDeviceGetEnforcedPowerLimit(pynvml.nvmlDeviceGetHandleByIndex(index)) / 1000.0
+    except Exception:  # pragma: no cover
+        return None
 
 
 # ----------------------------------------------------------------------------------------------
@@ -352,7 +375,7 @@ class DeviceBench(object):
         self.B = Bg // world
         self.Bg, self.n_z, self.hidden, self.H, self.W, self.E = Bg, n_z, hidden, H, W, E
         self.alg_bytes_unit = 4 * self.B * H * W * (n_z + hidden[0] + n_z + n_z) + 4 * self.B
-        nsets = max(2, -(-3 * 126 * 2 ** 20 // self.alg_bytes_unit))  # footprint >= 3x the 126 MB L2
+        nsets = max(2, -(-3 * L2_BYTES // self.alg_bytes_unit))  # footprint >= 3x the L2
         self.nsets = -(-nsets // E) * E                                # a whole number of ELBO groups
         self.op, self.layers_cpu, self.sets = make_workload(name, device, self.nsets, B=self.B)
         self.lib = self.op._lib
@@ -490,7 +513,17 @@ class DeviceBench(object):
         (ms,) = self._max_over_ranks([e0.elapsed_time(e1)])
         direct = self.op.launch_count() - l0
         n_launched = direct if direct else K * self.launches_per_step  # graph replays do not pass through the C ABI
+        self.scal = scal
         return ms * 1e-3 / K, int(n_launched), float(scal.sum()), len(groups)
+
+    def dump_outputs(self, K, out_dir):
+        """What the last of the K timed steps computed (it wrote set (K - 1) % nsets), plus the ELBO scalars."""
+        os.makedirs(out_dir, exist_ok=True)
+        s = self.sets[(K - 1) % self.nsets]
+        torch.cuda.synchronize()
+        for key, name in (("z_out", "z_out"), ("logsd", "arw_logsd"), ("logdet", "logdet")):
+            np.save(os.path.join(out_dir, name + ".npy"), s[key].detach().float().cpu().numpy())
+        np.save(os.path.join(out_dir, "elbo_scalars.npy"), self.scal.detach().double().cpu().numpy())
 
     def training_pair(self, iters=20):
         """Forward that keeps the activations (iaf_step_fwd_train) and backward from them (iaf_step_bwd_saved: gradients of z,
@@ -518,7 +551,7 @@ class DeviceBench(object):
                 "backward_path": op.backward_path(self.H, self.W, self.device)}
 
     def roofline(self, t_kernel):
-        hbm_gbs, bf16_tf, peak_src = measured_peaks()
+        hbm_gbs, bf16_tf, peak_src = peaks(self.device)
         op, H, W, dev = self.op, self.H, self.W, self.device
         alg_bytes = op.algorithmic_bytes(self.B, H, W, dev)
         alg_flops = op.algorithmic_flops(self.B, H, W, dev)
@@ -574,7 +607,9 @@ class DeviceBench(object):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=400)
+    ap.add_argument("--steps", type=int, default=400,
+                    help="timed steps of the headline region (value and roofline); the e2e, also and cpu_baseline legs "
+                         "size their own windows and report their step counts")
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default="c2a", choices=sorted(WORKLOADS))  # c2a = the headline
@@ -583,6 +618,9 @@ def main():
     ap.add_argument("--no-also", action="store_true", help="skip the second headline shape")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--batch", type=int, default=0, help="development: override the workload's global batch")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs (and the ELBO scalars) as .npy files into DIR; under "
+                         "torchrun rank 0 writes its own shard (samples [0, 256 / N)) of the global batch")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -625,6 +663,8 @@ def main():
         sampler.phase = "timed"
     t_kernel = db.time_kernels(K)
     t_step, n_launched, elbo_sum, n_groups = db.time_elbo_groups(K)
+    if args.dump_outputs and rank == 0:
+        db.dump_outputs(K, args.dump_outputs)
     if sampler:
         sampler.phase = "between"
     elems_step = db.Bg * db.n_z * db.H * db.W
@@ -682,10 +722,12 @@ def main():
         "ms_per_step": t_step * 1e3, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
         "dtype": "f32 (tc path: fp16 hi/lo operand pairs, three products per MAC, f32 accumulate)" if path == "tc" else "f32",
         "data": "synthetic",
-        "config": {"workload": workload_string(name), "global_batch": db.Bg, "samples_per_gpu": db.B,
+        "config": {"gpu": torch.cuda.get_device_name(device), "power_limit_w": power_limit_w(local_rank),
+                   "workload": workload_string(name), "global_batch": db.Bg, "samples_per_gpu": db.B,
                    "parallelism": "dp%d" % world, "path": path, "launch": db.launch_mode,
                    "kernels_per_step": db.launches_per_step, "steps_per_elbo": db.E, "elbo_evaluations": n_groups,
-                   "l2": "rotating %d input/output sets (%.0f MB > 126 MB L2)" % (db.nsets, db.nsets * db.alg_bytes_unit / 2 ** 20),
+                   "l2": "rotating %d input/output sets (%.0f MB > %d MB L2)" % (
+                       db.nsets, db.nsets * db.alg_bytes_unit / 2 ** 20, L2_BYTES // 2 ** 20),
                    "collective": ("one NCCL all-reduce of the ELBO scalar per evaluation (%d steps), on a side stream"
                                   % db.E) if world > 1 else "none",
                    "samples_per_s": value / (db.n_z * db.H * db.W)},

@@ -1,4 +1,4 @@
-"""Build libiaf_b200.so in-tree with nvcc for sm_100a (no JIT cache, no torch extension)."""
+"""Build libiaf_b200.so in-tree with nvcc for sm_90a (Hopper; no JIT cache, no torch extension)."""
 import os
 import shutil
 import subprocess
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libiaf_b200.so")
 SOURCES = ["iaf_capi.cu", "iaf_pack.cu", "iaf_simt.cu", "iaf_tc.cu", "iaf_bwd.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 
 

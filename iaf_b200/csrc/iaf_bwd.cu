@@ -576,7 +576,7 @@ __global__ void __launch_bounds__(BW_THREADS, 2) iaf_bwd_wgrad_kernel(const __gr
 __global__ void __launch_bounds__(BW_THREADS) iaf_bwd_reduce_kernel(const float* part, float* out, int n, int NG, int stride) {
   // One block per 32 outputs, one warp per SEGMENT of the NG split-K partials: warp w sums partials w, w + 8, w + 16, ...
   // (four interleaved chains, fixed order), then a fixed tree over the 8 segments.  Deterministic; NG / 32 dependent
-  // round trips per thread instead of NG / 8 (C2a's 64x64 layers have NG = 296: 40 us -> a few us per layer).
+  // round trips per thread instead of NG / 8 (a few hundred partials per output for small layers).
   __shared__ float seg_sum[BW_RED_SEG][32];
   const int lane = threadIdx.x & 31, seg = threadIdx.x >> 5;
   const int i = blockIdx.x * 32 + lane;
@@ -905,8 +905,8 @@ static int bw_ensure_scratch(IafBwdPlan* pl, int B) {
   if (cudaMalloc(&pl->hb, sizeof(float) * B * pl->ncol[last] * hw) != cudaSuccess) return IAF_ERR_CUDA;
   for (int a = 0; a < 2 && maxh; ++a)
     if (cudaMalloc(&pl->G[a], sizeof(float) * B * maxh * hw) != cudaSuccess) return IAF_ERR_CUDA;
-  // weight gradient: enough CTAs per tile to fill the machine twice over (the first version used a flat 32 and left
-  // C2a's 64x64 layers on 32 of 148 SMs: 1.76 ms; measured after: see DESIGN.md), never more than there are units
+  // weight gradient: enough CTAs per tile to fill the machine twice over (a flat count leaves most SMs idle on small
+  // layers), never more than there are units
   const int n_bands = (pl->d.H + pl->wg_RB - 1) / pl->wg_RB;
   size_t pmax = 0;
   for (int j = 0; j < pl->n_stages; ++j) {
@@ -957,7 +957,7 @@ int iaf_bwd_run(IafBwdPlan* pl, const IafBwdArgs* a, cudaStream_t stream, int* n
   int st = bw_ensure_scratch(pl, B);
   if (st != IAF_OK) return st;
   int nl_ = 0;
-  // elementwise kernels: grid-stride, at most 4 CTAs per SM on 148 SMs
+  // elementwise kernels: grid-stride, at most 592 CTAs (4 per SM and more on 132 SMs)
   auto ew_grid = [](size_t total) { return (int)std::min<size_t>(592, (total + BW_THREADS - 1) / BW_THREADS); };
 
   // activations: recomputed below, or the ones the training forward kept

@@ -162,7 +162,7 @@ const char* iaf_strerror(int status) {
     case IAF_OK: return "ok";
     case IAF_ERR_BAD_ARG: return "bad argument (null pointer or non-positive size)";
     case IAF_ERR_BAD_SHAPE: return "bad shape (channel counts must divide one another; two heads must be equal)";
-    case IAF_ERR_UNSUPPORTED: return "configuration not supported by the B200 kernels";
+    case IAF_ERR_UNSUPPORTED: return "configuration not supported by the H100 kernels";
     case IAF_ERR_CUDA: return "CUDA error (see iaf_last_cuda_error)";
     case IAF_ERR_NOT_PACKED: return "iaf_pack_weights has not been called on this plan";
     case IAF_ERR_NO_DEVICE: return "no CUDA device";

@@ -1,35 +1,25 @@
-// Tensor-core path of the fused IAF step: tcgen05 implicit GEMM on sm_100a.
+// Tensor-core path of the IAF step: wgmma implicit GEMM on sm_90a (Hopper).
 //
 // Formulation.  Every sample's H x W plane is laid out as a stream of "slots" with one
 // zero pad column per row and one zero row per sample (pitch Wp = W+1, SPS = (H+1)*Wp
 // slots per sample), all samples back to back.  In that stream a conv tap (dy,dx) is a
-// pure slot shift of dy*Wp+dx, the SAME zero padding is the pad slots, and the whole
-// masked-AR stack becomes, for every tile of 128 consecutive slots,
+// pure slot shift of dy*Wp+dx, the SAME zero padding is the pad slots, and every conv
+// stage of the masked-AR stack becomes, for every tile of 128 consecutive slots,
 //     D[128 x N] = sum over 5 live taps t, channel blocks k:  A_t,k[128 x 16] * W_t,k[16 x N]
 // with A_t,k simply the activation matrix read 'shift_t' rows further down.  Activations
-// live in shared memory in the UMMA no-swizzle K-major canonical layout
-//     [channel chunk of 8][slot][8 x bf16]          (16 B per slot per chunk)
-// so a tap shift is +16 B per slot on the descriptor start address, and the epilogue of
-// one layer (thread == slot == TMEM lane) writes the next layer's operand with fully
-// coalesced, conflict-free 16-byte stores.  Hidden activations never leave the SM.
+// live in shared memory in the wgmma no-swizzle K-major canonical layout
+//     [channel chunk of 8][slot][8 x fp16]          (16 B per slot per chunk)
+// so a tap shift is +16 B per slot on the descriptor start address.
 //
-// Precision.  north_star asks for 1e-4 relative parity with the fp32 reference; bf16 (or
-// tf32) single-pass operands cannot hold that through K = 160..800 and the 8192-element
-// log-det sum (SURVEY hard part 1).  Operands are therefore split x = hi + lo (both fp16,
-// 22 significant bits together; see umma_idesc) and three MMAs are issued per K block:
-// hi*hi + lo*hi + hi*lo, fp32 accumulation in TMEM.  Roofline numbers are always quoted
-// on ALGORITHMIC flops, not on the 3x issued.
+// Precision.  The step must match the fp32 reference to 1e-4 relative; bf16 (or tf32)
+// single-pass operands cannot hold that through K = 160..800 and the 8192-element log-det
+// sum.  Operands are therefore split x = hi + lo (both fp16, 22 significant bits together;
+// see wg_desc_lo) and three MMAs are issued per K block: hi*hi + lo*hi + hi*lo, fp32
+// accumulation.  Roofline numbers are always quoted on ALGORITHMIC flops, not on the 3x issued.
 //
-// Schedule.  Dependencies only run forward in the stream (a slot needs slots s .. s+Wp+1 of
-// the layer below), so a CTA walks a contiguous run of tiles as a wavefront.  One control
-// warp issues every tcgen05.mma; 16 worker warps (4 per TMEM lane quadrant, splitting the
-// accumulator columns) load z, run the epilogues and write the next layer's operand ring.
-// In period s the tensor pipe runs M_j(s+1-2j) while the workers run L(s+1), E_j(s-2j):
-// accumulators are double-buffered in TMEM, operand rings hold two tiles plus a mirrored
-// margin (so a shifted 128-row window never wraps), and every hand-off is an mbarrier
-// (TMA-style expect_tx for the weights, tcgen05.commit for MMA completion).
+// Schedule: one launch per conv stage (iaf_tc_gemm.cuh); the same stage kernel runs the data
+// gradient of the backward on the point-reflected stream.
 // Orientation of the Theano variant: see iaf_simt.cu (point reflection on load/store).
-#include <cuda.h>  // CUtensorMap (the encoder is fetched through cudaGetDriverEntryPoint: no link-time libcuda dependency)
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -41,36 +31,15 @@
 
 #include "iaf_tc.h"
 
-#ifndef TC_WORKERS
-#define TC_WORKERS 16  // worker warps (multiple of 4: TMEM lane quadrants)
-#endif
+#define TC_WORKERS 16  // worker warps of the stage kernel (four warpgroups)
 #define TC_WTHREADS (TC_WORKERS * 32)
-#define TC_THREADS (TC_WTHREADS + 64)
-#define TC_CTRL_WARP TC_WORKERS
-#define TC_RED_WARP (TC_WORKERS + 1)
 #define TC_TILE 128
 #ifdef IAF_TC_TIMELINE
 #define TC_SMEM_LIMIT (227 * 1024 - 512 - 2560)  // room for the static event buffers
 #else
 #define TC_SMEM_LIMIT (227 * 1024 - 512)  // opt-in maximum minus the kernels' static shared memory (barriers: < 512 B)
 #endif
-#ifndef TC_NGROUPS
-#define TC_NGROUPS 1   // 1: all 16 worker warps run every phase together; 2: two ping-pong groups by tile parity
-#endif
-#define TC_GWARPS (TC_WORKERS / TC_NGROUPS)
-#define TC_GTHREADS (TC_GWARPS * 32)
-#define TC_ZITEMS (TC_GTHREADS >= 512 ? 2 : (TC_GTHREADS >= 256 ? 3 : 5))  // z-window (slot, chunk) items per loader thread
-
-enum {
-  BAR_W = 0, BAR_ZFULL = 1, BAR_ZEMPTY = 2,
-  BAR_ACC_FULL = 3,    // + 2*j + b
-  BAR_ACC_EMPTY = 13,  // + 2*j + b
-  BAR_H_FULL = 23,     // + 2*j + b   (ring written by stage j)
-  BAR_H_EMPTY = 31,    // + 2*j + b
-  BAR_PART = 40,       // + tile parity: the workers' partial sums of a heads tile are deposited
-  BAR_PART_EMPTY = 42, // + tile parity: the reducer warp has consumed them
-  BAR_COUNT = 44
-};
+#define TC_ZITEMS 2  // z-window (slot, chunk) items per worker thread
 
 struct IafTcStage {
   const __nv_bfloat16* whi;  // global packed [K/8][N][8]
@@ -79,22 +48,9 @@ struct IafTcStage {
   const float* padw;         // [4][N] or nullptr
   float* hid_out;            // training forward: this (hidden) stage's activations, fp32 [B][N][HW]; nullptr = not kept
   int cin, N, K;
-  int w_bytes;               // K*N*2
-  int sm_whi, sm_wlo;        // smem byte offsets of the resident weight images
-  int sm_in;                 // smem byte offset of this stage's input operand (hi plane set)
-  int in_slots;              // slots per chunk plane of the input buffer
-  int sm_bias;               // smem byte offset of the fp32 bias (+ padw) table: [5][N]
-  int tmem_col;
-  int dbl;                   // accumulator double-buffered in TMEM
-  int merged;                // hi*[hi|lo] issued as ONE N' = 2N MMA (A is fetched once for both): accumulator spans 2N cols
-  int acc_cols;              // N or 2N
 };
 
-#define IAF_FZ_MAXROWS 10  // image rows a 16x16 tile window can touch ((WIN + Wp - 2) / Wp + 1)
 struct IafTcParams {
-  // iaf_fz_kernel, staged variant: TMA descriptor of z viewed as a 4-D tensor (x, y, channel, sample), box = one image
-  // row of every channel; 64-byte aligned as the hardware requires of a descriptor passed in kernel-parameter space
-  alignas(64) unsigned char tmap_z[IAF_FZ_MAXROWS][128];  // [r - 1]: box = r image rows of every channel of one sample
   const float* z; const float* ctx;
   const float* post_mean; const float* post_logsd; const float* prior_mean; const float* prior_logsd;
   float* z_out; float* elem; float* bc_out; float* persample_out;
@@ -105,28 +61,13 @@ struct IafTcParams {
   int B, C, H, W, Wp, SPS, HW;
   int S;         // total slots
   int NT;        // tiles
-  int MIR;       // mirrored margin (slots)
-  int WIN;       // z window slots (128 + MIR)
-  int RING;      // ring slots (256 + MIR)
+  int MIR;       // largest tap shift, rounded up to 8 (slots)
+  int WIN;       // A window slots (128 + MIR)
   int MAXS;      // max samples intersecting one tile
   int sm_part;   // smem byte offset of the per-tile partial-sum scratch
   int flip, nl;
   float scale;
-  int tmem_cols;
-  int prefetch;  // IAF_TC_PREFETCH: 1 bulk L2 prefetch of this CTA's context range at kernel start, 2: context and z,
-                 // 4: per-thread prefetch.global.L2 of the next tile's z window / context one period ahead
   unsigned mg_sps, mg_wp, mg_win;  // magic multipliers for fast_div
-  // iaf_fz_kernel (one hidden layer, independent overlapped tiles) only:
-  int TO;        // output slots per tile (128 - MIR)
-  int h_bytes;   // bytes of one hidden-activation operand buffer (hi + lo plane sets of 128 slots)
-  int z_bytes;   // bytes of one z operand window (hi + lo plane sets of WIN slots, rounded up to 128)
-  int nzw;       // z operand windows: 2 (loaders a full tile ahead) or 1
-  int nhb;       // hidden-activation operand buffers: 2, or 1 (staged variant: the space goes to a second staging buffer)
-  int nzs;       // fp32 z staging buffers (staged variant): 2 = the TMA copies run two tiles ahead of the loader warps
-  int zst_bytes; // bytes of one staging buffer
-  int sm_zst;    // byte offset of the fp32 z staging buffer the bulk copies land in (staged variant, 16x16 planes)
-  int dbg;       // IAF_FZ_DBG (development, timing only, results WRONG when set): 1 loaders issue no global loads,
-                 // 2 loaders also skip their stores, 4 E0 does nothing but the hand-off, 8 E1 likewise, 16 no MMAs, 32 no weight load
 };
 
 // ------------------------------------------------------------------------------------------
@@ -160,88 +101,38 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// one lane of a converged warp (the compiler then issues the tcgen05 ops straight from the uniform datapath)
-__device__ __forceinline__ uint32_t elect_one_sync() {
-  uint32_t pred = 0, laneid = 0;
-  asm volatile(
-      "{\n\t.reg .b32 %%rx;\n\t.reg .pred %%px;\n\t"
-      "elect.sync %%rx|%%px, %2;\n\t"
-      "@%%px mov.s32 %1, 1;\n\t"
-      "mov.s32 %0, %%rx;\n\t}"
-      : "+r"(laneid), "+r"(pred)
-      : "r"(0xFFFFFFFFu));
-  return pred;
-}
 __device__ __forceinline__ void worker_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(TC_WTHREADS) : "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], 16-bit operands (formats in the instruction descriptor) -> f32
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// Hopper warpgroup MMA (wgmma), all four warps of a warpgroup converged.  D[64 x 16] += A[64 x 16] * B[16 x 16]: fp16
+// operands from shared-memory descriptors (both K-major, or both MN-major with MN = 1), fp32 accumulators in registers.
+// Fragment of a thread (warp w of the warpgroup): d[4j + 2h + e] = row 16 w + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e.
+template <int MN>
+__device__ __forceinline__ void wgmma_m64n16k16(float* d, uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %11;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a_desc), "l"(b_desc), "r"(1), "n"(MN)
       : "memory");
 }
-// The same with the A-operand collector: `fill` keeps the A tile this instruction fetched, `lastuse` takes A from the
-// collector instead of shared memory (the caller names the same descriptor) and releases it.  SASS: UTCHMMA .A_KEEP / .A_REUSE.
-__device__ __forceinline__ void umma_f16_afill(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16.collector::a::fill [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_alast(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16.collector::a::lastuse [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// UMMA shared-memory descriptor, SWIZZLE_NONE, K-major (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-// canonical layout ((8,n),2):((16B,SBO),LBO): 8 rows x 16 B core matrices, SBO between 8-row groups
-// (128 B here: rows are linear at 16 B pitch), LBO between the two 8-element K chunks of one K=16 MMA.
-// Low word: start address >> 4 | (LBO >> 4) << 16.  High word: SBO >> 4 | version(1) << 14.
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
+// wgmma shared-memory matrix descriptor, no swizzle, K-major: canonical layout ((8,m),(8,2)):((16B,SBO),(1,LBO)) of
+// 8-row x 16-byte core matrices; SBO between 8-row groups (128 B here: rows are linear at 16 B pitch), LBO between the
+// two 8-element K chunks of one K = 16 instruction.  Low word: start address >> 4 | (LBO >> 4) << 16.  High word:
+// SBO >> 4 (base offset 0, layout type 0 = no swizzle).  Adding n to the low word moves the start by n x 16 bytes.
+// Why fp16 pairs and not bf16 pairs: the residual of a two-term WEIGHT split is the same for every pixel and so adds
+// up coherently over the 8192 elements of a sample's log-det (bf16 + bf16 leaves 2^-17 |w|, ~2e-4 absolute against the
+// fp64 oracle over 256 samples; fp16 + fp16 leaves 2^-23 |w|).  Weight-normalised weights are bounded by their gain
+// (|w| <= exp(g), exp(3s)); see split_store8 for the activations' range.
+__device__ __forceinline__ uint32_t wg_desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
   return ((saddr >> 4) & 0x3FFFu) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
 }
-#define UMMA_DESC_HI ((128u >> 4) | (1u << 14))
-__device__ __forceinline__ uint64_t mk_desc(uint32_t lo) { return ((uint64_t)UMMA_DESC_HI << 32) | lo; }
-// Instruction descriptor (InstrDescriptor): f32 accumulate, A and B fp16 (a_format bits [7,10), b_format bits [10,13):
-// 0 = f16, 1 = bf16), both K-major, M=128.  Why fp16 pairs and not bf16 pairs: the residual of a two-term WEIGHT split
-// is the same for every pixel and so adds up coherently over the 8192 elements of a sample's log-det (bf16 + bf16 leaves
-// 2^-17 |w|: ~2e-4 absolute, measured on the B200 against the fp64 oracle over all 256 samples; fp16 + fp16 leaves
-// 2^-23 |w|).  Weight-normalised weights are bounded by their gain (|w| <= exp(g), exp(3s)); see split_store8 for the
-// activations' range.
-__device__ __forceinline__ uint32_t umma_idesc(int N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(TC_TILE >> 4) << 24);
-}
-
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+#define WG_DESC_HI (128u >> 4)
+__device__ __forceinline__ uint64_t mk_desc(uint32_t lo) { return ((uint64_t)WG_DESC_HI << 32) | lo; }
 
 // exp via ex2.approx.ftz (2 ulp): used where 1e-7-level error is far inside the 1e-4 parity budget
 __device__ __forceinline__ float fast_exp(float x) {
@@ -270,27 +161,6 @@ __device__ __forceinline__ float tc_apply_nl(float v, int nl) {
   }
 }
 
-// Packed fp32 pairs (sm_100: FADD2 / FMUL2 / FFMA2, one issue slot for two lanes' worth of work).  Only used by the
-// -DTC_FAST_EPI build of the epilogues (development variant for A/B: fewer worker instructions per tile; the default
-// build is the one every number in DESIGN.md was measured with).
-__device__ __forceinline__ void add2(float& a0, float& a1, float b0, float b1) {
-  asm("{\n\t.reg .b64 ra, rb, rd;\n\tmov.b64 ra, {%0, %1};\n\tmov.b64 rb, {%2, %3};\n\tadd.rn.f32x2 rd, ra, rb;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "+f"(a0), "+f"(a1) : "f"(b0), "f"(b1));
-}
-__device__ __forceinline__ void sub2(float& a0, float& a1, float b0, float b1) {
-  asm("{\n\t.reg .b64 ra, rb, rd;\n\tmov.b64 ra, {%0, %1};\n\tmov.b64 rb, {%2, %3};\n\tsub.rn.f32x2 rd, ra, rb;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "+f"(a0), "+f"(a1) : "f"(b0), "f"(b1));
-}
-__device__ __forceinline__ void mul2(float& a0, float& a1, float b0, float b1) {
-  asm("{\n\t.reg .b64 ra, rb, rd;\n\tmov.b64 ra, {%0, %1};\n\tmov.b64 rb, {%2, %3};\n\tmul.rn.f32x2 rd, ra, rb;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "+f"(a0), "+f"(a1) : "f"(b0), "f"(b1));
-}
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 // split 8 floats into fp16 hi / lo (22 significant bits together) and store both 16-byte vectors.  fp16, not bf16: the
 // a_lo * w_lo product the three-MMA scheme drops and the residual of the two-term split both shrink 64x (CPU simulation
 // tools/experiments/prec_sim.py: worst per-sample log-det error on C2a 1.3e-4 with bf16 pairs, 5e-6 with fp16 pairs).
@@ -302,9 +172,7 @@ __device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, ui
   for (int i = 0; i < 4; ++i) {
     const __half2 hh = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
     const float2 hf = __half22float2(hh);
-    float r0 = v[2 * i], r1 = v[2 * i + 1];
-    sub2(r0, r1, hf.x, hf.y);
-    const __half2 ll = __floats2half2_rn(r0, r1);
+    const __half2 ll = __floats2half2_rn(v[2 * i] - hf.x, v[2 * i + 1] - hf.y);
     h[i] = *reinterpret_cast<const uint32_t*>(&hh);
     l[i] = *reinterpret_cast<const uint32_t*>(&ll);
   }
@@ -356,713 +224,21 @@ __device__ __forceinline__ SlotInfo decode_slot(const IafTcParams& p, int s, int
   return si;
 }
 
-// ------------------------------------------------------------------------------------------
-// the kernel.  PADW: Theano pad-channel bias; MODE: IAF_MODE_STEP | IAF_MODE_LAYER;
-// NLT: IAF_NL_ELU for the fast elu path, -1 for the run-time switch.
-// ------------------------------------------------------------------------------------------
-template <bool PADW, int MODE, int NLT, int THW>
-__global__ void __launch_bounds__(TC_THREADS, 1) iaf_tc_kernel(const __grid_constant__ IafTcParams p) {
-  const int HW = THW ? THW : p.HW;  // compile-time plane size turns every channel stride into an immediate
-  extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bars[BAR_COUNT];
-  __shared__ uint32_t s_tmem;
-  TL_DECL
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nst = p.n_stages;
-  const int G = gridDim.x;
-  const int t0 = (int)((long long)blockIdx.x * p.NT / G);
-  const int t1 = (int)((long long)(blockIdx.x + 1) * p.NT / G);
-  const int nt = t1 - t0;
-  const int s_max = nt + 2 * nst - 3;  // last period: heads on tile nt-1 at s = nt-1 + 2(nst-1)
-
-  // ---- one-time setup ----
-  // Programmatic dependent launch: let the next grid in the stream start launching while this one runs (its CTAs
-  // take the SMs our short-run CTAs free early), and do our own TMEM allocation / barrier init before waiting for
-  // the previous grid; nothing that another kernel may have written is touched before griddepcontrol.wait.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  if (warp == TC_CTRL_WARP) {
-    tmem_alloc(&s_tmem, (uint32_t)p.tmem_cols);
-    if (lane == 0) {
-      mbar_init(&bars[BAR_W], 1);
-      mbar_init(&bars[BAR_ZFULL], TC_GWARPS);
-      mbar_init(&bars[BAR_ZEMPTY], 1);
-      for (int i = 0; i < 10; ++i) {
-        mbar_init(&bars[BAR_ACC_FULL + i], 1);
-        mbar_init(&bars[BAR_ACC_EMPTY + i], TC_GWARPS);
-      }
-      for (int i = 0; i < 8; ++i) {
-        mbar_init(&bars[BAR_H_FULL + i], TC_GWARPS);
-        mbar_init(&bars[BAR_H_EMPTY + i], 1);
-      }
-      mbar_init(&bars[BAR_PART], TC_GWARPS);
-      mbar_init(&bars[BAR_PART + 1], TC_GWARPS);
-      mbar_init(&bars[BAR_PART_EMPTY], 1);
-      mbar_init(&bars[BAR_PART_EMPTY + 1], 1);
-      fence_barrier_init();
-      asm volatile("griddepcontrol.wait;" ::: "memory");
-      uint32_t total = 0;
-      for (int j = 0; j < nst; ++j) total += 2u * (uint32_t)p.st[j].w_bytes;
-      mbar_expect_tx(&bars[BAR_W], total);
-      for (int j = 0; j < nst; ++j) {
-        for (int off = 0; off < 2 * p.st[j].w_bytes; off += 32768) {
-          const uint32_t n = (uint32_t)min(32768, 2 * p.st[j].w_bytes - off);
-          bulk_g2s(smem + p.st[j].sm_whi + off, reinterpret_cast<const uint8_t*>(p.st[j].whi) + off, n, &bars[BAR_W]);
-        }
-      }
-    }
-  } else if (warp < TC_WORKERS) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    // bias (+ pad-channel) tables -> smem: [5][N] per stage (row 0 bias, rows 1..4 padw)
-    for (int j = 0; j < nst; ++j) {
-      float* tb = reinterpret_cast<float*>(smem + p.st[j].sm_bias);
-      const int N = p.st[j].N;
-      for (int i = tid; i < 5 * N; i += TC_WTHREADS) {
-        float v = 0.f;
-        if (i < N) v = __ldg(p.st[j].bias + i);
-        else if (PADW) v = __ldg(p.st[j].padw + (i - N));
-        tb[i] = v;
-      }
-    }
-  }
-  if (warp == TC_RED_WARP) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    // Optional (IAF_TC_PREFETCH): pull this CTA's whole input range into L2 now, in tile order, so that the workers'
-    // per-phase global loads later hit L2 instead of paying an HBM round trip inside the L -> E0 -> E1 chain.  The
-    // samples a CTA touches are contiguous in NCHW, so the range is one block per tensor.
-    if ((p.prefetch & 3) && nt > 0) {
-      const int n_first = fast_div(t0 * TC_TILE, p.SPS, p.mg_sps);
-      const int n_last = min(p.B - 1, fast_div(t1 * TC_TILE - 1, p.SPS, p.mg_sps));
-      const size_t c_bytes = (size_t)p.st[0].N * HW * 4, z_bytes = (size_t)p.C * HW * 4;
-      const int nsm = n_last - n_first + 1;
-      const uint32_t CH = 8192;
-      if (p.ctx && nst > 1) {
-        const uint8_t* base = reinterpret_cast<const uint8_t*>(p.ctx) + (size_t)n_first * c_bytes;
-        const size_t tot = (size_t)nsm * c_bytes;
-        for (size_t off = (size_t)lane * CH; off < tot; off += 32 * (size_t)CH) {
-          const uint32_t nb = (uint32_t)min((size_t)CH, tot - off);
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(base + off), "r"(nb) : "memory");
-        }
-      }
-      if ((p.prefetch & 3) >= 2) {
-        const uint8_t* base = reinterpret_cast<const uint8_t*>(p.z) + (size_t)n_first * z_bytes;
-        const size_t tot = (size_t)nsm * z_bytes;
-        for (size_t off = (size_t)lane * CH; off < tot; off += 32 * (size_t)CH) {
-          const uint32_t nb = (uint32_t)min((size_t)CH, tot - off);
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(base + off), "r"(nb) : "memory");
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
-
-  if (warp == TC_CTRL_WARP) {
-    // =====================================================================================
-    // control warp: one lane issues every MMA of this CTA
-    // =====================================================================================
-    // the whole warp walks the schedule (convergent, so addresses live in uniform registers);
-    // a single elected lane issues the MMAs and commits
-    {
-      mbar_wait(&bars[BAR_W], 0);
-      for (int s = -1; s <= s_max; ++s) {
-        for (int j = 0; j < nst; ++j) {
-          const int k = s + 1 - 2 * j;
-          if (k < 0 || k >= nt + (nst - 1 - j)) continue;
-          const IafTcStage& St = p.st[j];
-          const int b = St.dbl ? (k & 1) : 0;
-          const int use = St.dbl ? (k >> 1) : k;
-          if (j == 0) {
-            mbar_wait(&bars[BAR_ZFULL], (uint32_t)(k & 1));
-          } else {
-            mbar_wait(&bars[BAR_H_FULL + 2 * (j - 1) + (k & 1)], (uint32_t)((k >> 1) & 1));
-            mbar_wait(&bars[BAR_H_FULL + 2 * (j - 1) + ((k + 1) & 1)], (uint32_t)(((k + 1) >> 1) & 1));
-          }
-          if (use >= 1) mbar_wait(&bars[BAR_ACC_EMPTY + 2 * j + b], (uint32_t)((use - 1) & 1));
-          tc_fence_after();
-          if (lane == 0) TL(0, 100 + j, k);
-
-          const uint32_t d_tmem = tmem_base + (uint32_t)(St.tmem_col + b * St.acc_cols);
-          const uint32_t idesc = umma_idesc(St.N), idesc2 = umma_idesc(2 * St.N);
-          const int merged = St.merged;
-          const uint32_t a_plane = (uint32_t)St.in_slots * 16u;
-          const uint32_t a_base = smem_u32(smem + St.sm_in) + (uint32_t)((j == 0 ? 0 : (k & 1) * TC_TILE)) * 16u;
-          const uint32_t nchunk = (uint32_t)(St.cin >> 3);
-          const uint32_t b_plane = (uint32_t)(2 * St.N) * 16u;  // weight image plane: N hi rows then N lo rows
-          // descriptor low words; every step below is a plain add in units of 16 B
-          const uint32_t ah0 = umma_desc_lo(a_base, a_plane);
-          const uint32_t al0 = umma_desc_lo(a_base + nchunk * a_plane, a_plane);
-          uint32_t bh = umma_desc_lo(smem_u32(smem + St.sm_whi), b_plane);
-          uint32_t bl = umma_desc_lo(smem_u32(smem + St.sm_whi) + (uint32_t)St.N * 16u, b_plane);
-          const uint32_t a_kstep = (2u * a_plane) >> 4, b_kstep = (2u * b_plane) >> 4;
-          const int nks = St.cin >> 4;
-          if (elect_one_sync()) {
-          uint32_t acc = 0;
-          // (rolled on purpose: unrolled over the taps this issue code was 175 tcgen05.mma instructions / ~35 KB of SASS
-          //  per kernel and missed the instruction cache on every burst; see iaf_fz.cuh)
-#pragma unroll 1
-          for (int tp = 0; tp < IAF_NTAPS; ++tp) {
-            const uint32_t shv = tp < 2 ? (uint32_t)tp : (uint32_t)(p.Wp + tp - 3);  // slot shifts 0, 1, Wp-1, Wp, Wp+1
-            uint32_t ah = ah0 + shv, al = al0 + shv;
-#pragma unroll 1
-            for (int ks = 0; ks < nks; ++ks) {
-              if (merged) {
-                // hi * [hi | lo] as one N' = 2N instruction (A fetched once for both), then lo * hi into the hi half
-                umma_f16(d_tmem, mk_desc(ah), mk_desc(bh), idesc2, acc);
-                umma_f16(d_tmem, mk_desc(al), mk_desc(bh), idesc, 1u);
-              } else {
-                umma_f16(d_tmem, mk_desc(al), mk_desc(bh), idesc, acc);  // lo * hi
-                umma_f16(d_tmem, mk_desc(ah), mk_desc(bl), idesc, 1u);   // hi * lo
-                umma_f16(d_tmem, mk_desc(ah), mk_desc(bh), idesc, 1u);   // hi * hi
-              }
-              acc = 1;
-              ah += a_kstep; al += a_kstep; bh += b_kstep; bl += b_kstep;
-            }
-          }
-          umma_commit(&bars[BAR_ACC_FULL + 2 * j + b]);
-          if (j == 0) umma_commit(&bars[BAR_ZEMPTY]);
-          else umma_commit(&bars[BAR_H_EMPTY + 2 * (j - 1) + (k & 1)]);
-          TL(0, 200 + j, k);
-          }
-          __syncwarp();
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp < TC_WORKERS) {
-    // =====================================================================================
-    // worker warps: z loader + epilogues.  TMEM lane quadrant = warp % 4; the 4 warps of a
-    // quadrant split the accumulator columns in groups of 16.
-    // =====================================================================================
-    // two ping-pong groups of 8 warps: group g runs every phase of the tiles with (k & 1) == g, so one
-    // group's load / barrier latency is covered by the other group's arithmetic
-    const int q = warp & 3, cg = (warp >> 2) % (TC_GWARPS / 4), grp = warp / TC_GWARPS, gwarp = warp % TC_GWARPS, gtid = tid % TC_GTHREADS;
-    constexpr int CGS = TC_GWARPS / 4;  // warps sharing one lane quadrant = stride over column groups
-    const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-    float* s_part = reinterpret_cast<float*>(smem + p.sm_part);
-    const int nch0 = p.st[0].cin >> 3;
-    const int n_zitems = p.WIN * nch0;
-
-    for (int s = -1; s <= s_max; ++s) {
-      // ------------------------------ L(s+1): z window of stage-0 tile s+1 ------------------
-      const int kz = s + 1;
-      if (kz < nt + nst - 1 && (TC_NGROUPS == 1 || (kz & 1) == grp)) {
-        const IafTcStage& S0 = p.st[0];
-        const int plane = S0.in_slots * 16;
-        const int lo_off = nch0 * plane;
-        float v[TC_ZITEMS][8];
-        int dsto[TC_ZITEMS];
-#pragma unroll
-        for (int it = 0; it < TC_ZITEMS; ++it) {
-          const int idx = gtid + it * TC_GTHREADS;
-          dsto[it] = -1;
-          if (idx < n_zitems) {
-            const int ch = fast_div(idx, p.WIN, p.mg_win);
-            const int sl = idx - ch * p.WIN;
-            dsto[it] = ch * plane + sl * 16;
-#ifdef TC_HALO_TRIM
-            // development variant: the extra (halo) tile of a two-stage stack only feeds the first MIR hidden slots of
-            // the next CTA's range, i.e. z slots [0, 2*MIR): the rest of its window is never consumed (rows of an MMA are
-            // independent), so it is neither loaded nor written
-            if (nst == 2 && kz == nt && sl >= 2 * p.MIR) { dsto[it] = -1; continue; }
-#endif
-            const SlotInfo si = decode_slot(p, (t0 + kz) * TC_TILE + sl, HW);
-            if (si.valid) {
-              const size_t g = ((size_t)si.n * p.C + ch * 8) * HW + si.gp;
-#pragma unroll
-              for (int e = 0; e < 8; ++e) v[it][e] = __ldg(p.z + g + (size_t)e * HW);
-              if (MODE == IAF_MODE_LAYER) {  // z0 = mean + exp(logsd) * eps   (tf_train.py:57, distributions.py:20)
-#pragma unroll
-                for (int e = 0; e < 8; ++e)
-                  v[it][e] = fmaf(fast_exp(__ldg(p.post_logsd + g + (size_t)e * HW)), v[it][e],
-                                  __ldg(p.post_mean + g + (size_t)e * HW));
-              }
-            } else {
-#pragma unroll
-              for (int e = 0; e < 8; ++e) v[it][e] = 0.f;
-            }
-          }
-        }
-        if ((p.prefetch & 4) && kz + 1 < nt + nst - 1) {  // just-in-time L2 prefetch of the NEXT tile's z window
-#pragma unroll
-          for (int it = 0; it < TC_ZITEMS; ++it) {
-            const int idx = gtid + it * TC_GTHREADS;
-            if (idx < n_zitems) {
-              const int ch = fast_div(idx, p.WIN, p.mg_win);
-              const SlotInfo sn = decode_slot(p, (t0 + kz + 1) * TC_TILE + (idx - ch * p.WIN), HW);
-              if (sn.valid) {
-                const float* zp = p.z + ((size_t)sn.n * p.C + ch * 8) * HW + sn.gp;
-#pragma unroll
-                for (int e = 0; e < 8; ++e) prefetch_l2(zp + (size_t)e * HW);
-              }
-            }
-          }
-        }
-        if (gwarp == 0 && lane == 0) TL(1 + grp, 30, kz);
-        if (kz >= 1) mbar_wait(&bars[BAR_ZEMPTY], (uint32_t)((kz - 1) & 1));  // M0(kz-1) has drained the window
-        if (gwarp == 0 && lane == 0) TL(1 + grp, 31, kz);
-#pragma unroll
-        for (int it = 0; it < TC_ZITEMS; ++it) {
-          if (dsto[it] >= 0) {
-            uint8_t* dst = smem + S0.sm_in + dsto[it];
-            split_store8(v[it], dst, dst + lo_off);
-          }
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars[BAR_ZFULL]);
-        if (gwarp == 0 && lane == 0) TL(1 + grp, 32, kz);
-      }
-
-      // ------------------------------ E_j(s - 2j) ---------------------------------------------
-      for (int j = 0; j < nst; ++j) {
-        const int k = s - 2 * j;
-        if (k < 0 || k >= nt + (nst - 1 - j) || (TC_NGROUPS == 2 && (k & 1) != grp)) continue;
-        const IafTcStage& St = p.st[j];
-        const bool last = (j == nst - 1);
-        if (gwarp == 0 && lane == 0) TL(1 + grp, 10 + j, k);
-        const int b = St.dbl ? (k & 1) : 0;
-        const int use = St.dbl ? (k >> 1) : k;
-        const int u = t0 + k;
-        const int sl = q * 32 + lane;
-        const SlotInfo si = decode_slot(p, u * TC_TILE + sl, HW);
-        const bool bx0 = (si.x == 0), bxW = (si.x == p.W - 1), byH = (si.y == p.H - 1);
-        const float* tb = reinterpret_cast<const float*>(smem + St.sm_bias);
-        const uint32_t t_acc = t_lane + (uint32_t)(St.tmem_col + b * St.acc_cols);
-        const int ngroups = St.N >> 4;
-
-        if (!last) {
-          const IafTcStage& Nx = p.st[j + 1];
-          const int plane = Nx.in_slots * 16;
-          const int lo_off = (St.N >> 3) * plane;
-          uint8_t* obase = smem + Nx.sm_in + ((k & 1) * TC_TILE + sl) * 16;
-          const bool mirror = ((k & 1) == 0) && (sl < p.MIR);
-          bool waited = false;
-          if ((p.prefetch & 4) && j == 0 && k + 1 < nt + (nst - 1)) {  // just-in-time L2 prefetch of the NEXT tile's context
-            const SlotInfo sn = decode_slot(p, (u + 1) * TC_TILE + sl, HW);
-            if (sn.valid) {
-              for (int g = cg; g < ngroups; g += CGS) {
-                const float* cp = p.ctx + ((size_t)sn.n * St.N + g * 16) * HW + sn.gp;
-#pragma unroll
-                for (int e = 0; e < 16; ++e) prefetch_l2(cp + (size_t)e * HW);
-              }
-            }
-          }
-#ifdef TC_HALO_TRIM
-          // halo tile: only hidden slots [0, MIR) are consumed (by the heads of the last real tile); warps whose 32 slots
-          // lie beyond take part in the barrier protocol only
-          const bool trimw = (nst == 2 && k == nt && q * 32 >= p.MIR);
-#else
-          constexpr bool trimw = false;
-#endif
-          for (int g = trimw ? ngroups : cg; g < ngroups; g += CGS) {
-            const int c0 = g * 16;
-            float cx[16];
-            if (j == 0 && si.valid) {  // += context   (ar.py:402 / layers.py:163)
-              const float* cp = p.ctx + ((size_t)si.n * St.N + c0) * HW + si.gp;
-#pragma unroll
-              for (int e = 0; e < 16; ++e) cx[e] = __ldg(cp + (size_t)e * HW);
-            } else {
-#pragma unroll
-              for (int e = 0; e < 16; ++e) cx[e] = 0.f;
-            }
-            if (!waited) {
-              mbar_wait(&bars[BAR_ACC_FULL + 2 * j + b], (uint32_t)(use & 1));
-              tc_fence_after();
-              // ring slot k&1 was last read by M_{j+1}(k-2)
-              if (gwarp == 0 && lane == 0) TL(1 + grp, 40 + j, k);
-              if (k >= 2) mbar_wait(&bars[BAR_H_EMPTY + 2 * j + (k & 1)], (uint32_t)(((k >> 1) - 1) & 1));
-              if (gwarp == 0 && lane == 0) TL(1 + grp, 50 + j, k);
-              waited = true;
-            }
-            uint32_t r[16];
-            tmem_ld16(t_acc + (uint32_t)c0, r);
-            tmem_ld_wait();
-#ifdef TC_FAST_EPI
-            float v[16];
-            if (NLT == IAF_NL_ELU && !PADW) {
-              // packed-pair arithmetic: accumulator halves, bias, context, elu(a) = max(a, exp(min(a,0)) - 1), validity
-              uint32_t r2[16];
-              if (St.merged) {
-                tmem_ld16(t_acc + (uint32_t)(St.N + c0), r2);
-                tmem_ld_wait();
-              }
-              const float4* tb4 = reinterpret_cast<const float4*>(tb + c0);
-              const float validf = si.valid ? 1.f : 0.f;
-#pragma unroll
-              for (int e4 = 0; e4 < 4; ++e4) {
-                const float4 t4 = tb4[e4];
-                const float bs[4] = {t4.x, t4.y, t4.z, t4.w};
-#pragma unroll
-                for (int h2 = 0; h2 < 2; ++h2) {
-                  const int e = 4 * e4 + 2 * h2;
-                  float a0 = __uint_as_float(r[e]), a1 = __uint_as_float(r[e + 1]);
-                  if (St.merged) add2(a0, a1, __uint_as_float(r2[e]), __uint_as_float(r2[e + 1]));
-                  add2(a0, a1, bs[2 * h2], bs[2 * h2 + 1]);
-                  add2(a0, a1, cx[e], cx[e + 1]);
-                  float t0 = fminf(a0, 0.f), t1 = fminf(a1, 0.f);
-                  mul2(t0, t1, 1.4426950408889634f, 1.4426950408889634f);
-                  t0 = ex2_approx(t0); t1 = ex2_approx(t1);
-                  add2(t0, t1, -1.0f, -1.0f);
-                  float o0 = fmaxf(a0, t0), o1 = fmaxf(a1, t1);  // exp(a) - 1 >= a for a < 0, and = 0 <= a otherwise
-                  mul2(o0, o1, validf, validf);
-                  v[e] = o0; v[e + 1] = o1;
-                }
-              }
-            } else {
-              if (St.merged) {
-                uint32_t r2[16];
-                tmem_ld16(t_acc + (uint32_t)(St.N + c0), r2);
-                tmem_ld_wait();
-#pragma unroll
-                for (int e = 0; e < 16; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) + __uint_as_float(r2[e]));
-              }
-              const float4* tb4 = reinterpret_cast<const float4*>(tb + c0);
-              float bsv[16];
-#pragma unroll
-              for (int e4 = 0; e4 < 4; ++e4) {
-                const float4 t4 = tb4[e4];
-                bsv[4 * e4] = t4.x; bsv[4 * e4 + 1] = t4.y; bsv[4 * e4 + 2] = t4.z; bsv[4 * e4 + 3] = t4.w;
-              }
-              if (PADW) {
-                const float f1 = bxW ? 1.f : 0.f, f2 = (byH || bx0) ? 1.f : 0.f, f3 = byH ? 1.f : 0.f,
-                            f4 = (byH || bxW) ? 1.f : 0.f;
-#pragma unroll
-                for (int e = 0; e < 16; ++e)
-                  bsv[e] += f1 * tb[St.N + c0 + e] + f2 * tb[2 * St.N + c0 + e] + f3 * tb[3 * St.N + c0 + e] +
-                            f4 * tb[4 * St.N + c0 + e];
-              }
-              const float validf = si.valid ? 1.f : 0.f;
-#pragma unroll
-              for (int e = 0; e < 16; ++e) {
-                const float a = __uint_as_float(r[e]) + bsv[e] + cx[e];
-                float o;
-                if (NLT == IAF_NL_ELU) {
-                  const float ex = fast_exp(fminf(a, 0.f)) - 1.0f;
-                  o = a < 0.f ? ex : a;
-                } else {
-                  o = tc_apply_nl<NLT>(a, p.nl);
-                }
-                v[e] = o * validf;
-              }
-            }
-#else
-            if (St.merged) {  // hi*lo partial products sit in columns [N, 2N)
-              uint32_t r2[16];
-              tmem_ld16(t_acc + (uint32_t)(St.N + c0), r2);
-              tmem_ld_wait();
-#pragma unroll
-              for (int e = 0; e < 16; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) + __uint_as_float(r2[e]));
-            }
-            float v[16];
-            {
-              // branch-free: bias rows come in as 16-byte vectors, the pad-channel terms (conv.py:77-83: the pad
-              // channel is 1 where a tap falls outside the image) are 0/1-weighted FMAs, and an invalid slot
-              // (pad column, zero row, past the end) is multiplied to zero: that zero IS the conv's padding
-              const float4* tb4 = reinterpret_cast<const float4*>(tb + c0);
-              float bsv[16];
-#pragma unroll
-              for (int e4 = 0; e4 < 4; ++e4) {
-                const float4 t4 = tb4[e4];
-                bsv[4 * e4] = t4.x; bsv[4 * e4 + 1] = t4.y; bsv[4 * e4 + 2] = t4.z; bsv[4 * e4 + 3] = t4.w;
-              }
-              if (PADW) {
-                const float f1 = bxW ? 1.f : 0.f, f2 = (byH || bx0) ? 1.f : 0.f, f3 = byH ? 1.f : 0.f,
-                            f4 = (byH || bxW) ? 1.f : 0.f;
-#pragma unroll
-                for (int e = 0; e < 16; ++e)
-                  bsv[e] += f1 * tb[St.N + c0 + e] + f2 * tb[2 * St.N + c0 + e] + f3 * tb[3 * St.N + c0 + e] +
-                            f4 * tb[4 * St.N + c0 + e];
-              }
-              const float validf = si.valid ? 1.f : 0.f;
-#pragma unroll
-              for (int e = 0; e < 16; ++e) {
-                const float a = __uint_as_float(r[e]) + bsv[e] + cx[e];
-                float o;
-                if (NLT == IAF_NL_ELU) {
-                  const float ex = fast_exp(fminf(a, 0.f)) - 1.0f;  // elu, exp always evaluated: no divergence
-                  o = a < 0.f ? ex : a;
-                } else {
-                  o = tc_apply_nl<NLT>(a, p.nl);
-                }
-                v[e] = o * validf;
-              }
-            }
-#endif
-            if (St.hid_out && si.valid) {  // training forward: keep the activations for iaf_step_bwd_saved
-              float* hp = St.hid_out + ((size_t)si.n * St.N + c0) * HW + si.gp;
-#pragma unroll
-              for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] = v[e];
-            }
-#pragma unroll
-            for (int hch = 0; hch < 2; ++hch) {
-              uint8_t* dst = obase + ((c0 >> 3) + hch) * plane;
-              split_store8(v + 8 * hch, dst, dst + lo_off);
-              if (mirror) split_store8(v + 8 * hch, dst + 2 * TC_TILE * 16, dst + 2 * TC_TILE * 16 + lo_off);
-            }
-          }
-          if (!waited) {  // a warp with no column group still takes part in the hand-off
-            mbar_wait(&bars[BAR_ACC_FULL + 2 * j + b], (uint32_t)(use & 1));
-          }
-          tc_fence_before();
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(&bars[BAR_ACC_EMPTY + 2 * j + b]);
-            mbar_arrive(&bars[BAR_H_FULL + 2 * j + (k & 1)]);
-          }
-          if (gwarp == 0 && lane == 0) TL(1 + grp, 20 + j, k);
-        } else {
-          // ---------------- heads: columns in groups of 16 = (m x 8, s x 8) of 8 channels --------------
-          constexpr int NRED = (MODE == IAF_MODE_LAYER) ? 8 : 1;
-          float red[NRED];
-#pragma unroll
-          for (int i = 0; i < NRED; ++i) red[i] = 0.f;
-          const int tile_s0 = u * TC_TILE;
-          const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
-          const int n_last = min(p.B - 1, fast_div(tile_s0 + TC_TILE - 1, p.SPS, p.mg_sps));
-          const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
-          const int pb = k & 1;  // partial-sum buffer
-          if (MODE == IAF_MODE_LAYER && (p.persample_out || p.bc_out) && k >= 2)
-            mbar_wait(&bars[BAR_PART_EMPTY + pb], (uint32_t)(((k >> 1) - 1) & 1));
-          bool waited = false;
-          for (int g = cg; g < ngroups; g += CGS) {
-            const int c0 = g * 16;
-            const int ch0 = g * 8;
-            float zv[8];
-            size_t gi = 0;
-            if (si.valid) {
-              gi = ((size_t)si.n * p.C + ch0) * HW + si.gp;
-#pragma unroll
-              for (int e = 0; e < 8; ++e) zv[e] = __ldg(p.z + gi + (size_t)e * HW);
-            }
-            if (!waited) {
-              mbar_wait(&bars[BAR_ACC_FULL + 2 * j + b], (uint32_t)(use & 1));
-              tc_fence_after();
-              waited = true;
-              if (gwarp == 0 && lane == 0) TL(1 + grp, 50 + j, k);
-            }
-            uint32_t r[16];
-            tmem_ld16(t_acc + (uint32_t)c0, r);
-            tmem_ld_wait();
-            if (St.merged) {
-              uint32_t r2[16];
-              tmem_ld16(t_acc + (uint32_t)(St.N + c0), r2);
-              tmem_ld_wait();
-#ifdef TC_FAST_EPI
-#pragma unroll
-              for (int e = 0; e < 16; e += 2) {
-                float a0 = __uint_as_float(r[e]), a1 = __uint_as_float(r[e + 1]);
-                add2(a0, a1, __uint_as_float(r2[e]), __uint_as_float(r2[e + 1]));
-                r[e] = __float_as_uint(a0); r[e + 1] = __float_as_uint(a1);
-              }
-#else
-#pragma unroll
-              for (int e = 0; e < 16; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) + __uint_as_float(r2[e]));
-#endif
-            }
-            if (MODE == IAF_MODE_LAYER) {
-#pragma unroll
-              for (int i = 0; i < NRED; ++i) red[i] = 0.f;
-            }
-#ifdef TC_FAST_EPI
-            if (MODE == IAF_MODE_STEP && !PADW) {
-              // packed-pair form of the step epilogue (same arithmetic; the per-thread sum is accumulated as two lanes)
-              if (si.valid) {
-                const float4* tb4 = reinterpret_cast<const float4*>(tb + c0);
-                const float4 bm0 = tb4[0], bm1 = tb4[1], bs0 = tb4[2], bs1 = tb4[3];
-                const float bm[8] = {bm0.x, bm0.y, bm0.z, bm0.w, bm1.x, bm1.y, bm1.z, bm1.w};
-                const float bs[8] = {bs0.x, bs0.y, bs0.z, bs0.w, bs1.x, bs1.y, bs1.z, bs1.w};
-                float rp0 = 0.f, rp1 = 0.f;
-#pragma unroll
-                for (int e = 0; e < 8; e += 2) {
-                  float m0 = __uint_as_float(r[e]), m1 = __uint_as_float(r[e + 1]);
-                  float s0 = __uint_as_float(r[8 + e]), s1 = __uint_as_float(r[9 + e]);
-                  add2(m0, m1, bm[e], bm[e + 1]);
-                  add2(s0, s1, bs[e], bs[e + 1]);
-                  mul2(m0, m1, p.scale, p.scale);   // arw_mean
-                  mul2(s0, s1, p.scale, p.scale);   // arw_logsd          (models.py:282-285)
-                  float d0 = zv[e], d1 = zv[e + 1];
-                  sub2(d0, d1, m0, m1);
-                  float t0 = s0, t1 = s1;
-                  mul2(t0, t1, -1.4426950408889634f, -1.4426950408889634f);
-                  t0 = ex2_approx(t0); t1 = ex2_approx(t1);
-                  mul2(d0, d1, t0, t1);             // z' = (z - arw_mean) * exp(-arw_logsd)
-                  const size_t ge = gi + (size_t)e * HW;
-                  p.z_out[ge] = d0;
-                  p.z_out[ge + HW] = d1;
-                  if (p.elem) { p.elem[ge] = s0; p.elem[ge + HW] = s1; }
-                  add2(rp0, rp1, s0, s1);
-                }
-                red[0] += rp0 + rp1;
-              }
-            } else
-#endif
-            if (si.valid) {
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                float m = __uint_as_float(r[e]) + tb[c0 + e];
-                float sv = __uint_as_float(r[8 + e]) + tb[c0 + 8 + e];
-                if (PADW) {
-                  if (bxW) { m += tb[St.N + c0 + e]; sv += tb[St.N + c0 + 8 + e]; }
-                  if (byH || bx0) { m += tb[2 * St.N + c0 + e]; sv += tb[2 * St.N + c0 + 8 + e]; }
-                  if (byH) { m += tb[3 * St.N + c0 + e]; sv += tb[3 * St.N + c0 + 8 + e]; }
-                  if (byH || bxW) { m += tb[4 * St.N + c0 + e]; sv += tb[4 * St.N + c0 + 8 + e]; }
-                }
-                if (MODE == IAF_MODE_MULTICONV) {  // the un-fused operator: raw heads (ar.py:405-411 / layers.py:166)
-                  p.z_out[gi + (size_t)e * HW] = m;
-                  p.elem[gi + (size_t)e * HW] = sv;
-                  continue;
-                }
-                const float arw_mean = p.scale * m, arw_logsd = p.scale * sv;  // models.py:282-285
-                const size_t ge = gi + (size_t)e * HW;
-                float z0 = zv[e];
-                float eps = 0.f, pls = 0.f;
-                if (MODE == IAF_MODE_LAYER) {
-                  eps = z0;
-                  pls = __ldg(p.post_logsd + ge);
-                  z0 = fmaf(fast_exp(pls), eps, __ldg(p.post_mean + ge));
-                }
-                const float zn = (z0 - arw_mean) * fast_exp(-arw_logsd);
-                p.z_out[ge] = zn;
-                if (MODE == IAF_MODE_STEP) {
-                  if (p.elem) p.elem[ge] = arw_logsd;
-                  red[0] += arw_logsd;
-                } else {
-                  // logqs of the pre-flow sample + arw_logsd, prior logps at z'  (tf_train.py:68-75)
-                  const float logqs = -0.9189385332046727f - pls - 0.5f * eps * eps + arw_logsd;
-                  const float pl = __ldg(p.prior_logsd + ge);
-                  const float d = zn - __ldg(p.prior_mean + ge);
-                  const float logps = -0.9189385332046727f - pl - 0.5f * d * d * fast_exp(-2.0f * pl);
-                  const float kl = logqs - logps;
-                  if (p.elem) p.elem[ge] = kl;
-                  red[e] = kl;
-                }
-              }
-            }
-            if (MODE == IAF_MODE_LAYER) {
-              // per-(sample, channel) sums over this warp's 32 slots, fixed butterfly order
-              for (int nl_ = 0; nl_ < ns; ++nl_) {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                  float x = (si.valid && si.n == n_first + nl_) ? red[e] : 0.f;
-#pragma unroll
-                  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-                  if (lane == 0) s_part[((pb * 4 + q) * p.MAXS + nl_) * p.C + ch0 + e] = x;
-                }
-              }
-            }
-          }
-          if (!waited) mbar_wait(&bars[BAR_ACC_FULL + 2 * j + b], (uint32_t)(use & 1));
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bars[BAR_ACC_EMPTY + 2 * j + b]);
-          if (gwarp == 0 && lane == 0) TL(1 + grp, 20 + j, k);
-
-          // ---------------- deterministic per-sample reductions ----------------
-          // every worker warp deposits fixed-order partial sums for this tile in smem (double-buffered by
-          // tile parity), arrives on an mbarrier and moves on; worker warp 0 alone folds them into the
-          // per-tile partials in global memory and, for samples whose last tile this is, into the outputs.
-          if (p.persample_out || p.bc_out) {
-            constexpr bool LAY = (MODE == IAF_MODE_LAYER);
-            if (!LAY) {
-              if (k >= 2) mbar_wait(&bars[BAR_PART_EMPTY + pb], (uint32_t)(((k >> 1) - 1) & 1));
-              for (int nl_ = 0; nl_ < ns; ++nl_) {
-                float x = (si.valid && si.n == n_first + nl_) ? red[0] : 0.f;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-                if (lane == 0) s_part[(pb * TC_GWARPS + gwarp) * p.MAXS + nl_] = x;
-              }
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bars[BAR_PART + pb]);
-          }
-        }
-      }
-    }
-  }
-
-  if (warp == TC_RED_WARP && (p.persample_out || p.bc_out) && MODE != IAF_MODE_MULTICONV) {
-    // =====================================================================================
-    // reducer warp: folds the workers' per-tile partial sums into the per-tile partials in global memory and, for
-    // samples whose last tile this is, into the outputs -- off the workers' critical path
-    // =====================================================================================
-    float* s_part = reinterpret_cast<float*>(smem + p.sm_part);
-    constexpr bool LAY = (MODE == IAF_MODE_LAYER);
-    for (int k = 0; k < nt; ++k) {
-      const int u = t0 + k;
-      const int pb = k & 1;
-      const int tile_s0 = u * TC_TILE;
-      const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
-      const int n_last = min(p.B - 1, fast_div(tile_s0 + TC_TILE - 1, p.SPS, p.mg_sps));
-      const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
-      {
-              mbar_wait(&bars[BAR_PART + pb], (uint32_t)((k >> 1) & 1));
-              const int cred = LAY ? p.C : 1;
-              for (int i = lane; i < ns * cred; i += 32) {
-                float tot = 0.f;
-                if (LAY) {
-                  const int nl_ = i / p.C, c = i - nl_ * p.C;
-                  for (int qq = 0; qq < 4; ++qq) tot += s_part[((pb * 4 + qq) * p.MAXS + nl_) * p.C + c];
-                } else {
-                  for (int w = 0; w < TC_GWARPS; ++w) tot += s_part[(pb * TC_GWARPS + w) * p.MAXS + i];
-                }
-                p.tilepart[((size_t)u * p.MAXS) * cred + i] = tot;
-                __threadfence();
-              }
-              __syncwarp();
-              for (int i = lane; i < ns; i += 32) {
-                const int n = n_first + i;
-                const int a = n * p.SPS, bb = a + p.SPS - 1;
-                const int ta = a / TC_TILE, tbk = bb / TC_TILE;
-                const unsigned expected = (unsigned)(tbk - ta + 1);
-                __threadfence();
-                if (atomicAdd(p.counter + n, 1u) == expected - 1u) {
-                  __threadfence();
-                  p.counter[n] = 0u;  // ready for the next launch
-                  float cost = 0.f;
-                  for (int c = 0; c < cred; ++c) {
-                    float tot = 0.f;
-                    for (int tt = ta; tt <= tbk; ++tt) {
-                      const int nf = fast_div(tt * TC_TILE, p.SPS, p.mg_sps);
-                      tot += __ldcg(p.tilepart + ((size_t)tt * p.MAXS + (n - nf)) * cred + c);
-                    }
-                    if (LAY && p.bc_out) p.bc_out[(size_t)n * p.C + c] = tot;
-                    cost += tot;
-                  }
-                  if (p.persample_out) p.persample_out[n] = LAY ? cost : -cost;  // logdet = -sum(arw_logsd)
-                }
-              }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[BAR_PART_EMPTY + pb]);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  TL_FLUSH
-  if (warp == TC_CTRL_WARP) tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-}
-
 #include "iaf_tc_gemm.cuh"
 #include "iaf_wg.cuh"
-#include "iaf_fz.cuh"
 
 // ------------------------------------------------------------------------------------------
-// weight preparation for this path: same math as iaf_pack.cu, bf16 hi/lo split, written as
-// the UMMA B-operand image [K/8][N][8] (K index = tap*Cin + ci, K-major, no swizzle).
+// weight preparation for this path: same math as iaf_pack.cu, fp16 hi/lo split, written as
+// the wgmma B-operand image [K/8][N][8] (K index [ci / 16][tap][ci % 16], K-major, no swizzle).
 // ------------------------------------------------------------------------------------------
 struct TcPackLayer {
   const float* w; const float* scale; const float* bias;
   __nv_bfloat16* whi; __nv_bfloat16* wlo; float* bias_out; float* padw_out;
-  int cin, cout, N, zerodiag, head, is_head, merged;
+  int cin, cout, N, zerodiag, head, is_head;
 };
 struct TcPackParams {
   TcPackLayer layer[IAF_MAX_HIDDEN + IAF_MAX_HEADS];
-  int n_layers, variant, korder;
+  int n_layers, variant;
 };
 
 __device__ __forceinline__ bool tc_centre_visible(int ci, int co, int cin, int cout, int zd) {
@@ -1117,23 +293,17 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
       float v = tc_raw_weight(L, p.variant, t, ci, co);
       if (t == 0 && !tc_centre_visible(ci, co, L.cin, L.cout, L.zerodiag)) v = 0.f;
       v *= factor;
-      // K order: fused kernel [tap][ci]; layer-at-a-time kernel [ci / 16][tap][ci % 16]
-      const int k = p.korder ? (((ci >> 4) * IAF_NTAPS + t) * 16 + (ci & 15)) : (t * L.cin + ci);
+      // K order [ci / 16][tap][ci % 16]: one K-step of the stage kernel is one 16-channel block over the five taps
+      const int k = ((ci >> 4) * IAF_NTAPS + t) * 16 + (ci & 15);
       // fp16 hi + fp16 lo (22 significant bits); saturated at the fp16 range (a gain of e^11 is not a weight-norm layer)
       const float vc = fminf(fmaxf(v, -65000.f), 65000.f);
       const __half hh = __float2half_rn(vc);
       const __half lh = __float2half_rn(vc - __half2float(hh));
       const __nv_bfloat16 h = __ushort_as_bfloat16(__half_as_ushort(hh));  // raw 16-bit patterns travel in the bf16-typed images
       const __nv_bfloat16 l = __ushort_as_bfloat16(__half_as_ushort(lh));
-      if (p.korder && !L.merged) {  // layered kernel: separate hi / lo images [K/8][N][8] (merged heads: the interleaved one)
-        const size_t o = ((size_t)(k >> 3) * L.N + col) * 8 + (k & 7);
-        L.whi[o] = h;
-        L.wlo[o] = l;
-      } else {         // fused kernel: one image [K/8][2N][8], per K chunk the N hi rows then the N lo rows
-        const size_t o = ((size_t)(k >> 3) * 2 * L.N + col) * 8 + (k & 7);
-        L.whi[o] = h;
-        L.whi[o + (size_t)L.N * 8] = l;
-      }
+      const size_t o = ((size_t)(k >> 3) * L.N + col) * 8 + (k & 7);  // hi / lo images [K/8][N][8]
+      L.whi[o] = h;
+      L.wlo[o] = l;
     } else {
       const int t = e - n_real + 1;
       L.padw_out[(size_t)(t - 1) * L.N + col] = tc_raw_weight(L, p.variant, t, L.cin, co) * factor;
@@ -1153,285 +323,56 @@ struct IafTcPlan {
   __nv_bfloat16* wlo[IAF_MAX_STAGES];
   float* bias[IAF_MAX_STAGES];
   float* padw[IAF_MAX_STAGES];
-  int sm_whi[IAF_MAX_STAGES], sm_wlo[IAF_MAX_STAGES], sm_in[IAF_MAX_STAGES], in_slots[IAF_MAX_STAGES];
-  int sm_bias[IAF_MAX_STAGES], tmem_col[IAF_MAX_STAGES], dbl[IAF_MAX_STAGES], merged[IAF_MAX_STAGES], acc_cols[IAF_MAX_STAGES];
-  int MIR, WIN, RING, MAXS, sm_part, tmem_cols;
+  int MIR, WIN, MAXS;
   bool layer_ok;             // the per-(sample,channel) scratch of the fused-layer mode fits
-  // second-generation fused kernel (iaf_fz_kernel: exactly one hidden layer)
-  bool fz;
-  int TO, h_bytes, z_bytes;
-  // the kernel has two shared-memory layouts: [0] z gathered by the loader warps (two operand windows when they fit),
-  // [1] z staged by bulk copies (one operand window + an fp32 staging buffer; 16x16 planes, step / multiconv modes)
-  struct FzLay { bool ok, layer_ok; int nzw, nhb, nzs, zst_bytes, sm_zst, sm_in1, sm_bias[2], sm_part; size_t smem; } fzl[2];
-  // TMA descriptors of recently seen z tensors (the descriptor depends on the pointer and the batch size only; encoding
-  // one is a driver call, so steady-state callers that cycle through a few buffers pay for it once per buffer)
-  struct TmSlot { const float* z; int B; unsigned char tm[IAF_FZ_MAXROWS][128]; } tm_cache[16];
-  // layer-at-a-time mode (hidden widths that do not fit the fused kernel's on-chip rings)
-  bool layered;
+  // one launch per stage: an A window (first stage), an NB-deep ring, the bias table, the partials, the accumulator tile
   int ly_stage[IAF_MAX_STAGES];
   int ly_NB[IAF_MAX_STAGES], ly_sm_a[IAF_MAX_STAGES], ly_sm_b[IAF_MAX_STAGES], ly_sm_bias[IAF_MAX_STAGES],
-      ly_sm_part[IAF_MAX_STAGES], ly_tmem[IAF_MAX_STAGES], ly_merged[IAF_MAX_STAGES];
+      ly_sm_part[IAF_MAX_STAGES], ly_sm_acc[IAF_MAX_STAGES];
   size_t ly_smem[IAF_MAX_STAGES];
+  // one-launch step (one hidden layer): resident weights of both stages, hidden activations in shared memory
+  bool fused;
+  int fz_sm_a, fz_sm_h, fz_sm_bias[2], fz_sm_part, fz_sm_acc, fz_sm_b[2];
+  size_t fz_smem;
   __nv_bfloat16* img[2][2];  // ping-pong operand images: [which][hi|lo]
   int img_S_pad;
-  size_t smem;
   unsigned* counter;
   float* tilepart;
-  int scratch_B;
+  int scratch_B, scratch_NT;
   int num_sms;
 };
 
-typedef void (*TcKernel)(const IafTcParams);
-template <int THW>
-static TcKernel tc_kernel_pick(bool padw, int mode, bool elu) {
-  if (mode == IAF_MODE_MULTICONV) {
-    if (padw) return elu ? iaf_tc_kernel<true, IAF_MODE_MULTICONV, IAF_NL_ELU, THW> : iaf_tc_kernel<true, IAF_MODE_MULTICONV, -1, THW>;
-    return elu ? iaf_tc_kernel<false, IAF_MODE_MULTICONV, IAF_NL_ELU, THW> : iaf_tc_kernel<false, IAF_MODE_MULTICONV, -1, THW>;
-  }
-  if (mode == IAF_MODE_STEP) {
-    if (padw) return elu ? iaf_tc_kernel<true, IAF_MODE_STEP, IAF_NL_ELU, THW> : iaf_tc_kernel<true, IAF_MODE_STEP, -1, THW>;
-    return elu ? iaf_tc_kernel<false, IAF_MODE_STEP, IAF_NL_ELU, THW> : iaf_tc_kernel<false, IAF_MODE_STEP, -1, THW>;
-  }
-  if (padw) return elu ? iaf_tc_kernel<true, IAF_MODE_LAYER, IAF_NL_ELU, THW> : iaf_tc_kernel<true, IAF_MODE_LAYER, -1, THW>;
-  return elu ? iaf_tc_kernel<false, IAF_MODE_LAYER, IAF_NL_ELU, THW> : iaf_tc_kernel<false, IAF_MODE_LAYER, -1, THW>;
-}
-// 16x16 planes (every BASELINE config's first level) get compile-time channel strides
-static TcKernel tc_kernel_for(bool padw, int mode, bool elu, int hw) {
-  return hw == 256 ? tc_kernel_pick<256>(padw, mode, elu) : tc_kernel_pick<0>(padw, mode, elu);
-}
-
 typedef void (*LyKernel)(const IafLyParams);
-template <int THW>
+template <int NGW, bool FUSED>
 static LyKernel ly_kernel_pick(bool padw, int mode, bool elu) {
-  if (mode == IAF_MODE_MULTICONV) {
-    if (padw) return elu ? iaf_ly_kernel<true, IAF_MODE_MULTICONV, IAF_NL_ELU, THW> : iaf_ly_kernel<true, IAF_MODE_MULTICONV, -1, THW>;
-    return elu ? iaf_ly_kernel<false, IAF_MODE_MULTICONV, IAF_NL_ELU, THW> : iaf_ly_kernel<false, IAF_MODE_MULTICONV, -1, THW>;
+#define LY_PICK(MD)                                                                                                   \
+  if (padw) return elu ? iaf_ly_kernel<true, MD, IAF_NL_ELU, NGW, FUSED> : iaf_ly_kernel<true, MD, -1, NGW, FUSED>; \
+  return elu ? iaf_ly_kernel<false, MD, IAF_NL_ELU, NGW, FUSED> : iaf_ly_kernel<false, MD, -1, NGW, FUSED>;
+  if (mode == IAF_MODE_MULTICONV) { LY_PICK(IAF_MODE_MULTICONV) }
+  if (mode == IAF_MODE_STEP) { LY_PICK(IAF_MODE_STEP) }
+  LY_PICK(IAF_MODE_LAYER)
+#undef LY_PICK
+}
+// the stage kernel for a stage of N output columns: NGW = ceil(N / 32) 16-column groups per warpgroup
+static LyKernel ly_kernel_for(bool padw, int mode, bool elu, int N) {
+  switch ((N + 31) / 32) {
+    case 1: return ly_kernel_pick<1, false>(padw, mode, elu);
+    case 2: return ly_kernel_pick<2, false>(padw, mode, elu);
+    case 3: return ly_kernel_pick<3, false>(padw, mode, elu);
+    case 4: return ly_kernel_pick<4, false>(padw, mode, elu);
+    case 5: return ly_kernel_pick<5, false>(padw, mode, elu);
+    case 6: return ly_kernel_pick<6, false>(padw, mode, elu);
+    case 7: return ly_kernel_pick<7, false>(padw, mode, elu);
+    default: return ly_kernel_pick<8, false>(padw, mode, elu);
   }
-  if (mode == IAF_MODE_STEP) {
-    if (padw) return elu ? iaf_ly_kernel<true, IAF_MODE_STEP, IAF_NL_ELU, THW> : iaf_ly_kernel<true, IAF_MODE_STEP, -1, THW>;
-    return elu ? iaf_ly_kernel<false, IAF_MODE_STEP, IAF_NL_ELU, THW> : iaf_ly_kernel<false, IAF_MODE_STEP, -1, THW>;
-  }
-  if (padw) return elu ? iaf_ly_kernel<true, IAF_MODE_LAYER, IAF_NL_ELU, THW> : iaf_ly_kernel<true, IAF_MODE_LAYER, -1, THW>;
-  return elu ? iaf_ly_kernel<false, IAF_MODE_LAYER, IAF_NL_ELU, THW> : iaf_ly_kernel<false, IAF_MODE_LAYER, -1, THW>;
 }
-static LyKernel ly_kernel_for(bool padw, int mode, bool elu, int hw) {
-  return hw == 256 ? ly_kernel_pick<256>(padw, mode, elu) : ly_kernel_pick<0>(padw, mode, elu);
-}
-
-// cuTensorMapEncodeTiled through the runtime's driver entry-point lookup
-typedef CUresult (*TmapEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static TmapEncodeFn tmap_encoder() {
-  static TmapEncodeFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<TmapEncodeFn>(ptr);
-    else
-      cudaGetLastError();
-  }
-  return fn;
-}
-// z [B][C][H][W] fp32 as (x, y, c, n); box = (W, rows, C, 1): `rows` image rows of every channel of one sample, which
-// land in shared memory as [channel][row][x] (per channel rows * W * 4 contiguous bytes on both sides)
-static bool encode_z_tmap(unsigned char* out128, const float* z, int B, int C, int H, int W, int rows) {
-  TmapEncodeFn enc = tmap_encoder();
-  if (!enc) return false;
-  CUtensorMap tm;
-  const cuuint64_t dims[4] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)C, (cuuint64_t)B};
-  const cuuint64_t strides[3] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4, (cuuint64_t)C * H * W * 4};
-  const cuuint32_t box[4] = {(cuuint32_t)W, (cuuint32_t)rows, (cuuint32_t)C, 1u};
-  const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-  if (enc(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(z), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-    return false;
-  static_assert(sizeof(CUtensorMap) == 128, "CUtensorMap is 128 bytes");
-  memcpy(out128, &tm, 128);
-  return true;
-}
-
-template <int THW>
-static TcKernel fz_kernel_pick(bool padw, int mode, bool elu) {
-  if (mode == IAF_MODE_MULTICONV) {
-    if (padw) return elu ? iaf_fz_kernel<true, IAF_MODE_MULTICONV, IAF_NL_ELU, THW> : iaf_fz_kernel<true, IAF_MODE_MULTICONV, -1, THW>;
-    return elu ? iaf_fz_kernel<false, IAF_MODE_MULTICONV, IAF_NL_ELU, THW> : iaf_fz_kernel<false, IAF_MODE_MULTICONV, -1, THW>;
-  }
-  if (mode == IAF_MODE_STEP) {
-    if (padw) return elu ? iaf_fz_kernel<true, IAF_MODE_STEP, IAF_NL_ELU, THW> : iaf_fz_kernel<true, IAF_MODE_STEP, -1, THW>;
-    return elu ? iaf_fz_kernel<false, IAF_MODE_STEP, IAF_NL_ELU, THW> : iaf_fz_kernel<false, IAF_MODE_STEP, -1, THW>;
-  }
-  if (padw) return elu ? iaf_fz_kernel<true, IAF_MODE_LAYER, IAF_NL_ELU, THW> : iaf_fz_kernel<true, IAF_MODE_LAYER, -1, THW>;
-  return elu ? iaf_fz_kernel<false, IAF_MODE_LAYER, IAF_NL_ELU, THW> : iaf_fz_kernel<false, IAF_MODE_LAYER, -1, THW>;
-}
-// the compile-time-plane instantiation (THW = 256) is used for 16x16 planes only: it is also the one whose step /
-// multiconv modes stage z with bulk copies
-static TcKernel fz_kernel_for(bool padw, int mode, bool elu, bool plane256) {
-  return plane256 ? fz_kernel_pick<256>(padw, mode, elu) : fz_kernel_pick<0>(padw, mode, elu);
-}
+// the one-launch step of a one-hidden-layer stack (hidden and 2 n_z at most 64 columns: two groups per warpgroup)
+#define FZ_NGW 2
+static LyKernel fz_kernel_for(bool padw, int mode, bool elu) { return ly_kernel_pick<FZ_NGW, true>(padw, mode, elu); }
 
 static int tc_round_up(int a, int b) { return (a + b - 1) / b * b; }
 
-// iaf_fz_kernel: one hidden layer; weights resident, one z window, two hidden-activation buffers, both accumulators
-// double-buffered in TMEM
-static bool fz_layout(const iaf_desc_t* d, IafTcPlan* pl) {
-  if (d->n_hidden != 1 || d->n_heads != 2 || d->head[0] != d->n_z || d->head[1] != d->n_z) return false;
-  if (d->n_z % 16 != 0 || 2 * d->n_z > 256) return false;
-  if (d->hidden[0] % 16 != 0 || d->hidden[0] > 256) return false;
-  const int Wp = d->W + 1;
-  const int SPS = (d->H + 1) * Wp;
-  const int MIR = Wp + 1;  // largest tap shift
-  const int TO = TC_TILE - MIR;
-  if (TO < TC_TILE / 2) return false;
-  IafTcPlan tmp;
-  IafTcPlan* q = pl ? pl : &tmp;
-  q->n_stages = 2;
-  q->MIR = MIR; q->WIN = TC_TILE + MIR; q->RING = 0; q->TO = TO;
-  q->MAXS = (TO - 1) / SPS + 2;
-  int off = 0, prev = d->n_z;
-  for (int j = 0; j < 2; ++j) {
-    q->cin[j] = prev;
-    q->N[j] = (j == 0) ? d->hidden[0] : 2 * d->n_z;
-    q->K[j] = IAF_NTAPS * prev;
-    const int wb = q->K[j] * q->N[j] * 2;
-    q->sm_whi[j] = off; off += wb;
-    q->sm_wlo[j] = off; off += wb;
-    prev = q->N[j];
-  }
-  q->in_slots[0] = q->WIN;
-  q->sm_in[0] = off;
-  q->z_bytes = tc_round_up(2 * (q->cin[0] / 8) * q->WIN * 16, 128);
-  if ((q->cin[0] / 8) * q->WIN > FZ_ZB * FZ_LTHREADS || q->N[0] > 16 * FZ_CXG * FZ_LGS) return false;
-  q->in_slots[1] = TC_TILE;
-  q->h_bytes = 2 * (q->cin[1] / 8) * TC_TILE * 16;
-  if (q->MAXS > 32) return false;  // the reducer warp keeps one per-sample value per lane (8 in layer mode)
-  const int part_step = 2 * FZ_EPI * q->MAXS * 4;
-  const int part_layer = 2 * 4 * q->MAXS * d->n_z * 4;
-  const int zoff = off;
-  bool any = false;
-  for (int v = 0; v < 2; ++v) {
-    IafTcPlan::FzLay& L = q->fzl[v];
-    L.ok = false;
-    // staged: 16x16 planes only (the kernel's compile-time-plane instantiation is the staged one)
-    if (v == 1 && !(d->H == 16 && d->W == 16 && d->n_z <= 32 && tmap_encoder())) continue;
-    // gathered: two z windows when they fit (else one), two h buffers.  Staged: one z window, one staging buffer, two h
-    // buffers.  (IAF_FZ_TWO_STAGE=1 selects two staging buffers paid for with ONE h buffer -- measured on the B200: 26.2 us
-    // against 25.2 us; the loader warps wait just as long for the copies, so a tile's copy TIME, not how early it is
-    // issued, is what they wait for: ten boxes of 32 x 64-byte segments each, see profiles/r2_fz_probe_staging.log.)
-    const int rows = (q->WIN + Wp - 2) / Wp + 1;  // stream rows a window can touch
-    if (v == 1 && rows > IAF_FZ_MAXROWS) continue;
-    const int zst_bytes = tc_round_up(d->n_z * rows * d->W * 4, 128);
-    const char* e2 = getenv("IAF_FZ_TWO_STAGE");
-    const bool two_stage = v == 1 && e2 && e2[0] == '1';
-    for (int t = 0; t < 2 && !L.ok; ++t) {
-      const int nzw = (v == 1) ? 1 : 2 - t;
-      const int nzs = (v == 1) ? (two_stage && t == 0 ? 2 : 1) : 0;
-      const int nhb = (two_stage && t == 0) ? 1 : 2;
-      int o = zoff + nzw * q->z_bytes;
-      L.nzw = nzw; L.nhb = nhb; L.nzs = nzs; L.zst_bytes = zst_bytes;
-      L.sm_zst = o;
-      o += nzs * zst_bytes;
-      L.sm_in1 = o;
-      o += nhb * q->h_bytes;
-      o += tc_round_up(MIR * 16, 128);  // a shifted 128-row window of the last plane reads MIR rows past the buffer
-      for (int j = 0; j < 2; ++j) { L.sm_bias[j] = o; o += 5 * q->N[j] * 4; }
-      o = tc_round_up(o, 16);
-      L.sm_part = o;
-      L.layer_ok = v == 0 && (o + std::max(part_step, part_layer)) <= TC_SMEM_LIMIT && q->MAXS * d->n_z <= 256;
-      o += L.layer_ok ? std::max(part_step, part_layer) : part_step;
-      L.smem = (size_t)o;
-      L.ok = o <= TC_SMEM_LIMIT;
-    }
-    any = any || L.ok;
-  }
-  if (!q->fzl[0].ok) return false;  // the gathered variant serves every mode; the staged one is an extra
-  q->layer_ok = q->fzl[0].layer_ok;
-  q->smem = std::max(q->fzl[0].smem, q->fzl[1].ok ? q->fzl[1].smem : (size_t)0);
-  // TMEM: both accumulators double-buffered; what is left goes to the merged hi*[hi|lo] form, the heads first
-  int cols = 2 * (q->N[0] + q->N[1]);
-  if (cols > 512) return false;
-  const char* mg = getenv("IAF_TC_MERGED");
-  for (int j = 0; j < 2; ++j) { q->dbl[j] = 1; q->merged[j] = 0; q->acc_cols[j] = q->N[j]; }
-  for (int j = 1; j >= 0 && !(mg && mg[0] == '0'); --j) {
-    if (2 * q->N[j] <= 256 && cols + 2 * q->N[j] <= 512) { q->merged[j] = 1; q->acc_cols[j] = 2 * q->N[j]; cols += 2 * q->N[j]; }
-  }
-  int col = 0;
-  for (int j = 0; j < 2; ++j) { q->tmem_col[j] = col; col += 2 * q->acc_cols[j]; }
-  int tc = 32;
-  while (tc < col) tc *= 2;
-  q->tmem_cols = tc;
-  return true;
-}
-
-static bool tc_layout(const iaf_desc_t* d, IafTcPlan* pl) {
-  if (d->n_hidden < 1 || d->n_heads != 2 || d->head[0] != d->n_z || d->head[1] != d->n_z) return false;
-  if (d->n_z % 16 != 0 || 2 * d->n_z > 256) return false;
-  for (int i = 0; i < d->n_hidden; ++i)
-    if (d->hidden[i] % 16 != 0 || d->hidden[i] > 256) return false;
-  const int nst = d->n_hidden + 1;
-  const int Wp = d->W + 1;
-  const int SPS = (d->H + 1) * Wp;
-  const int MIR = tc_round_up(Wp + 1, 8);  // largest tap shift, rounded
-  if (MIR > TC_TILE) return false;
-  IafTcPlan tmp;
-  IafTcPlan* q = pl ? pl : &tmp;
-  q->n_stages = nst;
-  q->MIR = MIR; q->WIN = TC_TILE + MIR; q->RING = 2 * TC_TILE + MIR;
-  q->MAXS = (TC_TILE - 1) / SPS + 2;
-  if ((d->n_z / 8) * q->WIN > TC_ZITEMS * TC_GTHREADS) return false;
-  int off = 0, prev = d->n_z;
-  for (int j = 0; j < nst; ++j) {
-    q->cin[j] = prev;
-    q->N[j] = (j < d->n_hidden) ? d->hidden[j] : 2 * d->n_z;
-    q->K[j] = IAF_NTAPS * prev;
-    const int wb = q->K[j] * q->N[j] * 2;
-    q->sm_whi[j] = off; off += wb;
-    q->sm_wlo[j] = off; off += wb;
-    prev = q->N[j];
-  }
-  for (int j = 0; j < nst; ++j) {
-    q->in_slots[j] = (j == 0) ? q->WIN : q->RING;
-    q->sm_in[j] = off;
-    off += 2 * (q->cin[j] / 8) * q->in_slots[j] * 16;  // hi + lo plane sets
-  }
-  for (int j = 0; j < nst; ++j) {
-    q->sm_bias[j] = off;
-    off += 5 * q->N[j] * 4;
-  }
-  off = tc_round_up(off, 16);
-  q->sm_part = off;
-  const int part_step = 2 * TC_GWARPS * q->MAXS * 4;
-  const int part_layer = 2 * 4 * q->MAXS * d->n_z * 4;
-  q->layer_ok = (off + std::max(part_step, part_layer)) <= TC_SMEM_LIMIT;
-  off += q->layer_ok ? std::max(part_step, part_layer) : part_step;
-  // TMEM (512 columns): double-buffer every accumulator if possible, then spend what is left on the merged
-  // hi*[hi|lo] form (accumulator spans 2N columns, one MMA and one A fetch fewer per K step), the heads first
-  int cols = 0;
-  for (int j = 0; j < nst; ++j) { q->dbl[j] = 0; q->merged[j] = 0; q->acc_cols[j] = q->N[j]; cols += q->N[j]; }
-  if (cols > 512) return false;
-  for (int j = nst - 1; j >= 0; --j)
-    if (cols + q->N[j] <= 512) { q->dbl[j] = 1; cols += q->N[j]; }
-  // (A/B on one B200, C2a: merged 30.6 us vs 31.3 us without: the heads' MMAs drop 3.3K -> 2.7K cycles per tile, most of
-  //  which the second TMEM read in the epilogues gives back; IAF_TC_MERGED=0 switches it off)
-  const char* mg = getenv("IAF_TC_MERGED");
-  for (int j = nst - 1; j >= 0 && !(mg && mg[0] == '0'); --j) {
-    const int extra = q->N[j] * (1 + q->dbl[j]);
-    if (2 * q->N[j] <= 256 && cols + extra <= 512) { q->merged[j] = 1; q->acc_cols[j] = 2 * q->N[j]; cols += extra; }
-  }
-  int col = 0;
-  for (int j = 0; j < nst; ++j) { q->tmem_col[j] = col; col += q->acc_cols[j] * (1 + q->dbl[j]); }
-  int tc = 32;
-  while (tc < col) tc *= 2;
-  q->tmem_cols = tc;
-  q->smem = (size_t)off;
-  return off <= TC_SMEM_LIMIT;
-}
-
-// layer-at-a-time layout: per stage an A window, an NB-deep weight ring, the bias table and the partial scratch
+// per stage: an A window (first stage), the bias table, the partial scratch, the accumulator tile, an NB-deep ring
 static bool ly_layout(const iaf_desc_t* d, IafTcPlan* pl) {
   if (d->n_hidden < 1 || d->n_heads != 2 || d->head[0] != d->n_z || d->head[1] != d->n_z) return false;
   if (d->n_z % 16 != 0 || 2 * d->n_z > 256) return false;
@@ -1445,7 +386,7 @@ static bool ly_layout(const iaf_desc_t* d, IafTcPlan* pl) {
   IafTcPlan tmp;
   IafTcPlan* q = pl ? pl : &tmp;
   q->n_stages = nst;
-  q->MIR = MIR; q->WIN = TC_TILE + MIR; q->RING = 0;
+  q->MIR = MIR; q->WIN = TC_TILE + MIR;
   q->MAXS = (TC_TILE - 1) / SPS + 2;
   if ((d->n_z / 8) * q->WIN > TC_ZITEMS * LY_WTHREADS) return false;
   int prev = d->n_z;
@@ -1462,52 +403,63 @@ static bool ly_layout(const iaf_desc_t* d, IafTcPlan* pl) {
     off = tc_round_up(off, 16);
     q->ly_sm_part[j] = off;
     off += std::max(2 * LY_WORKERS * q->MAXS * 4, 2 * 4 * q->MAXS * d->n_z * 4);
+    off = tc_round_up(off, 16);
+    q->ly_sm_acc[j] = off; off += TC_TILE * ly_acc_pitch(q->N[j]) * 4;
     off = tc_round_up(off, 128);
     q->ly_sm_b[j] = off;
     const int slot = 2 * LY_KC * 2 * q->N[j] * 16 + (j ? 4 * q->WIN * 16 : 0);  // weight chunk hi+lo (+ A chunk pair hi+lo)
     q->ly_stage[j] = slot;
-    int nb = (TC_SMEM_LIMIT - off) / slot;
+    int nb = (TC_SMEM_LIMIT - LY_B_SLACK - off) / slot;
     if (nb < 2) return false;
     q->ly_NB[j] = std::min(nb, LY_MAX_NB);
-    q->ly_smem[j] = (size_t)off + (size_t)q->ly_NB[j] * slot;
-    if (2 * q->N[j] > 512) return false;
-    // heads stage: hi * [hi | lo] as one N' = 2N MMA when the doubled, double-buffered accumulator fits (N <= 128)
-    const char* me = getenv("IAF_LY_MERGED");
-    q->ly_merged[j] = (j == nst - 1 && 2 * q->N[j] <= 256 && 4 * q->N[j] <= 512 && !(me && me[0] == '0')) ? 1 : 0;
-    const int accw = q->ly_merged[j] ? 2 * q->N[j] : q->N[j];
-    int tc = 32;
-    while (tc < 2 * accw) tc *= 2;
-    q->ly_tmem[j] = tc;
+    q->ly_smem[j] = (size_t)off + (size_t)q->ly_NB[j] * slot + LY_B_SLACK;
   }
   return true;
 }
 
-bool iaf_tc_supported(const iaf_desc_t* d) { return fz_layout(d, nullptr) || tc_layout(d, nullptr) || ly_layout(d, nullptr); }
+// one-launch layout (after ly_layout filled cin / N / K / MIR / WIN / MAXS): A window, hidden operand buffer (TC_TILE + MIR
+// rows: the heads' shifted windows of the rows past TS read beyond the 128 computed rows; those rows are not stored), both
+// bias tables, the partials, the accumulator tile and both resident weight images
+static bool fz_layout(const iaf_desc_t* d, IafTcPlan* q) {
+  if (d->n_hidden != 1 || q->N[0] > 32 * FZ_NGW || q->N[1] > 32 * FZ_NGW) return false;
+  if (TC_TILE - q->MIR < TC_TILE / 2) return false;
+  const int nb0 = q->K[0] / 16 / LY_KC, nb1 = q->K[1] / 16 / LY_KC;
+  if (nb0 + nb1 > LY_MAX_NB) return false;
+  int off = 0;
+  q->fz_sm_a = off; off += 2 * (q->cin[0] / 8) * q->WIN * 16;
+  q->fz_sm_h = off; off += 2 * (q->N[0] / 8) * (TC_TILE + q->MIR) * 16;
+  for (int j = 0; j < 2; ++j) { q->fz_sm_bias[j] = off; off += 5 * q->N[j] * 4; }
+  off = tc_round_up(off, 16);
+  q->fz_sm_part = off; off += std::max(2 * LY_WORKERS * q->MAXS * 4, 2 * 4 * q->MAXS * d->n_z * 4);
+  off = tc_round_up(off, 16);
+  q->fz_sm_acc = off; off += TC_TILE * ly_acc_pitch(std::max(q->N[0], q->N[1])) * 4;
+  off = tc_round_up(off, 128);
+  for (int j = 0; j < 2; ++j) { q->fz_sm_b[j] = off; off += 2 * q->K[j] * q->N[j] * 2; }
+  off += LY_B_SLACK;
+  q->fz_smem = (size_t)off;
+  return off <= TC_SMEM_LIMIT;
+}
+
+bool iaf_tc_supported(const iaf_desc_t* d) { return ly_layout(d, nullptr); }
 
 int iaf_tc_plan_create(IafTcPlan** out, const iaf_desc_t* d) {
   IafTcPlan* pl = new (std::nothrow) IafTcPlan();
   if (!pl) return IAF_ERR_BAD_ARG;
   memset(pl, 0, sizeof(*pl));
   pl->d = *d;
-  pl->layered = false;
-  pl->fz = false;
-  const char* force = getenv("IAF_TC_FORCE_LAYERED");  // development switch: compare the two tensor-core schedules
-  const char* nofz = getenv("IAF_TC_FZ");              // development switch: IAF_TC_FZ=0 keeps the first-generation kernel
-  if (!(force && force[0] == '1') && !(nofz && nofz[0] == '0') && fz_layout(d, pl)) {
-    pl->fz = true;
-  } else if ((force && force[0] == '1') || !tc_layout(d, pl)) {
-    if (!ly_layout(d, pl)) { delete pl; return IAF_ERR_UNSUPPORTED; }
-    pl->layered = true;
-  }
+  if (!ly_layout(d, pl)) { delete pl; return IAF_ERR_UNSUPPORTED; }
+  // IAF_TC_FUSED=0 (development): one-hidden-layer stacks on the per-stage kernel too, for A/B against the fused one
+  const char* fe = getenv("IAF_TC_FUSED");
+  pl->fused = !(fe && fe[0] == '0') && fz_layout(d, pl);
   int dev = 0;
   cudaDeviceProp prop;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) { delete pl; return IAF_ERR_CUDA; }
-  if (prop.major != 10) { delete pl; return IAF_ERR_UNSUPPORTED; }  // tcgen05 needs sm_100
+  if (prop.major != 9) { delete pl; return IAF_ERR_UNSUPPORTED; }  // wgmma: sm_90a
   pl->num_sms = prop.multiProcessorCount;
   for (int j = 0; j < pl->n_stages; ++j) {
     const size_t wb = (size_t)pl->K[j] * pl->N[j] * 2;
-    // bias [N] and pad-channel weights [4][N] are ONE table [5][N] (iaf_fz_kernel fetches it with a single bulk copy)
-    if (cudaMalloc(&pl->whi[j], 2 * wb) != cudaSuccess || cudaMalloc(&pl->wlo[j], wb) != cudaSuccess ||
+    // bias [N] and pad-channel weights [4][N] are ONE table [5][N]
+    if (cudaMalloc(&pl->whi[j], wb) != cudaSuccess || cudaMalloc(&pl->wlo[j], wb) != cudaSuccess ||
         cudaMalloc(&pl->bias[j], sizeof(float) * 5 * pl->N[j]) != cudaSuccess) {
       iaf_tc_plan_destroy(pl);
       return IAF_ERR_CUDA;
@@ -1515,15 +467,10 @@ int iaf_tc_plan_create(IafTcPlan** out, const iaf_desc_t* d) {
     pl->padw[j] = pl->bias[j] + pl->N[j];
   }
   for (int a = 0; a < 12; ++a) {
-    cudaError_t e;
     const int md = (a >> 2) == 0 ? IAF_MODE_MULTICONV : ((a >> 2) == 1 ? IAF_MODE_STEP : IAF_MODE_LAYER);
-    if (pl->fz) {
-      e = iaf_smem_optin(fz_kernel_for(a & 1, md, a & 2, false));
-      if (e == cudaSuccess) e = iaf_smem_optin(fz_kernel_for(a & 1, md, a & 2, true));
-    } else if (pl->layered)
-      e = iaf_smem_optin(ly_kernel_for(a & 1, md, a & 2, d->H * d->W));
-    else
-      e = iaf_smem_optin(tc_kernel_for(a & 1, md, a & 2, d->H * d->W));
+    cudaError_t e = cudaSuccess;
+    if (pl->fused) e = iaf_smem_optin(fz_kernel_for(a & 1, md, a & 2));
+    for (int j = 0; j < pl->n_stages && e == cudaSuccess && !pl->fused; ++j) e = iaf_smem_optin(ly_kernel_for(a & 1, md, a & 2, pl->N[j]));
     if (e != cudaSuccess) {
       iaf_tc_plan_destroy(pl);
       return IAF_ERR_CUDA;
@@ -1554,11 +501,10 @@ int iaf_tc_pack(IafTcPlan* pl, const float* const* w, const float* const* scale,
   memset(&pp, 0, sizeof(pp));
   pp.n_layers = d.n_hidden + d.n_heads;
   pp.variant = d.variant;
-  pp.korder = pl->layered ? 1 : 0;
   int max_cout = 0;
   for (int j = 0; j < pl->n_stages; ++j) {
     const size_t wb = (size_t)pl->K[j] * pl->N[j] * 2;
-    if (cudaMemsetAsync(pl->whi[j], 0, 2 * wb, stream) != cudaSuccess) return IAF_ERR_CUDA;
+    if (cudaMemsetAsync(pl->whi[j], 0, wb, stream) != cudaSuccess) return IAF_ERR_CUDA;
     if (cudaMemsetAsync(pl->wlo[j], 0, wb, stream) != cudaSuccess) return IAF_ERR_CUDA;
     if (cudaMemsetAsync(pl->padw[j], 0, sizeof(float) * 4 * pl->N[j], stream) != cudaSuccess) return IAF_ERR_CUDA;
   }
@@ -1574,7 +520,6 @@ int iaf_tc_pack(IafTcPlan* pl, const float* const* w, const float* const* scale,
     L.zerodiag = is_head ? 1 : 0;
     L.is_head = is_head ? 1 : 0;
     L.head = is_head ? i - d.n_hidden : 0;
-    L.merged = pl->layered ? pl->ly_merged[j] : 0;
     max_cout = std::max(max_cout, L.cout);
   }
   dim3 grid(max_cout, pp.n_layers);
@@ -1601,49 +546,9 @@ extern "C" void iaf_tc_timeline_dump(void) {
 }
 #endif
 
-#ifdef IAF_FZ_PROBE
-extern "C" void iaf_fz_probe_dump(void) {
-  cudaDeviceSynchronize();
-  long long h[4][8];
-  cudaMemcpyFromSymbol(h, g_fz_probe, sizeof(h));
-  static const char* names[3][8] = {
-      {"wait ZFULL", "wait A0_INIT", "issue M0", "wait H_FULL", "wait A1_EMPTY", "issue M1", "wait weights", "loop glue"},
-      {"issue loads", "wait tables", "wait A0_EMPTY", "ctx -> TMEM", "wait ZEMPTY", "z -> smem", "-", "-"},
-      {"wait A0_FULL", "wait H_EMPTY", "E0 body", "E1 loads + wait A1_FULL", "E1 body", "wait PART_EMPTY", "wait tables", "loop glue"}};
-  static const char* roles[3] = {"MMA warp", "loader warp 0", "epilogue warp 0"};
-  for (int r = 0; r < 3; ++r) {
-    long long tot = 0;
-    for (int i = 0; i < 8; ++i) tot += h[r][i];
-    if (!tot) continue;
-    printf("PROBE %-16s total %7lld :", roles[r], tot);
-    for (int i = 0; i < 8; ++i) printf("  %s %lld", names[r][i], h[r][i]);
-    printf("\n");
-  }
-  // layer-at-a-time kernel: [stage][role][slot]
-  long long g[4][3][8];
-  cudaMemcpyFromSymbol(g, g_ly_probe, sizeof(g));
-  static const char* lnames[3][4] = {{"wait ring slot free", "issue copies", "-", "-"},
-                                     {"wait ACC_EMPTY", "wait A window", "wait ring stage", "issue MMAs + glue"},
-                                     {"wait ACC_FULL", "pre-wait (context / z loads)", "epilogue body", "z window build"}};
-  static const char* lroles[3] = {"producer", "MMA warp", "worker warp 0"};
-  for (int st = 0; st < 4; ++st)
-    for (int r = 0; r < 3; ++r) {
-      long long tot = 0;
-      for (int i = 0; i < 8; ++i) tot += g[st][r][i];
-      if (!tot) continue;
-      printf("PROBE layered stage %d %-14s total %7lld :", st, lroles[r], tot);
-      for (int i = 0; i < 4; ++i) printf("  %s %lld", lnames[r][i], g[st][r][i]);
-      printf("\n");
-    }
-  static long long zero[4][3][8];
-  cudaMemcpyToSymbol(g_ly_probe, zero, sizeof(zero));
-}
-#endif
-
 bool iaf_tc_mode_supported(const IafTcPlan* pl, int mode) {
   return mode == IAF_MODE_STEP || mode == IAF_MODE_MULTICONV || (mode == IAF_MODE_LAYER && pl->layer_ok);
 }
-bool iaf_tc_is_layered(const IafTcPlan* pl) { return pl->layered; }
 
 int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_launches) {
   const iaf_desc_t& d = pl->d;
@@ -1651,29 +556,28 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
   const int SPS = (d.H + 1) * (d.W + 1);
   if ((long long)B * SPS + TC_TILE >= (1LL << 31)) return IAF_ERR_UNSUPPORTED;
   const int S = B * SPS;
-  const int tile_step = pl->fz ? pl->TO : TC_TILE;  // output slots per tile
-  const int NT = (S + tile_step - 1) / tile_step;
-  if (B > pl->scratch_B) {
+  const int TS = pl->fused ? TC_TILE - pl->MIR : TC_TILE;  // slots a tile advances (fused: overlapped windows)
+  const int NT = (S + TS - 1) / TS;
+  if (B > pl->scratch_B || NT > pl->scratch_NT) {
     if (pl->counter) cudaFree(pl->counter);
     if (pl->tilepart) cudaFree(pl->tilepart);
     pl->counter = nullptr; pl->tilepart = nullptr; pl->scratch_B = 0;
-    if (pl->layered) {
-      int maxc = 0;
-      for (int j = 0; j + 1 < pl->n_stages; ++j) maxc = std::max(maxc, pl->N[j]);
-      pl->img_S_pad = (NT + 1) * TC_TILE;  // one zero tile past the end: windows of the last tile read into it
-      const size_t bytes = (size_t)(maxc / 8) * pl->img_S_pad * 16;
-      for (int a2 = 0; a2 < 2; ++a2)
-        for (int b2 = 0; b2 < 2; ++b2) {
-          if (pl->img[a2][b2]) cudaFree(pl->img[a2][b2]);
-          pl->img[a2][b2] = nullptr;
-          if (cudaMalloc(&pl->img[a2][b2], bytes) != cudaSuccess) return IAF_ERR_CUDA;
-          if (cudaMemset(pl->img[a2][b2], 0, bytes) != cudaSuccess) return IAF_ERR_CUDA;
-        }
-    }
+    int maxc = 0;
+    for (int j = 0; j + 1 < pl->n_stages; ++j) maxc = std::max(maxc, pl->N[j]);
+    pl->img_S_pad = (NT + 1) * TC_TILE;  // one zero tile past the end: windows of the last tile read into it
+    const size_t bytes = (size_t)(maxc / 8) * pl->img_S_pad * 16;
+    for (int a2 = 0; a2 < 2; ++a2)
+      for (int b2 = 0; b2 < 2; ++b2) {
+        if (pl->img[a2][b2]) cudaFree(pl->img[a2][b2]);
+        pl->img[a2][b2] = nullptr;
+        if (cudaMalloc(&pl->img[a2][b2], bytes) != cudaSuccess) return IAF_ERR_CUDA;
+        if (cudaMemset(pl->img[a2][b2], 0, bytes) != cudaSuccess) return IAF_ERR_CUDA;
+      }
     if (cudaMalloc(&pl->counter, sizeof(unsigned) * (size_t)B) != cudaSuccess) return IAF_ERR_CUDA;
     if (cudaMemset(pl->counter, 0, sizeof(unsigned) * (size_t)B) != cudaSuccess) return IAF_ERR_CUDA;
     if (cudaMalloc(&pl->tilepart, sizeof(float) * (size_t)NT * pl->MAXS * d.n_z) != cudaSuccess) return IAF_ERR_CUDA;
     pl->scratch_B = B;
+    pl->scratch_NT = NT;
   }
   IafTcParams p;
   memset(&p, 0, sizeof(p));
@@ -1684,134 +588,82 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
   p.bc_out = a->bc_out; p.persample_out = a->persample_out;
   p.tilepart = pl->tilepart;
   p.counter = pl->counter;
-  p.n_stages = pl->n_stages;
+  p.n_stages = 1;
+  p.B = B; p.C = d.n_z; p.H = d.H; p.W = d.W; p.Wp = d.W + 1; p.SPS = SPS; p.HW = d.H * d.W;
+  p.S = S; p.NT = NT;
+  p.MIR = pl->MIR; p.WIN = pl->WIN; p.MAXS = pl->MAXS;
+  p.flip = d.variant == IAF_VARIANT_THEANO ? 1 : 0;
+  p.nl = d.nl; p.scale = 0.1f;
+  p.mg_sps = (unsigned)((1ULL << 32) / (unsigned)SPS) + 1u;
+  p.mg_wp = (unsigned)((1ULL << 32) / (unsigned)p.Wp) + 1u;
+  p.mg_win = (unsigned)((1ULL << 32) / (unsigned)p.WIN) + 1u;
+  const int grid = std::min(pl->num_sms, NT);
+  const bool padw = d.variant == IAF_VARIANT_THEANO, elu = d.nl == IAF_NL_ELU;
+  auto launch = [&](LyKernel lk, const IafLyParams& q, size_t smem) {
+    const char* pe = getenv("IAF_PDL");
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(LY_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = (pe && pe[0] == '0') ? 0 : 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, lk, q) == cudaSuccess;
+  };
+  if (pl->fused) {
+    IafLyParams q;
+    memset(&q, 0, sizeof(q));
+    q.t = p;
+    for (int j = 0; j < 2; ++j) {
+      IafTcStage& S_ = q.t.st[j];
+      S_.whi = pl->whi[j]; S_.wlo = pl->wlo[j]; S_.bias = pl->bias[j]; S_.padw = pl->padw[j];
+      S_.hid_out = j == 0 ? a->hid_out[0] : nullptr;
+      S_.cin = pl->cin[j]; S_.N = pl->N[j]; S_.K = pl->K[j];
+    }
+    q.t.n_stages = 2;
+    q.t.sm_part = pl->fz_sm_part;
+    q.in_mode = 0; q.first = 1; q.is_heads = 0;
+    q.NB = LY_MAX_NB;
+    q.sm_a = pl->fz_sm_a; q.sm_h = pl->fz_sm_h; q.sm_bias = pl->fz_sm_bias[0]; q.sm_bias1 = pl->fz_sm_bias[1];
+    q.sm_part = pl->fz_sm_part; q.sm_acc = pl->fz_sm_acc; q.sm_b = pl->fz_sm_b[0]; q.sm_b1 = pl->fz_sm_b[1];
+    q.b_chunk_bytes = LY_KC * 2 * pl->N[0] * 16; q.n_bchunks = (pl->K[0] / 16) / LY_KC;
+    q.b_chunk_bytes1 = LY_KC * 2 * pl->N[1] * 16; q.n_bchunks1 = (pl->K[1] / 16) / LY_KC;
+    q.stage_bytes = 2 * q.b_chunk_bytes;
+    q.TS = TS; q.TO = TS;
+    q.tl_enable = 1;
+    if (!launch(fz_kernel_for(padw, a->mode, elu), q, pl->fz_smem)) return IAF_ERR_CUDA;
+    if (n_launches) *n_launches = 1;
+    return cudaGetLastError() == cudaSuccess ? IAF_OK : IAF_ERR_CUDA;
+  }
   for (int j = 0; j < pl->n_stages; ++j) {
-    IafTcStage& S_ = p.st[j];
+    IafLyParams q;
+    memset(&q, 0, sizeof(q));
+    q.t = p;
+    q.TS = TC_TILE; q.TO = TC_TILE;
+    IafTcStage& S_ = q.t.st[0];
     S_.whi = pl->whi[j]; S_.wlo = pl->wlo[j]; S_.bias = pl->bias[j];
     S_.padw = pl->padw[j];
     S_.hid_out = (j < IAF_MAX_HIDDEN && j + 1 < pl->n_stages) ? a->hid_out[j] : nullptr;
     S_.cin = pl->cin[j]; S_.N = pl->N[j]; S_.K = pl->K[j];
-    S_.w_bytes = pl->K[j] * pl->N[j] * 2;
-    S_.sm_whi = pl->sm_whi[j]; S_.sm_wlo = pl->sm_wlo[j]; S_.sm_in = pl->sm_in[j];
-    S_.in_slots = pl->in_slots[j]; S_.sm_bias = pl->sm_bias[j];
-    S_.tmem_col = pl->tmem_col[j]; S_.dbl = pl->dbl[j]; S_.merged = pl->merged[j]; S_.acc_cols = pl->acc_cols[j];
+    q.t.sm_part = pl->ly_sm_part[j];
+    q.a_hi = j ? pl->img[(j - 1) & 1][0] : nullptr;
+    q.a_lo = j ? pl->img[(j - 1) & 1][1] : nullptr;
+    q.o_hi = pl->img[j & 1][0];
+    q.o_lo = pl->img[j & 1][1];
+    q.S_pad = pl->img_S_pad;
+    q.in_mode = j ? 1 : 0;
+    q.first = j == 0;
+    q.is_heads = j == pl->n_stages - 1;
+    q.NB = pl->ly_NB[j];
+    q.sm_a = pl->ly_sm_a[j]; q.sm_b = pl->ly_sm_b[j]; q.sm_bias = pl->ly_sm_bias[j]; q.sm_part = pl->ly_sm_part[j];
+    q.sm_acc = pl->ly_sm_acc[j];
+    q.b_chunk_bytes = LY_KC * 2 * pl->N[j] * 16;
+    q.stage_bytes = pl->ly_stage[j];
+    q.n_bchunks = (pl->K[j] / 16) / LY_KC;
+    { const char* tls = getenv("IAF_TL_STAGE"); q.tl_enable = tls ? (atoi(tls) == j) : (j == pl->n_stages - 1); }
+    if (!launch(ly_kernel_for(padw, a->mode, elu, pl->N[j]), q, pl->ly_smem[j])) return IAF_ERR_CUDA;
   }
-  p.B = B; p.C = d.n_z; p.H = d.H; p.W = d.W; p.Wp = d.W + 1; p.SPS = SPS; p.HW = d.H * d.W;
-  p.S = S; p.NT = NT;
-  p.MIR = pl->MIR; p.WIN = pl->WIN; p.RING = pl->RING; p.MAXS = pl->MAXS; p.sm_part = pl->sm_part;
-  p.flip = d.variant == IAF_VARIANT_THEANO ? 1 : 0;
-  p.nl = d.nl; p.scale = 0.1f;
-  p.tmem_cols = pl->tmem_cols;
-  { const char* pf = getenv("IAF_TC_PREFETCH"); p.prefetch = (pf && a->mode != IAF_MODE_LAYER) ? atoi(pf) : 0; }
-  p.mg_sps = (unsigned)((1ULL << 32) / (unsigned)SPS) + 1u;
-  p.mg_wp = (unsigned)((1ULL << 32) / (unsigned)p.Wp) + 1u;
-  p.mg_win = (unsigned)((1ULL << 32) / (unsigned)p.WIN) + 1u;
-  p.TO = pl->TO; p.h_bytes = pl->h_bytes; p.z_bytes = pl->z_bytes;
-  size_t fz_smem = 0;
-  bool fz_plane256 = false;
-  if (pl->fz) {
-    // staged z (bulk copies) when the plan has that layout and the mode allows it; IAF_FZ_STAGE=0 switches it off (A/B)
-    const char* st = getenv("IAF_FZ_STAGE");
-    bool staged = pl->fzl[1].ok && a->mode != IAF_MODE_LAYER && !(st && st[0] == '0');
-    // the descriptor carries the z pointer, so it is encoded per call (host side, ~1 us) and travels in the parameters
-    if (staged) {
-      IafTcPlan::TmSlot& ts = pl->tm_cache[(reinterpret_cast<uintptr_t>(a->z) >> 12) & 15];
-      if (ts.z != a->z || ts.B != B) {
-        bool ok = (reinterpret_cast<uintptr_t>(a->z) & 15) == 0;
-        for (int r = 1; r <= IAF_FZ_MAXROWS && ok; ++r) ok = encode_z_tmap(ts.tm[r - 1], a->z, B, d.n_z, d.H, d.W, r);
-        if (!ok) {
-          staged = false;
-          ts.z = nullptr;
-        } else {
-          ts.z = a->z; ts.B = B;
-        }
-      }
-      if (staged) memcpy(p.tmap_z, ts.tm, sizeof(ts.tm));
-    }
-    fz_plane256 = d.H == 16 && d.W == 16 && (staged || a->mode == IAF_MODE_LAYER);
-    const IafTcPlan::FzLay& L = pl->fzl[staged ? 1 : 0];
-    p.nzw = L.nzw; p.nhb = L.nhb; p.nzs = L.nzs; p.zst_bytes = L.zst_bytes; p.sm_zst = L.sm_zst; p.sm_part = L.sm_part;
-
-    p.st[1].sm_in = L.sm_in1;
-    p.st[0].sm_bias = L.sm_bias[0]; p.st[1].sm_bias = L.sm_bias[1];
-    fz_smem = L.smem;
-  }
-  { const char* dbg = getenv("IAF_FZ_DBG"); p.dbg = dbg ? atoi(dbg) : 0; }
-  const int grid = std::min(pl->num_sms, NT);
-  if (pl->layered) {
-    LyKernel lk = ly_kernel_for(d.variant == IAF_VARIANT_THEANO, a->mode, d.nl == IAF_NL_ELU, d.H * d.W);
-    for (int j = 0; j < pl->n_stages; ++j) {
-      IafLyParams q;
-      memset(&q, 0, sizeof(q));
-      q.t = p;
-      q.t.st[0] = p.st[j];
-      q.t.n_stages = 1;
-      q.t.tmem_cols = pl->ly_tmem[j];
-      q.t.sm_part = pl->ly_sm_part[j];
-      q.a_hi = j ? pl->img[(j - 1) & 1][0] : nullptr;
-      q.a_lo = j ? pl->img[(j - 1) & 1][1] : nullptr;
-      q.o_hi = pl->img[j & 1][0];
-      q.o_lo = pl->img[j & 1][1];
-      q.S_pad = pl->img_S_pad;
-      q.in_mode = j ? 1 : 0;
-      q.stage_id = j;
-      q.merged = pl->ly_merged[j];
-      // A-operand collector for the (A_hi x B_lo, A_hi x B_hi) pair of every tap: measured C2b 117.4 -> 115.2 us, C3 36.9 -> 36.3 us
-      // (profiles/r2_mma_collector.log; the "liar" test there shows the second MMA really takes A from the collector).
-      { const char* ce = getenv("IAF_LY_COLLECTOR"); q.collector = ce ? atoi(ce) : 1; }
-      q.first = j == 0;
-      q.is_heads = j == pl->n_stages - 1;
-      q.NB = pl->ly_NB[j];
-      q.sm_a = pl->ly_sm_a[j]; q.sm_b = pl->ly_sm_b[j]; q.sm_bias = pl->ly_sm_bias[j]; q.sm_part = pl->ly_sm_part[j];
-      q.b_chunk_bytes = LY_KC * 2 * pl->N[j] * 16;
-      q.stage_bytes = pl->ly_stage[j];
-      q.n_bchunks = (pl->K[j] / 16) / LY_KC;
-      { const char* tls = getenv("IAF_TL_STAGE"); q.tl_enable = tls ? (atoi(tls) == j) : (j == pl->n_stages - 1); }
-      // Optional: clusters of CTAs share the weight stream through TMA multicast (IAF_LY_CLUSTER=2|4).  Measured on
-      // B200 (C2b): 118.8 us without, 119.8 us with 2-CTA clusters, 199 us with 4 -- the stage is not limited by L2
-      // reads of the weights but by shared-memory operand bandwidth, and lock-stepping the ring across CTAs costs
-      // more than the saved L2 traffic; so the default stays 1.
-      int cs = 1;
-      {
-        const char* e = getenv("IAF_LY_CLUSTER");
-        const int want = e ? atoi(e) : 1;
-        const bool streams = q.n_bchunks > q.NB || q.in_mode;
-        if (streams && (2 * q.b_chunk_bytes) % (16 * want) == 0 && (want == 2 || want == 4) && grid % want == 0) cs = want;
-      }
-      q.cs = cs;
-      {
-        const char* pe = getenv("IAF_PDL");
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(LY_THREADS); cfg.dynamicSmemBytes = pl->ly_smem[j]; cfg.stream = stream;
-        cudaLaunchAttribute at[2];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = (pe && pe[0] == '0') ? 0 : 1;
-        at[1].id = cudaLaunchAttributeClusterDimension;
-        at[1].val.clusterDim.x = cs; at[1].val.clusterDim.y = 1; at[1].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = cs > 1 ? 2 : 1;
-        if (cudaLaunchKernelEx(&cfg, lk, q) != cudaSuccess) return IAF_ERR_CUDA;
-      }
-    }
-    if (n_launches) *n_launches = pl->n_stages;
-    return cudaGetLastError() == cudaSuccess ? IAF_OK : IAF_ERR_CUDA;
-  }
-  TcKernel k = pl->fz ? fz_kernel_for(d.variant == IAF_VARIANT_THEANO, a->mode, d.nl == IAF_NL_ELU, fz_plane256)
-                      : tc_kernel_for(d.variant == IAF_VARIANT_THEANO, a->mode, d.nl == IAF_NL_ELU, d.H * d.W);
-  {
-    const char* e = getenv("IAF_PDL");
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(pl->fz ? FZ_THREADS : TC_THREADS);
-    cfg.dynamicSmemBytes = pl->fz ? fz_smem : pl->smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = (e && e[0] == '0') ? 0 : 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    if (cudaLaunchKernelEx(&cfg, k, p) != cudaSuccess) return IAF_ERR_CUDA;
-  }
-  if (n_launches) *n_launches = 1;
+  if (n_launches) *n_launches = pl->n_stages;
   return cudaGetLastError() == cudaSuccess ? IAF_OK : IAF_ERR_CUDA;
 }
 
@@ -1833,8 +685,8 @@ struct IafDgPlan {
   __nv_bfloat16* whi[IAF_MAX_STAGES];
   __nv_bfloat16* wlo[IAF_MAX_STAGES];
   float* zeros;  // bias table of the stages (the kernel adds it; the gradient has none)
-  int sm_bias[IAF_MAX_STAGES], sm_part[IAF_MAX_STAGES], sm_b[IAF_MAX_STAGES], stage[IAF_MAX_STAGES], NB[IAF_MAX_STAGES],
-      tmem[IAF_MAX_STAGES];
+  int sm_bias[IAF_MAX_STAGES], sm_part[IAF_MAX_STAGES], sm_acc[IAF_MAX_STAGES], sm_b[IAF_MAX_STAGES], stage[IAF_MAX_STAGES],
+      NB[IAF_MAX_STAGES];
   size_t smem[IAF_MAX_STAGES];
   int MIR, WIN, MAXS, max_ch;
   __nv_bfloat16* img[2][2];  // ping-pong operand images [buffer][hi | lo]
@@ -1957,7 +809,7 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
   int dev = 0;
   cudaDeviceProp prop;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return IAF_ERR_CUDA;
-  if (prop.major != 10) return IAF_ERR_UNSUPPORTED;
+  if (prop.major != 9) return IAF_ERR_UNSUPPORTED;  // wgmma: sm_90a
   const int Wp = d->W + 1;
   const int SPS = (d->H + 1) * Wp;
   const int MIR = tc_round_up(Wp + 1, 8);
@@ -1975,22 +827,21 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
     pl->kin[j] = kin; pl->nout[j] = N;
     pl->max_ch = std::max(pl->max_ch, std::max(kin, N));
     maxn = std::max(maxn, N);
-    if (kin % 16 || N % 16 || kin > 16 * LY_MAX_KS || N > 256 || N < 16) { iaf_dg_plan_destroy(pl); return IAF_ERR_UNSUPPORTED; }
+    if (kin % 16 || N % 16 || kin > 256 || N > 256 || N < 16) { iaf_dg_plan_destroy(pl); return IAF_ERR_UNSUPPORTED; }
     int off = 0;
     pl->sm_bias[j] = off; off += 5 * N * 4;
     off = tc_round_up(off, 16);
     pl->sm_part[j] = off; off += 2 * LY_WORKERS * pl->MAXS * 4;
+    off = tc_round_up(off, 16);
+    pl->sm_acc[j] = off; off += TC_TILE * ly_acc_pitch(N) * 4;
     off = tc_round_up(off, 128);
     pl->sm_b[j] = off;
     const int slot = 2 * LY_KC * 2 * N * 16 + 4 * pl->WIN * 16;  // weight chunk hi+lo + A chunk pair hi+lo
     pl->stage[j] = slot;
-    const int nb = (TC_SMEM_LIMIT - off) / slot;
+    const int nb = (TC_SMEM_LIMIT - LY_B_SLACK - off) / slot;
     if (nb < 2) { iaf_dg_plan_destroy(pl); return IAF_ERR_UNSUPPORTED; }
     pl->NB[j] = std::min(nb, LY_MAX_NB);
-    pl->smem[j] = (size_t)off + (size_t)pl->NB[j] * slot;
-    int tc = 32;
-    while (tc < 2 * N) tc *= 2;
-    pl->tmem[j] = tc;
+    pl->smem[j] = (size_t)off + (size_t)pl->NB[j] * slot + LY_B_SLACK;
     const size_t wb = (size_t)IAF_NTAPS * kin * N * 2;
     if (cudaMalloc(&pl->whi[j], wb) != cudaSuccess || cudaMalloc(&pl->wlo[j], wb) != cudaSuccess) {
       iaf_dg_plan_destroy(pl);
@@ -2002,8 +853,12 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
     iaf_dg_plan_destroy(pl);
     return IAF_ERR_CUDA;
   }
-  if (iaf_smem_optin(ly_kernel_for(false, IAF_MODE_MULTICONV, d->nl == IAF_NL_ELU, d->H * d->W)) != cudaSuccess ||
-      iaf_smem_optin(iaf_wg_kernel) != cudaSuccess) {
+  cudaError_t oe = cudaSuccess;
+  for (int j = 0; j < n_stages && oe == cudaSuccess; ++j)
+    oe = iaf_smem_optin(ly_kernel_for(false, IAF_MODE_MULTICONV, d->nl == IAF_NL_ELU, pl->nout[j]));
+  for (int k = 1; k <= WG_MAX_NP / 16 && oe == cudaSuccess; ++k)
+    for (int w = 1; w <= 2 && oe == cudaSuccess; ++w) oe = iaf_smem_optin(wg_kernel_pick(k, w));
+  if (oe != cudaSuccess) {
     iaf_dg_plan_destroy(pl);
     return IAF_ERR_CUDA;
   }
@@ -2083,14 +938,11 @@ int iaf_dg_stage(IafDgPlan* pl, int j, const float* w_packed, int in_buf, const 
   S_.whi = pl->whi[j]; S_.wlo = pl->wlo[j]; S_.bias = pl->zeros; S_.padw = nullptr;
   S_.hid_out = out;
   S_.cin = kin; S_.N = N; S_.K = IAF_NTAPS * kin;
-  S_.w_bytes = S_.K * N * 2;
-  S_.sm_bias = pl->sm_bias[j];
   p.B = B; p.C = d.n_z; p.H = d.H; p.W = d.W; p.Wp = d.W + 1; p.SPS = SPS; p.HW = d.H * d.W;
   p.S = S; p.NT = NT;
   p.MIR = pl->MIR; p.WIN = pl->WIN; p.MAXS = pl->MAXS; p.sm_part = pl->sm_part[j];
   p.flip = d.variant == IAF_VARIANT_THEANO ? 0 : 1;
   p.nl = d.nl; p.scale = 0.1f;
-  p.tmem_cols = pl->tmem[j];
   p.mg_sps = (unsigned)((1ULL << 32) / (unsigned)SPS) + 1u;
   p.mg_wp = (unsigned)((1ULL << 32) / (unsigned)p.Wp) + 1u;
   p.mg_win = (unsigned)((1ULL << 32) / (unsigned)p.WIN) + 1u;
@@ -2102,17 +954,14 @@ int iaf_dg_stage(IafDgPlan* pl, int j, const float* w_packed, int in_buf, const 
   q.is_heads = 0;
   q.first = hprev ? 1 : 0;
   q.NB = pl->NB[j];
-  q.sm_a = 0; q.sm_b = pl->sm_b[j]; q.sm_bias = pl->sm_bias[j]; q.sm_part = pl->sm_part[j];
+  q.sm_a = 0; q.sm_b = pl->sm_b[j]; q.sm_bias = pl->sm_bias[j]; q.sm_part = pl->sm_part[j]; q.sm_acc = pl->sm_acc[j];
   q.b_chunk_bytes = LY_KC * 2 * N * 16;
   q.stage_bytes = pl->stage[j];
   q.n_bchunks = kin / 16;
-  q.cs = 1;
-  q.merged = 0;
-  q.collector = 1;
-  q.stage_id = 3;
   q.bwd = hprev ? 1 : 2;
   q.amax = pl->amax;
-  LyKernel lk = ly_kernel_for(false, IAF_MODE_MULTICONV, d.nl == IAF_NL_ELU, d.H * d.W);
+  q.TS = TC_TILE; q.TO = TC_TILE;
+  LyKernel lk = ly_kernel_for(false, IAF_MODE_MULTICONV, d.nl == IAF_NL_ELU, N);
   const int grid = std::min(pl->num_sms, NT);
   lk<<<grid, LY_THREADS, pl->smem[j], stream>>>(q);
   return cudaGetLastError() == cudaSuccess ? IAF_OK : IAF_ERR_CUDA;
@@ -2143,7 +992,7 @@ int iaf_wg_run(IafDgPlan* pl, int j, const float* x, int g_buf, float* part, int
   q.part = part; q.amax = pl->amax;
   q.B = B; q.cin = cin; q.ncol = ncol; q.S_pad = pl->img_S_pad; q.Wp = d.W + 1;
   int Np = 16;
-  for (int c = 16; c <= 96; c += 16)
+  for (int c = 16; c <= WG_MAX_NP; c += 16)
     if (ncol % c == 0) Np = c;
   q.Np = Np; q.n_np = ncol / Np; q.n_mb = (cin + 127) / 128;
   const int NT = (B * SPS + TC_TILE - 1) / TC_TILE;
@@ -2158,7 +1007,8 @@ int iaf_wg_run(IafDgPlan* pl, int j, const float* x, int g_buf, float* part, int
   q.n_stages = std::min(WG_MAX_STAGES, (TC_SMEM_LIMIT - slack) / q.stage_bytes);
   if (q.n_stages < 2) return IAF_ERR_UNSUPPORTED;
   const size_t smem = (size_t)q.n_stages * q.stage_bytes + slack;
-  iaf_wg_kernel<<<ntiles * q.NG, WG_THREADS, smem, stream>>>(q);
+  const int nwg = cin > 64 ? 2 : 1;
+  wg_kernel_pick(q.Np / 16, nwg)<<<ntiles * q.NG, WG_THREADS(nwg), smem, stream>>>(q);
   if (ng_used) *ng_used = q.NG;
   return cudaGetLastError() == cudaSuccess ? IAF_OK : IAF_ERR_CUDA;
 }

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05) path of the IAF step: internal interface used by iaf_capi.cu.
+// Tensor-core (wgmma, sm_90a) path of the IAF step: internal interface used by iaf_capi.cu.
 #pragma once
 #include "iaf_common.h"
 

@@ -1,75 +1,36 @@
-// Layer-at-a-time tcgen05 kernel for stacks whose hidden width does not fit the fused kernel's
-// on-chip rings (hidden = 160: BASELINE configs C2b/C3/C4/C5).  Included by iaf_tc.cu.
+// Layer-at-a-time tensor-core kernel (Hopper wgmma): one launch per conv stage of the stack.  Included by iaf_tc.cu.
 //
-// One launch per conv stage.  Same slot-stream / implicit-GEMM formulation and bf16 hi/lo operand
-// split as iaf_tc_kernel, but
-//   * the stage's input operand comes from HBM/L2: either fp32 z (stage 0, split on the fly by the
-//     worker warps) or the previous stage's output, stored as pre-split bf16 "operand images"
-//     [channel chunk][slot][8] (hi and lo) so that a tile's A window is 2*Cin/8 contiguous runs that a
-//     producer warp fetches with 1-D TMA bulk copies;
-//   * the weights are NOT resident: a producer warp streams them in chunks of KC K-steps through an
-//     NB-deep shared-memory ring (cp.async.bulk + expect_tx; the MMA warp releases a ring slot with
-//     tcgen05.commit), every CTA re-reading them from L2 once per tile;
-//   * hidden stages write their output operand image back to global memory (16-byte coalesced stores),
-//     the heads stage applies the affine update exactly like the fused kernel.
-// Accumulators are double-buffered in TMEM, so the epilogue of tile i overlaps the loads and MMAs of
-// tile i+1.
+// Same slot-stream / implicit-GEMM formulation and fp16 hi/lo operand split as described there, and
+//   * the stage's input operand comes from HBM/L2: either fp32 z (first stage, split on the fly by the worker warps into
+//     a shared-memory A window) or the previous stage's output, stored as pre-split fp16 "operand images"
+//     [channel chunk][slot][8] (hi and lo), so that a tile's A chunk pair is a few contiguous runs that the producer warp
+//     fetches with 1-D bulk copies;
+//   * the weights are NOT resident (unless they fit the ring): the producer warp streams them in chunks of LY_KC
+//     K-steps through an NB-deep shared-memory ring (cp.async.bulk + expect_tx on an mbarrier); every worker warpgroup
+//     releases a ring stage once its wgmma reads of it have completed;
+//   * the 16 worker warps are four warpgroups: warpgroup w issues the wgmma m64n16k16 instructions for rows
+//     [64 (w & 1), +64) of the tile and every second 16-column group (starting at w >> 1), accumulating in registers.
+//     The accumulators then go through a shared-memory tile [128][N + 4] so that the epilogue keeps one thread per slot
+//     (coalesced global traffic along pixels);
+//   * hidden stages write their output operand image back to global memory (16-byte stores), the heads stage applies
+//     the affine update; per-sample sums go through the reducer warp in fixed order.
 #pragma once
-
-// Optional wait-time probe of the layer-at-a-time kernel (-DIAF_FZ_PROBE, development aid; see iaf_fz.cuh): CTA 1's lead
-// lanes accumulate the cycles spent per wait / phase; g_ly_probe[stage][role][slot].
-#ifdef IAF_FZ_PROBE
-__device__ long long g_ly_probe[4][3][8];
-#define LPROBE_DECL long long lpr_[8] = {0, 0, 0, 0, 0, 0, 0, 0}; long long lpt_ = clock64();
-#define LPROBE(slot) { const long long n_ = clock64(); lpr_[slot] += n_ - lpt_; lpt_ = n_; }
-#define LPROBE_DUMP(role) if (blockIdx.x == 1 && lane == 0) { for (int i_ = 0; i_ < 8; ++i_) g_ly_probe[q.stage_id & 3][role][i_] = lpr_[i_]; }
-#else
-#define LPROBE_DECL
-#define LPROBE(slot)
-#define LPROBE_DUMP(role)
-#endif
 
 #define LY_WORKERS 16
 #define LY_WTHREADS (LY_WORKERS * 32)
-#define LY_MMA_WARP LY_WORKERS
-#define LY_TMA_WARP (LY_WORKERS + 1)
-#define LY_RED_WARP (LY_WORKERS + 2)
-#define LY_THREADS (LY_WTHREADS + 96)
+#define LY_TMA_WARP LY_WORKERS
+#define LY_RED_WARP (LY_WORKERS + 1)
+#define LY_THREADS (LY_WTHREADS + 64)
 #define LY_KC 5        // K-steps (of 16) per weight chunk
 #define LY_MAX_NB 6
+// Bytes every layout of the stage kernel reserves past its last weight image: a padded column group (16 g >= N, see
+// ly_mma_tile) of the last K plane reads up to 16 * (32 * NGW - N) bytes past the plane's end -- 256 for the per-stage
+// instantiations, 512 for the fused one (NGW = 2, N = 32) -- and that read must stay inside the CTA's allocation.
+#define LY_B_SLACK 1024
 
-#define LY_MAX_KS 16   // K-steps per tap (Cin / 16), Cin <= 256
-enum { LB_ACC_FULL = 0, LB_ACC_EMPTY = 2, LB_BFULL = 4, LB_BEMPTY = 4 + LY_MAX_NB, LB_PART = 4 + 2 * LY_MAX_NB,
-       LB_AFULL = 6 + 2 * LY_MAX_NB,                 // + K-step: chunk pair (2ks, 2ks+1) of the A window has landed
-       LB_AEMPTY = 6 + 2 * LY_MAX_NB + LY_MAX_KS,    // + K-step: the MMAs of that chunk pair are done
-       LB_PART_EMPTY = 6 + 2 * LY_MAX_NB + 2 * LY_MAX_KS,  // + tile parity: the reducer warp has consumed the partials
-       LB_COUNT = 8 + 2 * LY_MAX_NB + 2 * LY_MAX_KS };
-
-// ---- thread-block-cluster helpers: the CTAs of a cluster stream the SAME weight chunks, so each loads 1/CS of a
-// chunk and TMA-multicasts it into every member's ring stage (L2 is read once per cluster instead of once per CTA)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void bulk_g2s_mcast(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
-          smem_u32(dst)),
-      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
-// MMA-completion arrive on the same barrier of every CTA in the mask
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
+enum { LB_BFULL = 0, LB_BEMPTY = LY_MAX_NB, LB_PART = 2 * LY_MAX_NB,
+       LB_PART_EMPTY = 2 + 2 * LY_MAX_NB,  // + tile parity: the reducer warp has consumed the partials
+       LB_COUNT = 4 + 2 * LY_MAX_NB };
 
 struct IafLyParams {
   IafTcParams t;               // geometry, pointers, slot decoding (t.st[0] describes THIS stage)
@@ -82,21 +43,27 @@ struct IafLyParams {
   int is_heads;                // 1: last stage
   int first;                   // 1: first stage (adds the context)
   int NB;                      // weight ring depth
-  int sm_a, sm_b, sm_bias, sm_part;
+  int sm_a, sm_b, sm_bias, sm_part, sm_acc;
   int stage_bytes;             // bytes of one ring stage: 2 * b_chunk_bytes (+ 4 * WIN * 16 when the A pair rides along)
   int b_chunk_bytes;           // bytes of one ring slot half (hi or lo): LY_KC * 2 * N * 16
   int n_bchunks;               // weight chunks per tile
   int tl_enable;               // timeline builds only: this launch flushes its events
-  int cs;                      // cluster size (1, 2 or 4): CTAs sharing the weight stream by TMA multicast
-  int merged;                  // heads stage: A_hi x [B_hi | B_lo] as ONE N' = 2N MMA (weights image [K/8][2N][8]); accumulator 2N columns
-  int collector;               // 1: the hi*lo / hi*hi pair of a tap shares ONE shared-memory fetch of A_hi (A collector)
-  int stage_id;                // which conv stage of the stack this launch is (probe / timeline builds)
+  // one-launch step for stacks with one hidden layer (the FUSED instantiation): t.st[0] is the hidden layer, t.st[1] the
+  // heads; both weight images are resident, the hidden activations stay in shared memory
+  int TS;                      // slots a tile advances: TC_TILE, or TC_TILE - MIR when fused (overlapped windows)
+  int TO;                      // rows of a tile that produce outputs (TC_TILE, or TS when fused)
+  int sm_h;                    // fused: the hidden operand buffer [chunk][TC_TILE + MIR][8] hi, then lo
+  int sm_b1, sm_bias1;         // fused: the heads' resident weights and bias table
+  int n_bchunks1, b_chunk_bytes1;
   // data-gradient use of a hidden stage (iaf_dg_run): the input image holds the gradient at this layer's output, scaled
   // per sample into fp16 range; weights are the transposed effective weights; t.ctx points at the activations h whose
   // nl' multiplies the result (bwd 1) or is null (bwd 2: gradient at the stack input, ACCUMULATED into hid_out)
   int bwd;                     // 0 forward, 1 x nl'(h), 2 identity and accumulate
   const float* amax;           // [B] per-sample max |gradient at the heads| (the scale is 2^(5 - floor(log2 amax)))
 };
+
+// floats per row of the shared-memory accumulator tile: N + 4 keeps a warp's 16-byte row reads conflict-free
+__host__ __device__ __forceinline__ int ly_acc_pitch(int N) { return N + 4; }
 
 // nl'(pre-activation) from the activation h = nl(pre-activation)   (same table as iaf_bwd.cu's bw_nl_grad)
 __device__ __forceinline__ float dg_nl_grad(float h, int nl) {
@@ -116,74 +83,156 @@ __device__ __forceinline__ float dg_scale_from_amax(float amax) {
   return __uint_as_float((uint32_t)(127 + 5 - e) << 23);
 }
 
-template <bool PADW, int MODE, int NLT, int THW>
+// The MMAs of one stage for one tile.  Warpgroup w (of the four worker warpgroups) computes rows [64 (w & 1), +64) and the
+// 16-column groups g = (w >> 1) + 2k, k < NGW: D[64 x 16] += A_t[64 x 16] B_t[16 x 16] over K-steps, taps and the three
+// split products, accumulating in registers, then writes its fragments into the accumulator tile.  NGW is a compile-time
+// count (groups past the stage's columns compute on whatever follows in shared memory -- the next K plane, the next
+// image, or the LY_B_SLACK bytes every layout reserves past its last one -- and are not stored), so every wgmma
+// is issued unconditionally and ptxas keeps them asynchronous.
+//   ring: weight chunk c sits in ring stage gchunk % NB (parity from gchunk / NB), released after its MMAs complete;
+//   otherwise resident: chunk c sits in stage c behind barrier bar0 + c (parity 0).
+//   a_in_stage: the A chunk pair of K-step c rides in the ring stage before the weights; otherwise A is a window at a_addr.
+template <int NGW>
+__device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float* s_acc, int N, int n_chunks, bool ring, int NB,
+                                            int& gchunk, int bar0, uint32_t b_addr0, uint32_t stage_bytes,
+                                            uint32_t b_chunk_bytes, bool a_in_stage, uint32_t a_addr, uint32_t a_plane,
+                                            uint32_t a_lo_off, int Wp) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2, rh = wg & 1, gh = wg >> 1, wl = warp & 3;
+  const uint32_t b_plane = (uint32_t)N * 16u;
+  const uint32_t sh[IAF_NTAPS] = {0u, 1u, (uint32_t)(Wp - 1), (uint32_t)Wp, (uint32_t)(Wp + 1)};  // 16-byte units
+  const uint32_t a_kstep = (2u * a_plane) >> 4, b_tstep = (2u * b_plane) >> 4;
+  const uint32_t a_row = (uint32_t)(rh * 64);  // 64 slots = 64 descriptor units
+  float acc[NGW][8];
+#pragma unroll
+  for (int k = 0; k < NGW; ++k)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[k][e] = 0.f;
+  int prev_stg = -1;
+  for (int c = 0; c < n_chunks; ++c) {
+    const int stg = ring ? gchunk % NB : c;
+    mbar_wait(&bars[bar0 + stg], ring ? (uint32_t)((gchunk / NB) & 1) : 0u);
+    const uint32_t sbase = b_addr0 + (uint32_t)stg * stage_bytes;
+    uint32_t ah0, al0, bbase;
+    if (a_in_stage) {
+      ah0 = wg_desc_lo(sbase, a_plane);
+      al0 = wg_desc_lo(sbase + 2u * a_plane, a_plane);
+      bbase = sbase + 4u * a_plane;
+    } else {
+      ah0 = wg_desc_lo(a_addr, a_plane) + (uint32_t)c * a_kstep;
+      al0 = wg_desc_lo(a_addr + a_lo_off, a_plane) + (uint32_t)c * a_kstep;
+      bbase = sbase;
+    }
+    ah0 += a_row; al0 += a_row;
+    const uint32_t bh0 = wg_desc_lo(bbase, b_plane) + (uint32_t)gh * 16u;  // 16 columns = 256 B
+    const uint32_t bl0 = wg_desc_lo(bbase + b_chunk_bytes, b_plane) + (uint32_t)gh * 16u;
+    wgmma_fence();
+#pragma unroll 1
+    for (int t = 0; t < IAF_NTAPS; ++t) {
+      const uint64_t ah = mk_desc(ah0 + sh[t]), al = mk_desc(al0 + sh[t]);
+      const uint32_t bt = (uint32_t)t * b_tstep;
+#pragma unroll
+      for (int k = 0; k < NGW; ++k) {
+        const uint32_t go = bt + (uint32_t)k * 32u;  // every second group: 32 columns = 512 B
+        wgmma_m64n16k16<0>(acc[k], al, mk_desc(bh0 + go));
+        wgmma_m64n16k16<0>(acc[k], ah, mk_desc(bl0 + go));
+        wgmma_m64n16k16<0>(acc[k], ah, mk_desc(bh0 + go));
+      }
+    }
+    wgmma_commit();
+    // keep this K-step's group in flight; the previous one has completed, so its ring stage can be refilled
+    wgmma_wait<1>();
+    if (ring && prev_stg >= 0 && wl == 0 && lane == 0) mbar_arrive(&bars[LB_BEMPTY + prev_stg]);
+    prev_stg = stg;
+    if (ring) ++gchunk;
+  }
+  wgmma_wait<0>();
+  if (ring && prev_stg >= 0 && wl == 0 && lane == 0) mbar_arrive(&bars[LB_BEMPTY + prev_stg]);
+  // fragment -> accumulator tile: acc[k][4j + 2h + e] = row 16 wl + lane / 4 + 8h, column 16 g + 8j + 2 (lane % 4) + e
+  const int pitch = ly_acc_pitch(N);
+  const int r0 = rh * 64 + wl * 16 + (lane >> 2);
+#pragma unroll
+  for (int k = 0; k < NGW; ++k) {
+    const int g = gh + 2 * k;
+    if (16 * g < N) {
+      const int col = g * 16 + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float2*>(s_acc + (r0 + 8 * h) * pitch + col + 8 * j) =
+              make_float2(acc[k][4 * j + 2 * h], acc[k][4 * j + 2 * h + 1]);
+    }
+  }
+}
+
+// NGW: 16-column groups per warpgroup of the stage, ceil(N / 32).  FUSED: the whole step of a one-hidden-layer stack in one
+// launch (NGW covers both stages), tiles of TS = TC_TILE - MIR output slots whose 128 hidden rows overlap the next tile's.
+template <bool PADW, int MODE, int NLT, int NGW, bool FUSED>
 __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_constant__ IafLyParams q) {
   const IafTcParams& p = q.t;
-  const int HW = THW ? THW : p.HW;
+  const int HW = p.HW;
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t bars[LB_COUNT];
-  __shared__ uint32_t s_tmem;
   TL_DECL
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const IafTcStage& St = p.st[0];
-  const int nchunk = St.cin >> 3;
+  const IafTcStage& St0 = p.st[0];
+  const int nchunk = St0.cin >> 3;
   const int a_plane = p.WIN * 16;          // bytes per chunk plane of the A window
   const int a_lo_off = nchunk * a_plane;
-  // tiles of this CTA: u = blockIdx.x + i * gridDim.x.  All CTAs of a cluster run the same number of iterations (the
-  // weight ring is shared); iterations whose tile index is past the end are "virtual": they consume the weight
-  // stream but load, compute and store nothing real.
-  const int cs = q.cs;
-  const int crank = cs > 1 ? (int)cluster_ctarank() : 0;
-  const int cfirst = (int)blockIdx.x - crank;  // first CTA of my cluster
-  const int n_my = (p.NT - cfirst + (int)gridDim.x - 1) / (int)gridDim.x;
-  const uint16_t cmask = (uint16_t)((1u << cs) - 1u);
-  const int acc_cols = q.merged ? 2 * St.N : St.N;
-  const bool resident = q.n_bchunks <= q.NB;
+  // tiles of this CTA: u = blockIdx.x + i * gridDim.x
+  const int n_my = (p.NT - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  const bool resident = FUSED || q.n_bchunks <= q.NB;
 
-  // programmatic dependent launch (see iaf_tc_kernel): everything up to the barrier init overlaps the previous grid
+  // programmatic dependent launch: everything up to the barrier init overlaps the previous grid
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  if (warp == LY_MMA_WARP) {
-    tmem_alloc(&s_tmem, (uint32_t)p.tmem_cols);
+  if (warp == LY_TMA_WARP) {
     if (lane == 0) {
-      for (int i = 0; i < LY_MAX_KS; ++i) {
-        mbar_init(&bars[LB_AFULL + i], q.in_mode ? 1 : LY_WORKERS);
-        mbar_init(&bars[LB_AEMPTY + i], 1);
-      }
       for (int i = 0; i < 2; ++i) {
-        mbar_init(&bars[LB_ACC_FULL + i], 1);
-        mbar_init(&bars[LB_ACC_EMPTY + i], LY_WORKERS);
         mbar_init(&bars[LB_PART + i], LY_WORKERS);
         mbar_init(&bars[LB_PART_EMPTY + i], 1);
       }
       for (int i = 0; i < LY_MAX_NB; ++i) {
         mbar_init(&bars[LB_BFULL + i], 1);
-        mbar_init(&bars[LB_BEMPTY + i], (uint32_t)q.cs);  // every member of the cluster releases the stage
+        mbar_init(&bars[LB_BEMPTY + i], LY_WORKERS / 4);  // every worker warpgroup releases the stage
       }
       fence_barrier_init();
     }
   } else if (warp < LY_WORKERS) {
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    float* tb = reinterpret_cast<float*>(smem + q.sm_bias);
-    for (int i = tid; i < 5 * St.N; i += LY_WTHREADS) {
-      float v = 0.f;
-      if (i < St.N) v = __ldg(St.bias + i);
-      else if (PADW) v = __ldg(St.padw + (i - St.N));
-      tb[i] = v;
+    for (int s = 0; s < (FUSED ? 2 : 1); ++s) {
+      const IafTcStage& S = p.st[s];
+      float* tb = reinterpret_cast<float*>(smem + (s ? q.sm_bias1 : q.sm_bias));
+      for (int i = tid; i < 5 * S.N; i += LY_WTHREADS) {
+        float v = 0.f;
+        if (i < S.N) v = __ldg(S.bias + i);
+        else if (PADW) v = __ldg(S.padw + (i - S.N));
+        tb[i] = v;
+      }
     }
   }
-  if (warp >= LY_WORKERS) asm volatile("griddepcontrol.wait;" ::: "memory");  // producer / MMA / reducer warps
-  tc_fence_before();
+  if (warp >= LY_WORKERS) asm volatile("griddepcontrol.wait;" ::: "memory");  // producer / reducer warps
   __syncthreads();
-  tc_fence_after();
-  if (cs > 1) cluster_sync_all();  // every member's barriers are initialised before any remote signal can arrive
-  const uint32_t tmem_base = s_tmem;
 
   if (warp == LY_TMA_WARP) {
     // ===================== producer: A windows (operand-image input) and the weight ring =====================
-    if (lane == 0) {
+    if (lane == 0 && FUSED) {
+      // both stages' weights, resident: hidden chunk c behind barrier c, heads chunk c behind barrier n_bchunks + c
+      for (int s = 0; s < 2; ++s) {
+        const IafTcStage& S = p.st[s];
+        const int nb = s ? q.n_bchunks1 : q.n_bchunks, bcb = s ? q.b_chunk_bytes1 : q.b_chunk_bytes;
+        uint8_t* base = smem + (s ? q.sm_b1 : q.sm_b);
+        for (int c = 0; c < nb; ++c) {
+          uint64_t* bar = &bars[LB_BFULL + (s ? q.n_bchunks : 0) + c];
+          const size_t bo = (size_t)c * bcb;
+          mbar_expect_tx(bar, (uint32_t)(2 * bcb));
+          bulk_g2s(base + 2 * c * bcb, reinterpret_cast<const uint8_t*>(S.whi) + bo, (uint32_t)bcb, bar);
+          bulk_g2s(base + 2 * c * bcb + bcb, reinterpret_cast<const uint8_t*>(S.wlo) + bo, (uint32_t)bcb, bar);
+        }
+      }
+    } else if (lane == 0) {
       int gchunk = 0;
-      LPROBE_DECL
       for (int i = 0; i < n_my; ++i) {
         const int u = (int)blockIdx.x + i * (int)gridDim.x;
         // K order is [K-step within a tap][tap]: weight chunk c and A chunk pair (2c, 2c+1) are consumed together,
@@ -192,492 +241,337 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
           if (resident && i >= 1 && !q.in_mode) continue;  // weights already resident, A comes from the workers
           const int stg = gchunk % q.NB;
           const int use = gchunk / q.NB;
-          LPROBE(1)
           if (use >= 1) mbar_wait(&bars[LB_BEMPTY + stg], (uint32_t)((use - 1) & 1));
-          LPROBE(0)
           uint8_t* dst = smem + q.sm_b + stg * q.stage_bytes;
           const size_t bo = (size_t)c * q.b_chunk_bytes;
-          const bool real = u < p.NT;
           if (q.in_mode) {
             // one ring stage = A chunk pair (hi c0, hi c1, lo c0, lo c1) + the weight chunk (hi, lo) of K-step c
-            mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)((real ? 4 * a_plane : 0) + 2 * q.b_chunk_bytes));
-            if (real) {
+            mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)(4 * a_plane + 2 * q.b_chunk_bytes));
 #pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const size_t go = ((size_t)(2 * c + h) * q.S_pad + (size_t)u * TC_TILE) * 8;
-                bulk_g2s(dst + h * a_plane, q.a_hi + go, (uint32_t)a_plane, &bars[LB_BFULL + stg]);
-                bulk_g2s(dst + (2 + h) * a_plane, q.a_lo + go, (uint32_t)a_plane, &bars[LB_BFULL + stg]);
-              }
+            for (int h = 0; h < 2; ++h) {
+              const size_t go = ((size_t)(2 * c + h) * q.S_pad + (size_t)u * TC_TILE) * 8;
+              bulk_g2s(dst + h * a_plane, q.a_hi + go, (uint32_t)a_plane, &bars[LB_BFULL + stg]);
+              bulk_g2s(dst + (2 + h) * a_plane, q.a_lo + go, (uint32_t)a_plane, &bars[LB_BFULL + stg]);
             }
             dst += 4 * a_plane;
           } else {
             mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)(2 * q.b_chunk_bytes));
           }
-          if (q.merged) {
-            // interleaved image: the [hi | lo] planes of K-step c are one contiguous run of 2 * b_chunk_bytes
-            const uint8_t* src = reinterpret_cast<const uint8_t*>(St.whi) + 2 * bo;
-            if (cs == 1) {
-              bulk_g2s(dst, src, (uint32_t)q.b_chunk_bytes, &bars[LB_BFULL + stg]);
-              bulk_g2s(dst + q.b_chunk_bytes, src + q.b_chunk_bytes, (uint32_t)q.b_chunk_bytes, &bars[LB_BFULL + stg]);
-            } else {
-              const int slice = 2 * q.b_chunk_bytes / cs;
-              bulk_g2s_mcast(dst + crank * slice, src + crank * slice, (uint32_t)slice, &bars[LB_BFULL + stg], cmask);
-            }
-          } else if (cs == 1) {
-            bulk_g2s(dst, reinterpret_cast<const uint8_t*>(St.whi) + bo, (uint32_t)q.b_chunk_bytes, &bars[LB_BFULL + stg]);
-            bulk_g2s(dst + q.b_chunk_bytes, reinterpret_cast<const uint8_t*>(St.wlo) + bo, (uint32_t)q.b_chunk_bytes,
-                     &bars[LB_BFULL + stg]);
-          } else {
-            // my 1/cs slice of the stage's [hi | lo] weight bytes, multicast into every member's stage
-            const int slice = 2 * q.b_chunk_bytes / cs;
-            const int so = crank * slice;
-            const uint8_t* src = so < q.b_chunk_bytes ? reinterpret_cast<const uint8_t*>(St.whi) + bo + so
-                                                      : reinterpret_cast<const uint8_t*>(St.wlo) + bo + (so - q.b_chunk_bytes);
-            bulk_g2s_mcast(dst + so, src, (uint32_t)slice, &bars[LB_BFULL + stg], cmask);
-          }
+          bulk_g2s(dst, reinterpret_cast<const uint8_t*>(St0.whi) + bo, (uint32_t)q.b_chunk_bytes, &bars[LB_BFULL + stg]);
+          bulk_g2s(dst + q.b_chunk_bytes, reinterpret_cast<const uint8_t*>(St0.wlo) + bo, (uint32_t)q.b_chunk_bytes,
+                   &bars[LB_BFULL + stg]);
           ++gchunk;
         }
       }
-      LPROBE(1)
-      LPROBE_DUMP(0)
     }
     __syncwarp();
-  } else if (warp == LY_MMA_WARP) {
-    // ===================== MMA issue (convergent warp, one elected lane) =====================
-    const uint32_t idesc = umma_idesc(St.N);
-    const uint32_t idesc2 = umma_idesc(2 * St.N);   // merged form only (2N <= 256 checked by the host layout)
-    const uint32_t a_base = smem_u32(smem + q.sm_a);
-    const uint32_t b_plane = (uint32_t)St.N * 16u * (q.merged ? 2u : 1u);
-    // slot shifts of the taps (0,0) (0,+1) (+1,-1) (+1,0) (+1,+1), in 16-byte descriptor units
-    const uint32_t sh1 = 1u, sh2 = (uint32_t)(p.Wp - 1), sh3 = (uint32_t)p.Wp, sh4 = (uint32_t)(p.Wp + 1);
-    const uint32_t a_kstep = (2u * (uint32_t)a_plane) >> 4, b_tstep = (2u * b_plane) >> 4;
-    const uint32_t ah_base = umma_desc_lo(a_base, (uint32_t)a_plane);
-    const uint32_t al_base = umma_desc_lo(a_base + (uint32_t)a_lo_off, (uint32_t)a_plane);
-    int gchunk = 0;
-    LPROBE_DECL
-    for (int i = 0; i < n_my; ++i) {
-      const int b = i & 1, use = i >> 1;
-      LPROBE(3)
-      if (use >= 1) mbar_wait(&bars[LB_ACC_EMPTY + b], (uint32_t)((use - 1) & 1));
-      LPROBE(0)
-      tc_fence_after();
-      if (lane == 0) TL(0, 100, i);
-      const uint32_t d_tmem = tmem_base + (uint32_t)(b * acc_cols);
-      for (int c = 0; c < q.n_bchunks; ++c) {
-        const bool res = resident && !q.in_mode;
-        const int stg = res ? c : gchunk % q.NB;
-        LPROBE(3)
-        if (!q.in_mode) mbar_wait(&bars[LB_AFULL + c], (uint32_t)(i & 1));
-        LPROBE(1)
-        mbar_wait(&bars[LB_BFULL + stg], res ? 0u : (uint32_t)((gchunk / q.NB) & 1));
-        LPROBE(2)
-        tc_fence_after();
-        const uint32_t sbase = smem_u32(smem + q.sm_b + stg * q.stage_bytes);
-        uint32_t ah0, al0, bbase;
-        if (q.in_mode) {  // operands of this K-step both live in the ring stage
-          ah0 = umma_desc_lo(sbase, (uint32_t)a_plane);
-          al0 = umma_desc_lo(sbase + 2u * (uint32_t)a_plane, (uint32_t)a_plane);
-          bbase = sbase + 4u * (uint32_t)a_plane;
-        } else {
-          ah0 = ah_base + (uint32_t)c * a_kstep;
-          al0 = al_base + (uint32_t)c * a_kstep;
-          bbase = sbase;
-        }
-        const uint32_t bh0 = umma_desc_lo(bbase, b_plane);
-        const uint32_t bl0 = umma_desc_lo(bbase + (uint32_t)q.b_chunk_bytes, b_plane);
-        const uint32_t acc0 = c ? 1u : 0u;
-        if (elect_one_sync()) {
-#define LY_TAP(T, SH, ACC)                                                                   \
-          umma_f16(d_tmem, mk_desc(al0 + (SH)), mk_desc(bh0 + (T) * b_tstep), idesc, (ACC)); \
-          umma_f16(d_tmem, mk_desc(ah0 + (SH)), mk_desc(bl0 + (T) * b_tstep), idesc, 1u);    \
-          umma_f16(d_tmem, mk_desc(ah0 + (SH)), mk_desc(bh0 + (T) * b_tstep), idesc, 1u);
-#define LY_TAP_C(T, SH, ACC)                                                                       \
-          umma_f16(d_tmem, mk_desc(al0 + (SH)), mk_desc(bh0 + (T) * b_tstep), idesc, (ACC));       \
-          umma_f16_afill(d_tmem, mk_desc(ah0 + (SH)), mk_desc(bl0 + (T) * b_tstep), idesc, 1u);    \
-          umma_f16_alast(d_tmem, mk_desc(ah0 + (SH)), mk_desc(bh0 + (T) * b_tstep), idesc, 1u);
-#define LY_TAP_M(T, SH, ACC)                                                                  \
-          umma_f16(d_tmem, mk_desc(ah0 + (SH)), mk_desc(bh0 + (T) * b_tstep), idesc2, (ACC)); \
-          umma_f16(d_tmem, mk_desc(al0 + (SH)), mk_desc(bh0 + (T) * b_tstep), idesc, 1u);
-          if (q.merged) {  // hi * [hi | lo] in one instruction (columns [N, 2N) collect hi * lo), then lo * hi
-            LY_TAP_M(0u, 0u, acc0)
-            LY_TAP_M(1u, sh1, 1u)
-            LY_TAP_M(2u, sh2, 1u)
-            LY_TAP_M(3u, sh3, 1u)
-            LY_TAP_M(4u, sh4, 1u)
-          } else if (q.collector) {
-            LY_TAP_C(0u, 0u, acc0)
-            LY_TAP_C(1u, sh1, 1u)
-            LY_TAP_C(2u, sh2, 1u)
-            LY_TAP_C(3u, sh3, 1u)
-            LY_TAP_C(4u, sh4, 1u)
-          } else {
-            LY_TAP(0u, 0u, acc0)
-            LY_TAP(1u, sh1, 1u)
-            LY_TAP(2u, sh2, 1u)
-            LY_TAP(3u, sh3, 1u)
-            LY_TAP(4u, sh4, 1u)
-          }
-#undef LY_TAP
-#undef LY_TAP_C
-#undef LY_TAP_M
-          if (!res) {
-            if (cs == 1) umma_commit(&bars[LB_BEMPTY + stg]);
-            else umma_commit_mcast(&bars[LB_BEMPTY + stg], cmask);
-          }
-          if (!q.in_mode) umma_commit(&bars[LB_AEMPTY + c]);
-          if (c == q.n_bchunks - 1) {
-            umma_commit(&bars[LB_ACC_FULL + b]);
-            TL(0, 200, i);
-          }
-        }
-        __syncwarp();
-        if (!res) ++gchunk;
-      }
-    }
-    LPROBE(3)
-    LPROBE_DUMP(1)
   } else if (warp < LY_WORKERS) {
-    // ===================== workers: (first stage) z -> operand window; epilogues =====================
+    // ===================== workers: (first stage) z -> operand window; MMAs; epilogues =====================
     const int qd = warp & 3, cg = warp >> 2;
     constexpr int CGS = LY_WORKERS / 4;
     const int sl = qd * 32 + lane;
-    const uint32_t t_lane = tmem_base + ((uint32_t)(qd * 32) << 16);
-    const float* tb = reinterpret_cast<const float*>(smem + q.sm_bias);
     float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
-    const int ngroups = St.N >> 4;
+    float* s_acc = reinterpret_cast<float*>(smem + q.sm_acc);
+    // this thread's slot row of the accumulator tile, 16 columns from c0
+    auto acc_ld16 = [&](int c0, uint32_t* r, int pitch) {
+      const float4* s4 = reinterpret_cast<const float4*>(s_acc + sl * pitch + c0);
+#pragma unroll
+      for (int e4 = 0; e4 < 4; ++e4) {
+        const float4 v4 = s4[e4];
+        r[4 * e4] = __float_as_uint(v4.x); r[4 * e4 + 1] = __float_as_uint(v4.y);
+        r[4 * e4 + 2] = __float_as_uint(v4.z); r[4 * e4 + 3] = __float_as_uint(v4.w);
+      }
+    };
+    const int h_plane = (TC_TILE + p.MIR) * 16;  // fused: bytes per chunk plane of the hidden operand buffer
 
-    auto load_window = [&](int i) {  // fp32 z -> bf16 hi/lo A window of this CTA's i-th tile
+    auto load_window = [&](int i) {  // fp32 z -> fp16 hi/lo A window of this CTA's i-th tile
       const int u = (int)blockIdx.x + i * (int)gridDim.x;
-      float v[TC_ZITEMS][8];
-      int dsto[TC_ZITEMS];
 #pragma unroll
       for (int it = 0; it < TC_ZITEMS; ++it) {
         const int idx = tid + it * LY_WTHREADS;
-        dsto[it] = -1;
         if (idx < p.WIN * nchunk) {
           const int ch = fast_div(idx, p.WIN, p.mg_win);
           const int s_ = idx - ch * p.WIN;
-          dsto[it] = ch * a_plane + s_ * 16;
-          const SlotInfo si = decode_slot(p, u * TC_TILE + s_, HW);
+          const SlotInfo si = decode_slot(p, u * q.TS + s_, HW);
+          float v[8];
 #pragma unroll
-          for (int e = 0; e < 8; ++e) v[it][e] = 0.f;
+          for (int e = 0; e < 8; ++e) v[e] = 0.f;
           if (si.valid) {
             const size_t g = ((size_t)si.n * p.C + ch * 8) * HW + si.gp;
 #pragma unroll
-            for (int e = 0; e < 8; ++e) v[it][e] = __ldg(p.z + g + (size_t)e * HW);
+            for (int e = 0; e < 8; ++e) v[e] = __ldg(p.z + g + (size_t)e * HW);
             if (MODE == IAF_MODE_LAYER) {
 #pragma unroll
               for (int e = 0; e < 8; ++e)
-                v[it][e] = fmaf(fast_exp(__ldg(p.post_logsd + g + (size_t)e * HW)), v[it][e],
-                                __ldg(p.post_mean + g + (size_t)e * HW));
+                v[e] = fmaf(fast_exp(__ldg(p.post_logsd + g + (size_t)e * HW)), v[e], __ldg(p.post_mean + g + (size_t)e * HW));
             }
           }
+          uint8_t* dst = smem + q.sm_a + ch * a_plane + s_ * 16;
+          split_store8(v, dst, dst + a_lo_off);
         }
       }
-      if (warp == 0 && lane == 0) TL(1, 30, i);
-      if (i >= 1) mbar_wait(&bars[LB_AEMPTY + q.n_bchunks - 1], (uint32_t)((i - 1) & 1));  // commits are in order
-      if (warp == 0 && lane == 0) TL(1, 31, i);
-#pragma unroll
-      for (int it = 0; it < TC_ZITEMS; ++it) {
-        if (dsto[it] >= 0) {
-          uint8_t* dst = smem + q.sm_a + dsto[it];
-          split_store8(v[it], dst, dst + a_lo_off);
-        }
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0)
-        for (int c = 0; c < q.n_bchunks; ++c) mbar_arrive(&bars[LB_AFULL + c]);
+      fence_proxy_async();  // generic-proxy stores -> the wgmma (async proxy) reads of the window
     };
 
-    LPROBE_DECL
-    if (!q.in_mode && n_my > 0) load_window(0);
+    int gchunk = 0;
     for (int i = 0; i < n_my; ++i) {
-      LPROBE(2)
-      if (!q.in_mode && i + 1 < n_my) load_window(i + 1);
-      LPROBE(3)
       const int u = (int)blockIdx.x + i * (int)gridDim.x;
-      const int b = i & 1, use = i >> 1;
-      const SlotInfo si = decode_slot(p, u * TC_TILE + sl, HW);
-      const bool bx0 = (si.x == 0), bxW = (si.x == p.W - 1), byH = (si.y == p.H - 1);
-      const uint32_t t_acc = t_lane + (uint32_t)(b * acc_cols);
+      // the previous tile's epilogue is done with the accumulator tile and its MMAs with the A window
+      worker_bar_sync();
+      if (!q.in_mode) {
+        load_window(i);
+        worker_bar_sync();
+      }
       if (warp == 0 && lane == 0) TL(1, 10, i);
+      ly_mma_tile<NGW>(smem, bars, s_acc, St0.N, q.n_bchunks, !resident || q.in_mode, q.NB, gchunk, LB_BFULL,
+                       smem_u32(smem + q.sm_b), (uint32_t)(FUSED ? 2 * q.b_chunk_bytes : q.stage_bytes),
+                       (uint32_t)q.b_chunk_bytes, q.in_mode != 0, smem_u32(smem + q.sm_a), (uint32_t)a_plane,
+                       (uint32_t)a_lo_off, p.Wp);
+      worker_bar_sync();
+      if (warp == 0 && lane == 0) TL(1, 50, i);
+      const SlotInfo si_all = decode_slot(p, u * q.TS + sl, HW);
+      const bool bx0 = (si_all.x == 0), bxW = (si_all.x == p.W - 1), byH = (si_all.y == p.H - 1);
 
-      if (!q.is_heads) {
-        bool waited = false;
-        // context of the NEXT column group is fetched while the current one is computed
-        float cxn[16];
-        auto fetch_ctx = [&](int g) {
-          if (q.first && si.valid && g < ngroups) {  // += context   (ar.py:402 / layers.py:163)
-            const float* cp = p.ctx + ((size_t)si.n * St.N + g * 16) * HW + si.gp;
-#pragma unroll
-            for (int e = 0; e < 16; ++e) cxn[e] = __ldg(cp + (size_t)e * HW);
+      // hidden stage epilogue: the next operand (global image, or the fused kernel's shared-memory buffer)
+      auto hidden_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch, const SlotInfo si) {
+        auto store_operand = [&](const float* v8, int chunk) {
+          if (FUSED) {
+            uint8_t* dst = smem + q.sm_h + chunk * h_plane + sl * 16;
+            split_store8(v8, dst, dst + (St.N >> 3) * h_plane);
           } else {
-#pragma unroll
-            for (int e = 0; e < 16; ++e) cxn[e] = 0.f;
+            const size_t go = ((size_t)chunk * q.S_pad + (size_t)u * TC_TILE + sl) * 8;
+            split_store8(v8, reinterpret_cast<uint8_t*>(q.o_hi + go), reinterpret_cast<uint8_t*>(q.o_lo + go));
           }
         };
-        fetch_ctx(cg);
-        for (int g = cg; g < ngroups; g += CGS) {
-          const int c0 = g * 16;
-          float cx[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) cx[e] = cxn[e];
-          fetch_ctx(g + CGS);
-          if (!waited) {
-            LPROBE(1)
-            mbar_wait(&bars[LB_ACC_FULL + b], (uint32_t)(use & 1));
-            tc_fence_after();
-            LPROBE(0)
-            waited = true;
-            if (warp == 0 && lane == 0) TL(1, 50, i);
-          }
-          uint32_t r[16];
-          tmem_ld16(t_acc + (uint32_t)c0, r);
-          tmem_ld_wait();
-          if (q.bwd) {
-            // data gradient: acc = W^T g (scaled units); x nl'(h), evaluated from the activation itself
-            const float sc = si.valid ? dg_scale_from_amax(__ldg(q.amax + si.n)) : 1.0f;
-            const float inv = 1.0f / sc;
-            float vb[16];
-#pragma unroll
-            for (int e = 0; e < 16; ++e) {
-              const float a = __uint_as_float(r[e]);
-              const float d = (q.bwd == 1) ? dg_nl_grad(cx[e], p.nl) : 1.0f;
-              vb[e] = si.valid ? a * d : 0.f;
+          // context of the NEXT column group is fetched while the current one is computed
+          float cxn[16];
+          auto fetch_ctx = [&](int g) {
+            if (q.first && si.valid && g < ngroups) {  // += context   (ar.py:402 / layers.py:163)
+              const float* cp = p.ctx + ((size_t)si.n * St.N + g * 16) * HW + si.gp;
+  #pragma unroll
+              for (int e = 0; e < 16; ++e) cxn[e] = __ldg(cp + (size_t)e * HW);
+            } else {
+  #pragma unroll
+              for (int e = 0; e < 16; ++e) cxn[e] = 0.f;
             }
-            if (St.hid_out && si.valid && u < p.NT) {
-              float* hp = St.hid_out + ((size_t)si.n * St.N + c0) * HW + si.gp;
-              if (q.bwd == 2) {
-#pragma unroll
-                for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] += vb[e] * inv;
-              } else {
-#pragma unroll
-                for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] = vb[e] * inv;
+          };
+          fetch_ctx(cg);
+          for (int g = cg; g < ngroups; g += CGS) {
+            const int c0 = g * 16;
+            float cx[16];
+  #pragma unroll
+            for (int e = 0; e < 16; ++e) cx[e] = cxn[e];
+            fetch_ctx(g + CGS);
+            uint32_t r[16];
+            acc_ld16(c0, r, pitch);
+            if (q.bwd) {
+              // data gradient: acc = W^T g (scaled units); x nl'(h), evaluated from the activation itself
+              const float sc = si.valid ? dg_scale_from_amax(__ldg(q.amax + si.n)) : 1.0f;
+              const float inv = 1.0f / sc;
+              float vb[16];
+  #pragma unroll
+              for (int e = 0; e < 16; ++e) {
+                const float a = __uint_as_float(r[e]);
+                const float d = (q.bwd == 1) ? dg_nl_grad(cx[e], p.nl) : 1.0f;
+                vb[e] = si.valid ? a * d : 0.f;
               }
-            }
-            if (u < p.NT && q.o_hi) {
-#pragma unroll
-              for (int hch = 0; hch < 2; ++hch) {
-                const size_t go = (((size_t)((c0 >> 3) + hch)) * q.S_pad + (size_t)u * TC_TILE + sl) * 8;
-                split_store8(vb + 8 * hch, reinterpret_cast<uint8_t*>(q.o_hi + go), reinterpret_cast<uint8_t*>(q.o_lo + go));
-              }
-            }
-            continue;
-          }
-#ifdef TC_FAST_EPI
-          float v[16];
-          if (NLT == IAF_NL_ELU && !PADW) {  // packed-pair arithmetic, see iaf_tc_kernel
-            const float4* tb4 = reinterpret_cast<const float4*>(tb + c0);
-            const float validf = si.valid ? 1.f : 0.f;
-#pragma unroll
-            for (int e4 = 0; e4 < 4; ++e4) {
-              const float4 t4 = tb4[e4];
-              const float bs[4] = {t4.x, t4.y, t4.z, t4.w};
-#pragma unroll
-              for (int h2 = 0; h2 < 2; ++h2) {
-                const int e = 4 * e4 + 2 * h2;
-                float a0 = __uint_as_float(r[e]), a1 = __uint_as_float(r[e + 1]);
-                add2(a0, a1, bs[2 * h2], bs[2 * h2 + 1]);
-                add2(a0, a1, cx[e], cx[e + 1]);
-                float t0 = fminf(a0, 0.f), t1 = fminf(a1, 0.f);
-                mul2(t0, t1, 1.4426950408889634f, 1.4426950408889634f);
-                t0 = ex2_approx(t0); t1 = ex2_approx(t1);
-                add2(t0, t1, -1.0f, -1.0f);
-                float o0 = fmaxf(a0, t0), o1 = fmaxf(a1, t1);
-                mul2(o0, o1, validf, validf);
-                v[e] = o0; v[e + 1] = o1;
-              }
-            }
-          } else
-#else
-          float v[16];
-#endif
-          {
-            // branch-free: bias rows come in as 16-byte vectors, the pad-channel terms (conv.py:77-83: the pad
-            // channel is 1 where a tap falls outside the image) are 0/1-weighted FMAs, and an invalid slot
-            // (pad column, zero row, past the end) is multiplied to zero: that zero IS the conv's padding
-            const float4* tb4 = reinterpret_cast<const float4*>(tb + c0);
-            float bsv[16];
-#pragma unroll
-            for (int e4 = 0; e4 < 4; ++e4) {
-              const float4 t4 = tb4[e4];
-              bsv[4 * e4] = t4.x; bsv[4 * e4 + 1] = t4.y; bsv[4 * e4 + 2] = t4.z; bsv[4 * e4 + 3] = t4.w;
-            }
-            if (PADW) {
-              const float f1 = bxW ? 1.f : 0.f, f2 = (byH || bx0) ? 1.f : 0.f, f3 = byH ? 1.f : 0.f,
-                          f4 = (byH || bxW) ? 1.f : 0.f;
-#pragma unroll
-              for (int e = 0; e < 16; ++e)
-                bsv[e] += f1 * tb[St.N + c0 + e] + f2 * tb[2 * St.N + c0 + e] + f3 * tb[3 * St.N + c0 + e] +
-                          f4 * tb[4 * St.N + c0 + e];
-            }
-            const float validf = si.valid ? 1.f : 0.f;
-#pragma unroll
-            for (int e = 0; e < 16; ++e) {
-              const float a = __uint_as_float(r[e]) + bsv[e] + cx[e];
-              float o;
-              if (NLT == IAF_NL_ELU) {
-                const float ex = fast_exp(fminf(a, 0.f)) - 1.0f;  // elu, exp always evaluated: no divergence
-                o = a < 0.f ? ex : a;
-              } else {
-                o = tc_apply_nl<NLT>(a, p.nl);
-              }
-              v[e] = o * validf;
-            }
-          }
-          if (St.hid_out && si.valid && u < p.NT) {  // training forward: keep the activations for iaf_step_bwd_saved
-            float* hp = St.hid_out + ((size_t)si.n * St.N + c0) * HW + si.gp;
-#pragma unroll
-            for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] = v[e];
-          }
-          if (u < p.NT) {
-#pragma unroll
-            for (int hch = 0; hch < 2; ++hch) {
-              const size_t go = (((size_t)((c0 >> 3) + hch)) * q.S_pad + (size_t)u * TC_TILE + sl) * 8;
-              split_store8(v + 8 * hch, reinterpret_cast<uint8_t*>(q.o_hi + go), reinterpret_cast<uint8_t*>(q.o_lo + go));
-            }
-          }
-        }
-        if (!waited) mbar_wait(&bars[LB_ACC_FULL + b], (uint32_t)(use & 1));
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars[LB_ACC_EMPTY + b]);
-        if (warp == 0 && lane == 0) TL(1, 20, i);
-      } else {
-        // ---------------- heads: identical arithmetic to iaf_tc_kernel's last stage ----------------
-        constexpr int NRED = (MODE == IAF_MODE_LAYER) ? 8 : 1;
-        float red[NRED];
-#pragma unroll
-        for (int k_ = 0; k_ < NRED; ++k_) red[k_] = 0.f;
-        const int tile_s0 = u * TC_TILE;
-        const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
-        const int n_last = min(p.B - 1, fast_div(tile_s0 + TC_TILE - 1, p.SPS, p.mg_sps));
-        const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
-        const int pb = i & 1;
-        if (MODE == IAF_MODE_LAYER && (p.persample_out || p.bc_out) && i >= 2)
-          mbar_wait(&bars[LB_PART_EMPTY + pb], (uint32_t)(((i >> 1) - 1) & 1));
-        bool waited = false;
-        for (int g = cg; g < ngroups; g += CGS) {
-          const int c0 = g * 16;
-          const int ch0 = g * 8;
-          float zv[8];
-          size_t gi = 0;
-          if (si.valid) {
-            gi = ((size_t)si.n * p.C + ch0) * HW + si.gp;
-#pragma unroll
-            for (int e = 0; e < 8; ++e) zv[e] = __ldg(p.z + gi + (size_t)e * HW);
-          }
-          if (!waited) {
-            LPROBE(1)
-            mbar_wait(&bars[LB_ACC_FULL + b], (uint32_t)(use & 1));
-            tc_fence_after();
-            LPROBE(0)
-            waited = true;
-            if (warp == 0 && lane == 0) TL(1, 50, i);
-          }
-          uint32_t r[16];
-          tmem_ld16(t_acc + (uint32_t)c0, r);
-          if (q.merged) {  // the hi * lo partial products sit in columns [N, 2N)
-            uint32_t r2[16];
-            tmem_ld16(t_acc + (uint32_t)(St.N + c0), r2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) + __uint_as_float(r2[e]));
-          } else {
-            tmem_ld_wait();
-          }
-          if (MODE == IAF_MODE_LAYER) {
-#pragma unroll
-            for (int k_ = 0; k_ < NRED; ++k_) red[k_] = 0.f;
-          }
-          if (si.valid) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              float m = __uint_as_float(r[e]) + tb[c0 + e];
-              float sv = __uint_as_float(r[8 + e]) + tb[c0 + 8 + e];
-              if (PADW) {
-                if (bxW) { m += tb[St.N + c0 + e]; sv += tb[St.N + c0 + 8 + e]; }
-                if (byH || bx0) { m += tb[2 * St.N + c0 + e]; sv += tb[2 * St.N + c0 + 8 + e]; }
-                if (byH) { m += tb[3 * St.N + c0 + e]; sv += tb[3 * St.N + c0 + 8 + e]; }
-                if (byH || bxW) { m += tb[4 * St.N + c0 + e]; sv += tb[4 * St.N + c0 + 8 + e]; }
-              }
-              if (MODE == IAF_MODE_MULTICONV) {  // the un-fused operator: raw heads (ar.py:405-411 / layers.py:166)
-                  p.z_out[gi + (size_t)e * HW] = m;
-                  p.elem[gi + (size_t)e * HW] = sv;
-                  continue;
+              if (St.hid_out && si.valid && sl < q.TO && u < p.NT) {
+                float* hp = St.hid_out + ((size_t)si.n * St.N + c0) * HW + si.gp;
+                if (q.bwd == 2) {
+  #pragma unroll
+                  for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] += vb[e] * inv;
+                } else {
+  #pragma unroll
+                  for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] = vb[e] * inv;
                 }
-                const float arw_mean = p.scale * m, arw_logsd = p.scale * sv;  // models.py:282-285
-              const size_t ge = gi + (size_t)e * HW;
-              float z0 = zv[e];
-              float eps = 0.f, pls = 0.f;
-              if (MODE == IAF_MODE_LAYER) {
-                eps = z0;
-                pls = __ldg(p.post_logsd + ge);
-                z0 = fmaf(fast_exp(pls), eps, __ldg(p.post_mean + ge));
               }
-              const float zn = (z0 - arw_mean) * fast_exp(-arw_logsd);
-              p.z_out[ge] = zn;
-              if (MODE == IAF_MODE_STEP) {
-                if (p.elem) p.elem[ge] = arw_logsd;
-                red[0] += arw_logsd;
-              } else {
-                const float logqs = -0.9189385332046727f - pls - 0.5f * eps * eps + arw_logsd;
-                const float pl = __ldg(p.prior_logsd + ge);
-                const float d = zn - __ldg(p.prior_mean + ge);
-                const float logps = -0.9189385332046727f - pl - 0.5f * d * d * fast_exp(-2.0f * pl);
-                const float kl = logqs - logps;
-                if (p.elem) p.elem[ge] = kl;
-                red[e] = kl;
+              if (u < p.NT && q.o_hi) {
+  #pragma unroll
+                for (int hch = 0; hch < 2; ++hch) {
+                  store_operand(vb + 8 * hch, (c0 >> 3) + hch);
+                }
+              }
+              continue;
+            }
+            float v[16];
+            {
+              // branch-free: bias rows come in as 16-byte vectors, the pad-channel terms (conv.py:77-83: the pad
+              // channel is 1 where a tap falls outside the image) are 0/1-weighted FMAs, and an invalid slot
+              // (pad column, zero row, past the end) is multiplied to zero: that zero IS the conv's padding
+              const float4* tb4 = reinterpret_cast<const float4*>(tb + c0);
+              float bsv[16];
+  #pragma unroll
+              for (int e4 = 0; e4 < 4; ++e4) {
+                const float4 t4 = tb4[e4];
+                bsv[4 * e4] = t4.x; bsv[4 * e4 + 1] = t4.y; bsv[4 * e4 + 2] = t4.z; bsv[4 * e4 + 3] = t4.w;
+              }
+              if (PADW) {
+                const float f1 = bxW ? 1.f : 0.f, f2 = (byH || bx0) ? 1.f : 0.f, f3 = byH ? 1.f : 0.f,
+                            f4 = (byH || bxW) ? 1.f : 0.f;
+  #pragma unroll
+                for (int e = 0; e < 16; ++e)
+                  bsv[e] += f1 * tb[St.N + c0 + e] + f2 * tb[2 * St.N + c0 + e] + f3 * tb[3 * St.N + c0 + e] +
+                            f4 * tb[4 * St.N + c0 + e];
+              }
+              const float validf = si.valid ? 1.f : 0.f;
+  #pragma unroll
+              for (int e = 0; e < 16; ++e) {
+                const float a = __uint_as_float(r[e]) + bsv[e] + cx[e];
+                float o;
+                if (NLT == IAF_NL_ELU) {
+                  const float ex = fast_exp(fminf(a, 0.f)) - 1.0f;  // elu, exp always evaluated: no divergence
+                  o = a < 0.f ? ex : a;
+                } else {
+                  o = tc_apply_nl<NLT>(a, p.nl);
+                }
+                v[e] = o * validf;
+              }
+            }
+            if (St.hid_out && si.valid && sl < q.TO && u < p.NT) {  // training forward: keep the activations for iaf_step_bwd_saved
+              float* hp = St.hid_out + ((size_t)si.n * St.N + c0) * HW + si.gp;
+  #pragma unroll
+              for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] = v[e];
+            }
+            if (u < p.NT) {
+  #pragma unroll
+              for (int hch = 0; hch < 2; ++hch) {
+                store_operand(v + 8 * hch, (c0 >> 3) + hch);
               }
             }
           }
-          if (MODE == IAF_MODE_LAYER) {
-            for (int nl_ = 0; nl_ < ns; ++nl_) {
-#pragma unroll
+      };
+      // heads epilogue: affine update, per-element and per-sample outputs
+      auto heads_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch, const SlotInfo si) {
+          // ---------------- heads: affine update, per-element and per-sample outputs ----------------
+          constexpr int NRED = (MODE == IAF_MODE_LAYER) ? 8 : 1;
+          float red[NRED];
+  #pragma unroll
+          for (int k_ = 0; k_ < NRED; ++k_) red[k_] = 0.f;
+          const int tile_s0 = u * q.TS;
+          const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
+          const int n_last = min(p.B - 1, fast_div(tile_s0 + q.TS - 1, p.SPS, p.mg_sps));
+          const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
+          const int pb = i & 1;
+          if (MODE == IAF_MODE_LAYER && (p.persample_out || p.bc_out) && i >= 2)
+            mbar_wait(&bars[LB_PART_EMPTY + pb], (uint32_t)(((i >> 1) - 1) & 1));
+          for (int g = cg; g < ngroups; g += CGS) {
+            const int c0 = g * 16;
+            const int ch0 = g * 8;
+            float zv[8];
+            size_t gi = 0;
+            if (si.valid) {
+              gi = ((size_t)si.n * p.C + ch0) * HW + si.gp;
+  #pragma unroll
+              for (int e = 0; e < 8; ++e) zv[e] = __ldg(p.z + gi + (size_t)e * HW);
+            }
+            uint32_t r[16];
+            acc_ld16(c0, r, pitch);
+            if (MODE == IAF_MODE_LAYER) {
+  #pragma unroll
+              for (int k_ = 0; k_ < NRED; ++k_) red[k_] = 0.f;
+            }
+            if (si.valid) {
+  #pragma unroll
               for (int e = 0; e < 8; ++e) {
-                float x = (si.valid && si.n == n_first + nl_) ? red[e] : 0.f;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-                if (lane == 0) s_part[((pb * 4 + qd) * p.MAXS + nl_) * p.C + ch0 + e] = x;
+                float m = __uint_as_float(r[e]) + tb[c0 + e];
+                float sv = __uint_as_float(r[8 + e]) + tb[c0 + 8 + e];
+                if (PADW) {
+                  if (bxW) { m += tb[St.N + c0 + e]; sv += tb[St.N + c0 + 8 + e]; }
+                  if (byH || bx0) { m += tb[2 * St.N + c0 + e]; sv += tb[2 * St.N + c0 + 8 + e]; }
+                  if (byH) { m += tb[3 * St.N + c0 + e]; sv += tb[3 * St.N + c0 + 8 + e]; }
+                  if (byH || bxW) { m += tb[4 * St.N + c0 + e]; sv += tb[4 * St.N + c0 + 8 + e]; }
+                }
+                if (MODE == IAF_MODE_MULTICONV) {  // the un-fused operator: raw heads (ar.py:405-411 / layers.py:166)
+                    p.z_out[gi + (size_t)e * HW] = m;
+                    p.elem[gi + (size_t)e * HW] = sv;
+                    continue;
+                  }
+                  const float arw_mean = p.scale * m, arw_logsd = p.scale * sv;  // models.py:282-285
+                const size_t ge = gi + (size_t)e * HW;
+                float z0 = zv[e];
+                float eps = 0.f, pls = 0.f;
+                if (MODE == IAF_MODE_LAYER) {
+                  eps = z0;
+                  pls = __ldg(p.post_logsd + ge);
+                  z0 = fmaf(fast_exp(pls), eps, __ldg(p.post_mean + ge));
+                }
+                const float zn = (z0 - arw_mean) * fast_exp(-arw_logsd);
+                p.z_out[ge] = zn;
+                if (MODE == IAF_MODE_STEP) {
+                  if (p.elem) p.elem[ge] = arw_logsd;
+                  red[0] += arw_logsd;
+                } else {
+                  const float logqs = -0.9189385332046727f - pls - 0.5f * eps * eps + arw_logsd;
+                  const float pl = __ldg(p.prior_logsd + ge);
+                  const float d = zn - __ldg(p.prior_mean + ge);
+                  const float logps = -0.9189385332046727f - pl - 0.5f * d * d * fast_exp(-2.0f * pl);
+                  const float kl = logqs - logps;
+                  if (p.elem) p.elem[ge] = kl;
+                  red[e] = kl;
+                }
+              }
+            }
+            if (MODE == IAF_MODE_LAYER) {
+              for (int nl_ = 0; nl_ < ns; ++nl_) {
+  #pragma unroll
+                for (int e = 0; e < 8; ++e) {
+                  float x = (si.valid && si.n == n_first + nl_) ? red[e] : 0.f;
+  #pragma unroll
+                  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+                  if (lane == 0) s_part[((pb * 4 + qd) * p.MAXS + nl_) * p.C + ch0 + e] = x;
+                }
               }
             }
           }
-        }
-        if (!waited) mbar_wait(&bars[LB_ACC_FULL + b], (uint32_t)(use & 1));
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars[LB_ACC_EMPTY + b]);
 
-        if (p.persample_out || p.bc_out) {
-          constexpr bool LAY = (MODE == IAF_MODE_LAYER);
-          if (!LAY) {
-            if (i >= 2) mbar_wait(&bars[LB_PART_EMPTY + pb], (uint32_t)(((i >> 1) - 1) & 1));
-            for (int nl_ = 0; nl_ < ns; ++nl_) {
-              float x = (si.valid && si.n == n_first + nl_) ? red[0] : 0.f;
-#pragma unroll
-              for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-              if (lane == 0) s_part[(pb * LY_WORKERS + warp) * p.MAXS + nl_] = x;
+          if (p.persample_out || p.bc_out) {
+            constexpr bool LAY = (MODE == IAF_MODE_LAYER);
+            if (!LAY) {
+              if (i >= 2) mbar_wait(&bars[LB_PART_EMPTY + pb], (uint32_t)(((i >> 1) - 1) & 1));
+              for (int nl_ = 0; nl_ < ns; ++nl_) {
+                float x = (si.valid && si.n == n_first + nl_) ? red[0] : 0.f;
+  #pragma unroll
+                for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+                if (lane == 0) s_part[(pb * LY_WORKERS + warp) * p.MAXS + nl_] = x;
+              }
             }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&bars[LB_PART + pb]);
           }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bars[LB_PART + pb]);
-        }
+      };
+
+      const float* tb0 = reinterpret_cast<const float*>(smem + q.sm_bias);
+      if (FUSED) {
+        hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
+        fence_proxy_async();
+        worker_bar_sync();
+        const IafTcStage& St1 = p.st[1];
+        int g1 = 0;
+        ly_mma_tile<NGW>(smem, bars, s_acc, St1.N, q.n_bchunks1, false, 1, g1, LB_BFULL + q.n_bchunks,
+                         smem_u32(smem + q.sm_b1), (uint32_t)(2 * q.b_chunk_bytes1), (uint32_t)q.b_chunk_bytes1, false,
+                         smem_u32(smem + q.sm_h), (uint32_t)h_plane, (uint32_t)((St1.cin >> 3) * h_plane), p.Wp);
+        worker_bar_sync();
+        SlotInfo si_out = si_all;
+        si_out.valid = si_all.valid && sl < q.TO;
+        heads_epi(St1, reinterpret_cast<const float*>(smem + q.sm_bias1), St1.N >> 4, ly_acc_pitch(St1.N), si_out);
+      } else if (!q.is_heads) {
+        hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
+      } else {
+        heads_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
       }
     }
-    if (warp == 0) { LPROBE(2) LPROBE_DUMP(2) }
   }
 
-  if (warp == LY_RED_WARP && q.is_heads && (p.persample_out || p.bc_out) && MODE != IAF_MODE_MULTICONV) {
+  if (warp == LY_RED_WARP && (FUSED || q.is_heads) && (p.persample_out || p.bc_out) && MODE != IAF_MODE_MULTICONV) {
     // ===================== reducer warp: per-tile partials -> per-sample outputs, off the workers' critical path ==========
     float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
     constexpr bool LAY = (MODE == IAF_MODE_LAYER);
     for (int i = 0; i < n_my; ++i) {
       const int u = (int)blockIdx.x + i * (int)gridDim.x;
       const int pb = i & 1;
-      const int tile_s0 = u * TC_TILE;
+      const int tile_s0 = u * q.TS;
       const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
-      const int n_last = min(p.B - 1, fast_div(tile_s0 + TC_TILE - 1, p.SPS, p.mg_sps));
+      const int n_last = min(p.B - 1, fast_div(tile_s0 + q.TS - 1, p.SPS, p.mg_sps));
       const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
       {
             mbar_wait(&bars[LB_PART + pb], (uint32_t)((i >> 1) & 1));
@@ -697,7 +591,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             for (int k_ = lane; k_ < ns; k_ += 32) {
               const int n = n_first + k_;
               const int a = n * p.SPS, bb = a + p.SPS - 1;
-              const int ta = a / TC_TILE, tbk = bb / TC_TILE;
+              const int ta = a / q.TS, tbk = bb / q.TS;
               const unsigned expected = (unsigned)(tbk - ta + 1);
               __threadfence();
               if (atomicAdd(p.counter + n, 1u) == expected - 1u) {
@@ -707,7 +601,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                 for (int c = 0; c < cred; ++c) {
                   float tot = 0.f;
                   for (int tt = ta; tt <= tbk; ++tt) {
-                    const int nf = fast_div(tt * TC_TILE, p.SPS, p.mg_sps);
+                    const int nf = fast_div(tt * q.TS, p.SPS, p.mg_sps);
                     tot += __ldcg(p.tilepart + ((size_t)tt * p.MAXS + (n - nf)) * cred + c);
                   }
                   if (LAY && p.bc_out) p.bc_out[(size_t)n * p.C + c] = tot;
@@ -722,9 +616,6 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (cs > 1) cluster_sync_all();  // no member leaves while peers may still multicast into it or signal its barriers
   if (q.tl_enable) { TL_FLUSH }
-  if (warp == LY_MMA_WARP) tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
 }

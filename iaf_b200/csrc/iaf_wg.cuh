@@ -6,12 +6,12 @@
 // forward and the data gradient use -- [chunk of 8 channels][slot][8] fp16 hi / lo -- but read with the SLOT stream as
 // K: 8 consecutive slots of a chunk plane are exactly one core matrix of the canonical no-swizzle MN-MAJOR layout
 // (8 K-rows x 16 bytes of 8 contiguous channels), LBO = 128 B between K groups, SBO = the plane pitch between channel
-// groups, and a tap is still `shift x 16` bytes on G's start address (tools/mma_mnmajor.cu, profiles/r2_mma_mnmajor.log:
-// exact for shifts 0 / 1 / 8 / 17 / 18).  So per tap and per 16 slots: D_tap[ci][co] += X^T G with M = 128 input channels
-// (a block; M = 64 for a block of at most 64; rows past the layer's channels read whatever follows in shared memory and
-// are never stored), N = a part of
-// the columns (5 accumulators of N <= 96 columns fill the 512 TMEM columns), the same three split-operand products as
-// everywhere (X_lo G_hi, X_hi G_lo, X_hi G_hi; A-operand collector on the pair).
+// groups, and a tap is still `shift x 16` bytes on G's start address.  Both operands are MN-major (wgmma transpose
+// flags).  Per tap and per 16 slots: D_tap[ci][co] += X^T G; two warpgroups of M = 64 input channels make a block of
+// 128 (rows past the layer's channels read whatever follows in shared memory and are never stored), N = a part of the
+// columns of at most 48 (5 taps x Np / 2 accumulator registers per thread), the same three split-operand products as
+// everywhere (X_lo G_hi, X_hi G_lo, X_hi G_hi).  Layers of at most 64 input channels run one warpgroup per CTA.  The
+// column groups (NGRP) and warpgroups (NWG) are compile-time counts, so no wgmma sits behind a run-time condition.
 //
 // Work split: one CTA per (channel block, column part, split-K group); the group walks K tiles of WG_KT slots through a
 // bulk-copy ring; partial sums go to part[group][...] and the fixed-order reduction kernel of iaf_bwd.cu adds them.
@@ -22,10 +22,8 @@
 #define WG_KT 64          // slots per K tile (4 MMAs of K = 16 per tap and product)
 #define WG_HALO 24        // G slots past the tile a tap can reach (>= Wp + 1, multiple of 8)
 #define WG_MAX_STAGES 6
-#define WG_EPI 4          // epilogue warps (one per TMEM lane quadrant)
-#define WG_W_MMA WG_EPI
-#define WG_W_TMA (WG_EPI + 1)
-#define WG_THREADS ((WG_EPI + 2) * 32)
+#define WG_MAX_NP 48      // columns per CTA (5 taps x 24 accumulator registers per thread at most)
+#define WG_THREADS(NWG) ((4 * (NWG) + 1) * 32)  // NWG consumer warpgroups of 64 input channels, one producer warp
 
 struct IafWgTcParams {
   const __nv_bfloat16* x_hi;  // [x_planes/8][S_pad][8]
@@ -42,13 +40,13 @@ struct IafWgTcParams {
   int xplanes, gplanes;       // chunk planes staged per tile: of this CTA's channel block / column part
 };
 
-__global__ void __launch_bounds__(WG_THREADS, 1) iaf_wg_kernel(const __grid_constant__ IafWgTcParams p) {
+template <int NGRP, int NWG>
+__global__ void __launch_bounds__(WG_THREADS(NWG), 1) iaf_wg_kernel(const __grid_constant__ IafWgTcParams p) {
+  constexpr int WG_CONS = 4 * NWG, WG_W_TMA = WG_CONS;
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bars[2 * WG_MAX_STAGES + 1];
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t bars[2 * WG_MAX_STAGES];
   uint64_t* full = bars;
   uint64_t* empty = bars + WG_MAX_STAGES;
-  uint64_t* acc_full = bars + 2 * WG_MAX_STAGES;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int bid = blockIdx.x;
   const int np = bid % p.n_np; bid /= p.n_np;
@@ -57,25 +55,15 @@ __global__ void __launch_bounds__(WG_THREADS, 1) iaf_wg_kernel(const __grid_cons
   const int x_pitch = WG_KT * 16, g_pitch = (WG_KT + WG_HALO) * 16;  // bytes per chunk plane in a stage
   const int n_my = (p.NTK - g + p.NG - 1) / p.NG;                      // K tiles u = g, g + NG, ...
   const int xpl = min(p.xplanes, (p.cin >> 3) - mb * 16);               // chunk planes this channel block really has
-  // a block with at most 64 channels issues M = 64 instructions (half the A fetch; the accumulator then sits in lanes
-  // 0-15 of every 32-lane quadrant: row m -> lane (m / 16) * 32 + m % 16, tools/mma_mnmajor.cu)
-  const bool m64 = xpl <= 8;
 
-  if (warp == WG_W_MMA) {
-    tmem_alloc(&s_tmem, 512u);
-    if (lane == 0) {
-      for (int i = 0; i < WG_MAX_STAGES; ++i) {
-        mbar_init(&full[i], 1);
-        mbar_init(&empty[i], 1);
-      }
-      mbar_init(acc_full, 1);
-      fence_barrier_init();
+  if (warp == WG_W_TMA && lane == 0) {
+    for (int i = 0; i < WG_MAX_STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], NWG);  // every consumer warpgroup releases a stage
     }
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
   if (warp == WG_W_TMA) {
     // one bulk copy per chunk plane and image; the lanes of the warp issue them side by side
@@ -104,73 +92,87 @@ __global__ void __launch_bounds__(WG_THREADS, 1) iaf_wg_kernel(const __grid_cons
       }
       __syncwarp();
     }
-  } else if (warp == WG_W_MMA) {
-    // instruction descriptor: fp16 x fp16 -> f32, BOTH operands MN-major (bits 15, 16), M = 128, N = Np
-    const uint32_t idesc = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(p.Np >> 3) << 17) | ((uint32_t)((m64 ? 64 : 128) >> 4) << 24);
-    const uint32_t xh_hi = ((uint32_t)x_pitch >> 4) | (1u << 14);  // high words: SBO = plane pitch, descriptor version 1
-    const uint32_t gh_hi = ((uint32_t)g_pitch >> 4) | (1u << 14);
+  } else if (warp < WG_CONS) {
+    // consumer warpgroup wgi: input channels [64 wgi, +64) of the block, every column of the part, all five taps
+    const int wgi = warp >> 2, wl = warp & 3;
+    float* out = p.part + (size_t)g * p.part_stride;
+    float acc[IAF_NTAPS][NGRP][8];
+#pragma unroll
+    for (int t = 0; t < IAF_NTAPS; ++t)
+#pragma unroll
+      for (int k = 0; k < NGRP; ++k)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[t][k][e] = 0.f;
+    // high words: SBO = the plane pitch (next 8 channels); low words: start (16-byte units) | LBO = 128 B (next 8 slots)
+    const uint32_t x_hi_w = (uint32_t)x_pitch >> 4, g_hi_w = (uint32_t)g_pitch >> 4;
     const uint32_t sh[IAF_NTAPS] = {0u, 1u, (uint32_t)(p.Wp - 1), (uint32_t)p.Wp, (uint32_t)(p.Wp + 1)};
     for (int i = 0; i < n_my; ++i) {
       const int stg = i % p.n_stages, use = i / p.n_stages;
       mbar_wait(&full[stg], (uint32_t)(use & 1));
-      tc_fence_after();
       const uint32_t sbase = smem_u32(smem + (size_t)stg * p.stage_bytes);
-      // low words: start address (16-byte units) | LBO = 128 B (next 8 slots) << 16
-      const uint32_t xh0 = ((sbase >> 4) & 0x3FFFu) | ((128u >> 4) << 16);
-      const uint32_t xl0 = (((sbase + (uint32_t)(p.xplanes * x_pitch)) >> 4) & 0x3FFFu) | ((128u >> 4) << 16);
-      const uint32_t gh0 = (((sbase + (uint32_t)p.xa_bytes) >> 4) & 0x3FFFu) | ((128u >> 4) << 16);
-      const uint32_t gl0 = (((sbase + (uint32_t)p.xa_bytes + (uint32_t)(p.gplanes * g_pitch)) >> 4) & 0x3FFFu) | ((128u >> 4) << 16);
-      if (elect_one_sync()) {
-#pragma unroll 1
-        for (int t = 0; t < IAF_NTAPS; ++t) {
-          const uint32_t d = tmem_base + (uint32_t)(t * p.Np);
-#pragma unroll 1
-          for (int ks = 0; ks < WG_KT / 16; ++ks) {
-            const uint32_t xo = (uint32_t)(ks * 16), go = (uint32_t)(ks * 16) + sh[t];  // 16-byte units = slots
-            const uint64_t xh = ((uint64_t)xh_hi << 32) | (xh0 + xo), xl = ((uint64_t)xh_hi << 32) | (xl0 + xo);
-            const uint64_t gh = ((uint64_t)gh_hi << 32) | (gh0 + go), gl = ((uint64_t)gh_hi << 32) | (gl0 + go);
-            const uint32_t acc = (i > 0 || ks > 0) ? 1u : 0u;
-            umma_f16(d, xl, gh, idesc, acc);
-            umma_f16_afill(d, xh, gl, idesc, 1u);
-            umma_f16_alast(d, xh, gh, idesc, 1u);
+      const uint32_t xh0 = wg_desc_lo(sbase + (uint32_t)(wgi * 8 * x_pitch), 128u);
+      const uint32_t xl0 = wg_desc_lo(sbase + (uint32_t)((p.xplanes + wgi * 8) * x_pitch), 128u);
+      const uint32_t gh0 = wg_desc_lo(sbase + (uint32_t)p.xa_bytes, 128u);
+      const uint32_t gl0 = wg_desc_lo(sbase + (uint32_t)p.xa_bytes + (uint32_t)(p.gplanes * g_pitch), 128u);
+      const uint32_t g_grp = (uint32_t)(2 * g_pitch) >> 4;  // 16 columns = two chunk planes
+      wgmma_fence();
+#pragma unroll
+      for (int t = 0; t < IAF_NTAPS; ++t) {
+#pragma unroll
+        for (int ks = 0; ks < WG_KT / 16; ++ks) {
+          const uint32_t xo = (uint32_t)(ks * 16), go = (uint32_t)(ks * 16) + sh[t];  // 16-byte units = slots
+          const uint64_t xh = ((uint64_t)x_hi_w << 32) | (xh0 + xo), xl = ((uint64_t)x_hi_w << 32) | (xl0 + xo);
+#pragma unroll
+          for (int k = 0; k < NGRP; ++k) {
+            const uint32_t gk = go + (uint32_t)k * g_grp;
+            const uint64_t gh = ((uint64_t)g_hi_w << 32) | (gh0 + gk), gl = ((uint64_t)g_hi_w << 32) | (gl0 + gk);
+            wgmma_m64n16k16<1>(acc[t][k], xl, gh);
+            wgmma_m64n16k16<1>(acc[t][k], xh, gl);
+            wgmma_m64n16k16<1>(acc[t][k], xh, gh);
           }
         }
-        umma_commit(&empty[stg]);
-        if (i == n_my - 1) umma_commit(acc_full);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (wl == 0 && lane == 0) mbar_arrive(&empty[stg]);
     }
-  } else {
-    // epilogue warps: D_tap[ci][co] (lanes = input channels of this block) -> part[g][(tap * cin + ci) * ncol + co] / c
-    const int ci = m64 ? (lane < 16 ? mb * 128 + warp * 16 + lane : p.cin) : mb * 128 + warp * 32 + lane;
-    float* out = p.part + (size_t)g * p.part_stride;
+    // D_tap[ci][co] -> part[g][(tap * cin + ci) * ncol + co] / c
+    float inv_c = 0.f;
     if (n_my > 0) {
       float am = 0.f;
       for (int n = 0; n < p.B; ++n) am = fmaxf(am, __ldg(p.amax + n));
-      const float inv_c = 1.0f / dg_scale_from_amax(am);
-      mbar_wait(acc_full, 0u);
-      tc_fence_after();
-      const uint32_t t_lane = tmem_base + ((uint32_t)(warp * 32) << 16);
-      for (int t = 0; t < IAF_NTAPS; ++t)
-        for (int c0 = 0; c0 < p.Np; c0 += 16) {
-          uint32_t r[16];
-          tmem_ld16(t_lane + (uint32_t)(t * p.Np + c0), r);
-          tmem_ld_wait();
-          if (ci < p.cin) {
-            float* o = out + ((size_t)t * p.cin + ci) * p.ncol + np * p.Np + c0;
+      inv_c = 1.0f / dg_scale_from_amax(am);
+    }
+    const int ci0 = mb * 128 + wgi * 64 + wl * 16 + (lane >> 2);
 #pragma unroll
-            for (int e4 = 0; e4 < 4; ++e4)
-              *reinterpret_cast<float4*>(o + 4 * e4) =
-                  make_float4(__uint_as_float(r[4 * e4]) * inv_c, __uint_as_float(r[4 * e4 + 1]) * inv_c,
-                              __uint_as_float(r[4 * e4 + 2]) * inv_c, __uint_as_float(r[4 * e4 + 3]) * inv_c);
+    for (int t = 0; t < IAF_NTAPS; ++t)
+#pragma unroll
+      for (int k = 0; k < NGRP; ++k) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int ci = ci0 + 8 * h;
+          if (ci < p.cin) {
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              const int co = np * p.Np + 16 * k + 8 * j + 2 * (lane & 3);
+              *reinterpret_cast<float2*>(out + ((size_t)t * p.cin + ci) * p.ncol + co) =
+                  make_float2(acc[t][k][4 * j + 2 * h] * inv_c, acc[t][k][4 * j + 2 * h + 1] * inv_c);
+            }
           }
         }
-    } else if (ci < p.cin) {
-      for (int t = 0; t < IAF_NTAPS; ++t)
-        for (int c0 = 0; c0 < p.Np; ++c0) out[((size_t)t * p.cin + ci) * p.ncol + np * p.Np + c0] = 0.f;
-    }
+      }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == WG_W_MMA) tmem_dealloc(tmem_base, 512u);
+}
+
+typedef void (*WgKernel)(const IafWgTcParams);
+// column groups of 16 per CTA (Np / 16) and consumer warpgroups (2 for layers of more than 64 input channels)
+static WgKernel wg_kernel_pick(int ngrp, int nwg) {
+  switch (ngrp * 2 + (nwg - 1)) {
+    case 2: return iaf_wg_kernel<1, 1>;
+    case 3: return iaf_wg_kernel<1, 2>;
+    case 4: return iaf_wg_kernel<2, 1>;
+    case 5: return iaf_wg_kernel<2, 2>;
+    case 6: return iaf_wg_kernel<3, 1>;
+    default: return iaf_wg_kernel<3, 2>;
+  }
 }

@@ -1,6 +1,6 @@
 """ELBO forward around the IAF operator (SURVEY 8f-2): the TF model's `CVAE1._forward`
 (tf_train.py:161-219) with `IAFLayer.up/down` (tf_train.py:29-95), restated in PyTorch so that
-bits/dim can be compared between the B200 operator and the oracle operator on identical weights
+bits/dim can be compared between the CUDA operator and the oracle operator on identical weights
 and inputs ("bits/dim parity" in BASELINE.json's metric).
 
 Only the stochastic-layer block (posterior sample -> IAF step -> KL) is the hot path and goes
@@ -154,7 +154,7 @@ def make_params(hps, seed=0, dtype=np.float32):
 
 
 class CudaIAF(object):
-    """iaf_layer callable backed by the fused B200 operator (one IAFOperator per layer scope, weights cached)."""
+    """iaf_layer callable backed by the fused CUDA operator (one IAFOperator per layer scope, weights cached)."""
 
     def __init__(self, params, hps, path="auto"):
         from .ops import IAFOperator

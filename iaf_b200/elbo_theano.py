@@ -2,7 +2,7 @@
 `cvae1.f_encode_decode` (models.py:435-497) with `cvae_layer.up` / `cvae_layer.down_q` (models.py:133-328) for
 ``posterior='down_iaf2_nl'`` (the README configs, train.py:55-75) and ``posterior='up_iaf2_nl'`` (the bottom-up
 placement of the same operator, models.py:169-178), ``prior='diag'``, ``px='logistic'``, ``downsample_type='nn'``,
-restated in PyTorch so that bits/dim can be compared between the B200 operator and the oracle
+restated in PyTorch so that bits/dim can be compared between the CUDA operator and the oracle
 operator on identical weights, inputs and noise.
 
 As in :mod:`iaf_b200.elbo`, only the stochastic-layer block goes through a pluggable callable: for down_iaf2_nl the
@@ -203,7 +203,7 @@ def make_params(hps, seed=0, dtype=np.float32):
 
 
 class CudaIAF(object):
-    """iaf_layer callable backed by the fused B200 operator, Theano variant (one IAFOperator per layer name)."""
+    """iaf_layer callable backed by the fused CUDA operator, Theano variant (one IAFOperator per layer name)."""
 
     def __init__(self, w, hps, path="auto"):
         from .ops import IAFOperator

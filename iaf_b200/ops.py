@@ -1,4 +1,4 @@
-"""Host side of the B200 IAF step: the reference's python operator signatures over the C ABI.
+"""Host side of the H100 IAF step: the reference's python operator signatures over the C ABI.
 
 PyTorch tensors are used as device storage and for the current stream only; all compute
 is in libiaf_b200.so (include/iaf_b200.h).  Three entry points mirror the reference:
@@ -308,8 +308,7 @@ class IAFOperator(object):
     def layer(self, eps, post_mean, post_logsd, prior_mean, prior_logsd, context, want_kl=True):
         """Fused posterior-sample -> IAF step -> KL block (tf_train.py:56-85, models.py:273-328).
         Returns (z', kl [B,C,H,W] or None, kl_bc [B,C], kl_cost [B]).  Differentiable: when an input or a parameter
-        requires grad the call is ONE autograd node (backward = iaf_layer_bwd; confirmed on a B200 in round 2:
-        worst relative gradient error 6.4e-4 on the whole training objective).  IAF_LAYER_AUTOGRAD=0 switches it off."""
+        requires grad the call is ONE autograd node (backward = iaf_layer_bwd).  IAF_LAYER_AUTOGRAD=0 switches it off."""
         if os.environ.get("IAF_LAYER_AUTOGRAD", "1") != "0" and self._needs_grad(eps, post_mean, post_logsd, prior_mean,
                                                                                    prior_logsd, context):
             self.invalidate()  # training: parameters may have been stepped through .data since the last call
@@ -479,7 +478,7 @@ class _MulticonvFn(torch.autograd.Function):
     """autograd node of the un-fused operator: forward = iaf_multiconv_fwd, backward = iaf_multiconv_bwd."""
 
     # The forward keeps the hidden activations (iaf_multiconv_fwd_train) and the backward skips the recompute
-    # (iaf_multiconv_bwd_saved), as the fused step's node does (confirmed on a B200 in round 2).
+    # (iaf_multiconv_bwd_saved), as the fused step's node does.
     # IAF_MULTICONV_SAVED=0 falls back to recomputing them in the backward.
     @staticmethod
     def forward(ctx, op, z, context, *flat):

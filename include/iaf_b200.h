@@ -1,5 +1,5 @@
 /*
- * iaf_b200 -- C ABI of the B200-native IAF posterior step.
+ * iaf_b200 -- C ABI of the H100-native (sm_90a) IAF posterior step.
  *
  * The reference (openai/iaf) has no FFI layer: its boundary for this path is a python
  * callable.  These entry points are what a python (ctypes/cffi) binding of that callable
@@ -31,7 +31,7 @@ typedef enum {
   IAF_ERR_UNSUPPORTED = -3, /* valid in the reference but outside what the kernels cover       */
   IAF_ERR_CUDA = -4,        /* a CUDA runtime call failed; see iaf_last_cuda_error()           */
   IAF_ERR_NOT_PACKED = -5,  /* iaf_step_* called before iaf_pack_weights                       */
-  IAF_ERR_NO_DEVICE = -6    /* no sm_100 device                                                */
+  IAF_ERR_NO_DEVICE = -6    /* no sm_90 device                                                 */
 } iaf_status;
 
 /* which of the reference's two implementations the numerics follow (SURVEY F2) */
@@ -46,7 +46,7 @@ typedef enum { IAF_NL_NONE = 0, IAF_NL_ELU = 1, IAF_NL_SOFTPLUS = 2, IAF_NL_RELU
 typedef enum {
   IAF_PATH_AUTO = 0, /* tensor cores when the shape qualifies, else SIMT            */
   IAF_PATH_SIMT = 1, /* exact-fp32 FMA kernel (parity anchor, any shape)            */
-  IAF_PATH_TC = 2    /* tcgen05 implicit-GEMM kernel, bf16x3 split operands         */
+  IAF_PATH_TC = 2    /* wgmma implicit-GEMM kernel, fp16 hi/lo split operands        */
 } iaf_path;
 
 /*

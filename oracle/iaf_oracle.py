@@ -6,7 +6,7 @@ This file is a numpy restatement of the reference's algorithm for the hot path
 reference`` legs may import it.  Nothing under ``iaf_b200/`` imports it and the
 product path never falls back to it.
 
-PARITY PIN STATUS.  The reference (openai/iaf, /root/reference) ships no test,
+PARITY PIN STATUS.  The reference (openai/iaf) ships no test,
 fixture or golden vector for this path (tf_utils/distributions_test.py and
 tf_utils/hparams_test.py are its only tests) and neither Theano nor TensorFlow
 can be imported in the build container, so the reference cannot be *run*
@@ -16,7 +16,7 @@ reference's OWN python source for ``get_linear_ar_mask``, ``get_conv_ar_mask``,
 ``ar.conv2d`` / ``ar.multiconv2d`` (graphy/nodes/ar.py), ``pad2dwithchannel``
 (graphy/nodes/conv.py), ``DiagonalGaussian`` / ``compute_lowerbound`` /
 ``logsumexp`` / ``repeat`` (tf_utils/distributions.py) and ``IAFLayer.down``
-(tf_train.py) is exec'd from /root/reference against small numpy stand-ins for
+(tf_train.py) is exec'd from the reference source against small numpy stand-ins for
 the handful of TF / Theano primitives it calls (conv2d, l2_normalize, elu,
 dnn_conv, ...), and the resulting tensors are committed as fixtures under
 tests/golden/.  The third-party primitives themselves (cuDNN conv through
@@ -24,7 +24,7 @@ TF / Theano; versions unpinned by the reference) are restated from their
 published semantics; that part of parity is therefore "restated, not executed".
 
 Every function cites the reference file:line it follows (paths relative to
-/root/reference).  All arithmetic is done in the dtype of the inputs (use
+the reference repository).  All arithmetic is done in the dtype of the inputs (use
 float64 inputs for the truth oracle, float32 for the like-for-like CPU port).
 """
 from __future__ import annotations

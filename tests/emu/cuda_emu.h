@@ -10,7 +10,7 @@
 // Covered: __global__/__device__ qualifiers, threadIdx/blockIdx/blockDim/gridDim, static and dynamic shared memory,
 // __syncthreads (std::barrier; a thread that returns early drops out of the barrier as on the device), __threadfence,
 // atomicAdd, __ldg/__ldcg, float4, and the handful of runtime calls iaf_capi.cu makes (malloc/memset/memcpy as host
-// operations, streams and events as no-ops).  Not covered on purpose: warp shuffles, inline PTX, tcgen05/TMA.
+// operations, streams and events as no-ops).  Not covered on purpose: warp shuffles, inline PTX, wgmma/TMA.
 #pragma once
 #include <atomic>
 #include <barrier>

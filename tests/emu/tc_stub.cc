@@ -1,4 +1,4 @@
-// Host-emulation build only (tests/emu): the tcgen05 path cannot be emulated, so the library reports it as unsupported
+// Host-emulation build only (tests/emu): the wgmma path cannot be emulated, so the library reports it as unsupported
 // and every plan takes the SIMT path.  TEST INFRASTRUCTURE ONLY.
 #include "iaf_tc.h"
 

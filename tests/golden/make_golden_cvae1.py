@@ -2,12 +2,12 @@
 """Generate tests/golden/cvae1_forward.npz by EXECUTING the reference's own `CVAE1._forward` (tf_train.py:161-219), with
 `IAFLayer.up` / `IAFLayer.down` (tf_train.py:23-95), `conv2d` / `deconv2d` / `ar_multiconv2d` / `resize_nearest_neighbor`
 (tf_utils/layers.py) and `discretized_logistic` / `compute_lowerbound` / `repeat` (tf_utils/distributions.py) all run from
-/root/reference through the same python-2 shims and numpy-backed TensorFlow stand-in as make_golden.py (extended here
+the reference through the same python-2 shims and numpy-backed TensorFlow stand-in as make_golden.py (extended here
 by the handful of primitives the whole forward pass needs: strided SAME convolution, conv2d_transpose, transpose,
 clip_by_value, floor, sigmoid, nearest-neighbour resize).  The convolution primitives themselves are stood in for by
 torch CPU float64 ops -- independent of both iaf_b200/elbo.py's restatement (which the fixture pins) and the oracle.
 
-Run in the build container only (needs /root/reference):   python tests/golden/make_golden_cvae1.py
+Needs a checkout of the reference (IAF_REFERENCE, see make_golden.py):   python tests/golden/make_golden_cvae1.py
 """
 import os
 import sys

@@ -3,7 +3,7 @@
 `N.ar.multiconv2d` (graphy/nodes/ar.py), `N.rand.gaussian_diag` (graphy/nodes/rand.py:78-87) and the
 nearest-neighbour resamplers (conv.py:36-49), for posterior='down_iaf2_nl' and 'up_iaf2_nl', prior='diag'.
 
-Run in the build container only (needs /root/reference):  python tests/golden/make_golden_theano_layer.py
+Needs a checkout of the reference (IAF_REFERENCE, see make_golden.py):  python tests/golden/make_golden_theano_layer.py
 Writes tests/golden/cvae_layer_down.npz.  Same approach as make_golden.py: python2 -> python3 syntax shims, an
 eager ndarray stand-in for Theano tensors, cuDNN replaced by torch CPU float64 convolution.
 """

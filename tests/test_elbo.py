@@ -1,4 +1,4 @@
-"""bits/dim parity (BASELINE.json metric, SURVEY 8f-2): the restated ELBO forward evaluated with the B200
+"""bits/dim parity (BASELINE.json metric, SURVEY 8f-2): the restated ELBO forward evaluated with the CUDA
 operator equals the same forward evaluated with the oracle operator on identical weights, inputs and noise."""
 import numpy as np
 import pytest
@@ -46,8 +46,8 @@ def test_plumbing_against_oracle_primitives_cpu():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("hps,B", [
-    (dict(z_size=32, h_size=64, depth=2, num_blocks=2, kl_min=0.25, image_size=32), 4),   # fused tcgen05 path, two levels
-    (dict(z_size=32, h_size=160, depth=1, num_blocks=3, kl_min=0.1, image_size=32), 2),   # C3 shapes: layered tcgen05 path
+    (dict(z_size=32, h_size=64, depth=2, num_blocks=2, kl_min=0.25, image_size=32), 4),   # tensor-core path, two levels
+    (dict(z_size=32, h_size=160, depth=1, num_blocks=3, kl_min=0.1, image_size=32), 2),   # C3 shapes: tensor-core path
 ])
 def test_bits_per_dim_parity(hps, B):
     pg, xg, ng = _setup(hps, B, 7, torch.float32, "cuda")
@@ -111,7 +111,7 @@ def test_torch_oracle_layer_equals_numpy_oracle_layer_cpu():
     (dict(z_size=8, h_size=16, depth=1, num_blocks=2, kl_min=0.0, image_size=16), 4),
 ])
 def test_training_objective_gradient_parity(hps, B):
-    """SURVEY 8f-4: d(objective)/d(every parameter) through the B200 operator's autograd node (iaf_step_fwd /
+    """SURVEY 8f-4: d(objective)/d(every parameter) through the CUDA operator's autograd node (iaf_step_fwd /
     iaf_step_bwd) equals torch autograd through the oracle block, in fp64 on the CPU."""
     from oracle.elbo_oracle import TorchIAF
     pg, xg, ng = _setup(hps, B, 9, torch.float32, "cuda")
@@ -234,7 +234,7 @@ def test_tf_training_gradients_over_the_emulated_abi(monkeypatch, fused):
 def test_forward_against_reference_executed_cvae1_forward():
     """elbo.forward (the restatement used for every bits/dim parity number) against what the reference's OWN
     `CVAE1._forward` (tf_train.py:161-219, with IAFLayer.up/down, conv2d/deconv2d/ar_multiconv2d, discretized_logistic,
-    compute_lowerbound executed from /root/reference by tests/golden/make_golden_cvae1.py) produced on the same
+    compute_lowerbound executed from the reference source by tests/golden/make_golden_cvae1.py) produced on the same
     parameters, image and noise: the objective, the loss and bits/dim."""
     import os
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", "cvae1_forward.npz"))

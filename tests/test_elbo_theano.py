@@ -1,6 +1,6 @@
 """Theano front-end ELBO (SURVEY 8f-2, configs C1 / C4): the restated `cvae_layer` / `cvae1.f_encode_decode` plumbing is
 pinned against vectors produced by executing the reference's own models.py (tests/golden/make_golden_theano_layer.py),
-and bits/dim computed with the B200 operator equals bits/dim computed with the oracle operator."""
+and bits/dim computed with the CUDA operator equals bits/dim computed with the oracle operator."""
 import os
 
 import numpy as np
@@ -64,9 +64,9 @@ def test_forward_free_bits_and_shapes_cpu(posterior):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("hps,B", [
-    # C1 shapes (README.md:30): n_h 64, depth_ar 1, three levels -> 16x16, 8x8, 4x4 latents; fused tcgen05 kernel
+    # C1 shapes (README.md:30): n_h 64, depth_ar 1, three levels -> 16x16, 8x8, 4x4 latents; tensor-core kernel
     (dict(n_z=32, n_h1=64, n_h2=64, depths=[2, 2, 2], depth_ar=1, nl="elu", kl_min=0.25, image_size=32), 4),
-    # C4 shapes (README.md:55-58): n_h 160, depth_ar 2, two levels; layer-at-a-time tcgen05 kernel
+    # C4 shapes (README.md:55-58): n_h 160, depth_ar 2, two levels; tensor-core kernel
     (dict(n_z=32, n_h1=160, n_h2=160, depths=[2, 2], depth_ar=2, nl="elu", kl_min=0.25, image_size=32), 2),
     # cvae1's default nonlinearity (models.py:384) runs on the exact-fp32 kernel's run-time switch as well
     (dict(n_z=32, n_h1=64, n_h2=64, depths=[1, 1], depth_ar=1, nl="softplus", kl_min=0.0, image_size=32), 2),

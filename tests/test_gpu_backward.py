@@ -42,8 +42,8 @@ def _build(variant, n_z, hidden, heads, H, W, B, nl, path="auto"):
 
 BWD_CASES = [
     # variant, n_z, hidden, H, W, B, nl
-    ("tf", 32, [64], 16, 16, 4, "elu"),            # C2a shape (forward on the fused tcgen05 kernel)
-    ("tf", 32, [160, 160], 16, 16, 2, "elu"),      # C2b / C3 shape (forward on the layered tcgen05 kernel)
+    ("tf", 32, [64], 16, 16, 4, "elu"),            # C2a shape (forward on the tensor cores)
+    ("tf", 32, [160, 160], 16, 16, 2, "elu"),      # C2b / C3 shape (forward on the tensor cores)
     ("theano", 32, [64], 8, 8, 3, "elu"),          # C1 level 1
     ("theano", 32, [160, 160], 16, 16, 2, "softplus"),  # C4 shape, cvae1's default nl
     ("tf", 8, [16, 16], 5, 7, 2, "elu"),
@@ -52,6 +52,9 @@ BWD_CASES = [
     ("theano", 4, [], 4, 4, 2, "elu"),             # depth_ar = 0 (SURVEY F8)
     ("tf", 4, [8], 40, 24, 1, "leakyrelu"),        # several row bands
     ("theano", 4, [4], 2, 2, 70, "elu"),           # more (sample, band) units than weight-gradient CTAs
+    ("tf", 16, [32], 16, 16, 3, "elu"),            # tensor cores, padded column groups (one-launch forward)
+    ("theano", 16, [48, 48], 8, 8, 2, "elu"),      # tensor cores, padded column groups (per-stage forward, 48-wide data
+                                                   # gradient and weight gradient)
 ]
 
 
@@ -188,7 +191,7 @@ def test_backward_error_behaviour():
                          ids=["c2a", "c4-softplus", "c3-8x8"])
 def test_tensor_core_backward_is_taken_and_matches_the_simt_backward(variant, hidden, H, W, nl, monkeypatch):
     """The backward of a tensor-core plan runs its data gradient (layered-kernel stage on the point-reflected stream) and
-    its weight gradient (MN-major MMAs over the slot stream) on the tensor cores -- `backward_path` says so -- and agrees
+    its weight gradient (MN-major wgmma over the slot stream) on the tensor cores -- `backward_path` says so -- and agrees
     with the exact-fp32 SIMT backward of the same operator (IAF_BWD_TC=0) within the parity tolerance; a plan pinned to the
     SIMT path keeps the SIMT backward."""
     n_z, B = 32, 5
@@ -273,3 +276,14 @@ def test_tensor_core_backward_after_a_larger_batch():
     # batch here), so the summation order differs; slots left over from the larger batch would be an O(1) error
     for a, b in zip(got, want):
         assert float((a.double() - b.double()).abs().max()) <= 1e-5 * max(float(b.abs().max()), 1e-30)
+
+
+@pytest.mark.parametrize("variant,hidden,H,W", [("tf", [32], 16, 16), ("theano", [48, 48], 8, 8)],
+                         ids=["one-launch", "per-stage"])
+def test_padded_column_group_shapes_run_on_the_tensor_cores(variant, hidden, H, W):
+    """The n_z = 16 cases of BWD_CASES (and of test_gpu_parity's STEP_CASES) exercise the padded column groups of the wgmma
+    kernels -- stages whose width is an odd multiple of 16 -- only if they run there: forward and backward of both shapes
+    are on the tensor cores."""
+    op = _build(variant, 16, hidden, [16, 16], H, W, 2, "elu")[0]
+    assert op.path_used(H, W, "cuda") == "tc"
+    assert op.backward_path(H, W, "cuda") == "tc"

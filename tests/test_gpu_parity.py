@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): the CUDA path, called through the C ABI, against
+"""GPU parity tests (H100): the CUDA path, called through the C ABI, against
  (1) the fixtures produced by executing the reference's own source (tests/golden),
  (2) the fp64 oracle on seeded inputs,
  (3) size-independent properties at BASELINE.json's full size (B=256).
@@ -77,6 +77,8 @@ STEP_CASES = [
     ("theano", 2, 4, [], 5, 5, "elu"),            # depth_ar = 0: context unused (F8)
     ("tf", 2, 6, [12], 6, 6, "tanh"),             # channels not a multiple of 4/8
     ("tf", 2, 8, [4], 6, 6, "elu"),               # n_out < n_in in the hidden layer
+    ("tf", 3, 16, [32], 16, 16, "elu"),           # one-launch tensor-core step, 32 columns: padded column groups
+    ("theano", 2, 16, [48, 48], 8, 8, "elu"),     # per-stage tensor-core kernels, 48 columns: padded column groups
 ]
 
 
@@ -272,14 +274,14 @@ def test_step_host_entry_matches_device_entry():
 
 
 @pytest.mark.parametrize("variant,B,hidden,H,W", [
-    ("tf", 300, [64], 16, 16),         # 678 tiles over 148 CTAs: runs of 4 and 5 tiles
+    ("tf", 300, [64], 16, 16),         # 678 tiles over 132 CTAs: runs of 5 and 6 tiles
     ("theano", 97, [64], 16, 16),      # odd batch, point-reflected orientation, pad channel
     ("theano", 515, [64], 4, 4),       # 5+ samples per 128-slot tile
     ("tf", 37, [160, 160], 16, 16),    # layer-at-a-time kernels, fewer tiles than SMs
     ("theano", 150, [160, 160], 8, 8), # layered, several samples per tile
 ])
 def test_tensor_core_paths_agree_with_fp32_path_at_odd_batches(variant, B, hidden, H, W):
-    """Cross-check of the two independent CUDA implementations (exact-fp32 SIMT vs tcgen05) on batch sizes that
+    """Cross-check of the two independent CUDA implementations (exact-fp32 SIMT vs wgmma) on batch sizes that
     exercise uneven tile runs, partial last tiles and tiles spanning many samples."""
     n_z = 32
     hid, heads = O.make_params(variant, n_z, hidden, [n_z, n_z], seed=5)

@@ -175,7 +175,7 @@ def test_bits_per_dim_c4_full_depth():
 
 @pytest.mark.parametrize("name", ["tc_kl01", "tc_kl0"])
 def test_tensor_core_fused_layer_against_iaflayer_down_fixture(name):
-    """iaf_layer_fwd on the TENSOR-CORE path (z 32, h 64, 8x8: hidden [64, 64] runs the layer-at-a-time tcgen05 kernels in
+    """iaf_layer_fwd on the TENSOR-CORE path (z 32, h 64, 8x8: hidden [64, 64] runs the tensor-core stage kernels in
     their layer mode) against tensors IAFLayer.down (tf_train.py:46-95) produced when executed from the reference's source
     (tests/golden/make_golden.py): z', kl_cost, the per-(sample, channel) KL sums and the free-bits objective."""
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", "iaflayer_down_tc.npz"))

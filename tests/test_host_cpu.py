@@ -204,17 +204,17 @@ def test_bench_reference_arm_line_schema():
     assert "theano-variant" in d["config"]["workload"]
 
 
-def test_development_variants_still_compile_for_sm100a(tmp_path):
-    """The flag-gated kernel variants kept for A/B (tools/experiments/README.md: TC_FAST_EPI, TC_HALO_TRIM, BW_FASTDIV)
-    must keep compiling for sm_100a next to the default build (nvcc cross-compiles without a GPU)."""
+def test_development_variants_still_compile_for_sm90a(tmp_path):
+    """The flag-gated development variants (IAF_TC_TIMELINE: in-kernel timeline of the tensor-core stage kernel;
+    BW_FASTDIV) must keep compiling for sm_90a next to the default build (nvcc cross-compiles without a GPU)."""
     import shutil
     import subprocess
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
         pytest.skip("nvcc not available")
     csrc = os.path.join(ROOT, "iaf_b200", "csrc")
-    base = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-std=c++17", "-c"]
-    jobs = [(["-DTC_FAST_EPI", "-DTC_HALO_TRIM"], "iaf_tc.cu"), (["-DBW_FASTDIV"], "iaf_bwd.cu")]
+    base = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-std=c++17", "-c"]
+    jobs = [(["-DIAF_TC_TIMELINE"], "iaf_tc.cu"), (["-DBW_FASTDIV"], "iaf_bwd.cu")]
     procs = [subprocess.Popen(base + flags + [src, "-o", str(tmp_path / (src + ".o"))], cwd=csrc, stdout=subprocess.PIPE,
                               stderr=subprocess.STDOUT, text=True) for flags, src in jobs]
     for (flags, src), pr in zip(jobs, procs):

@@ -1,5 +1,5 @@
 """Two-GPU NCCL test of the batch-sharded ELBO (BASELINE config C5 structure; tf_train.py:126-142): every rank evaluates
-its slice with the B200 operator, ONE all-reduce of the scalar gives the global bits/dim, which must equal the
+its slice with the CUDA operator, ONE all-reduce of the scalar gives the global bits/dim, which must equal the
 single-process evaluation of the whole batch with the same rank-local free-bits rule.  Skips with fewer than two GPUs (the
 gloo world-2 twin in tests/test_elbo.py covers the host logic on CPU)."""
 import os

@@ -1,8 +1,8 @@
-"""CPU simulation of operand precision for the IAF step (development aid, see DESIGN.md section 7): rounds the conv operands
+"""CPU simulation of operand precision for the IAF step (development aid): rounds the conv operands
 of an fp64 evaluation of the oracle to candidate tensor-core formats and reports the z' / logdet errors the parity tests
 measure.  usage: python tools/experiments/prec_sim.py"""
-import sys, time
-sys.path.insert(0, '/root/repo')
+import os, sys, time
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), '..', '..'))
 import numpy as np, torch
 import torch.nn.functional as F
 from oracle import iaf_oracle as O, iaf_oracle_torch as OT
