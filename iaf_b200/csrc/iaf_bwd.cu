@@ -1105,7 +1105,7 @@ int iaf_bwd_run(IafBwdPlan* pl, const IafBwdArgs* a, cudaStream_t stream, int* n
       if ((st = iaf_dg_stage(pl->dg, j, a->w_packed[j], (last - j) & 1, j > 0 ? hcur[j] : nullptr, outp, j > 0 ? 1 : 0, B,
                              stream)) != IAF_OK)
         return st;
-      nl_ += 2;
+      nl_ += 3;  // weight scale, weight images, stage kernel
       Gcur = Gnext;
       g_planes = pl->cin[j];
       continue;

@@ -353,7 +353,10 @@ static LyKernel ly_kernel_pick(bool padw, int mode, bool elu) {
   LY_PICK(IAF_MODE_LAYER)
 #undef LY_PICK
 }
-// the stage kernel for a stage of N output columns: NGW = ceil(N / 32) 16-column groups per warpgroup
+// the stage kernel for a stage of N output columns: NGW = ceil(N / 32) 16-column groups per warpgroup.  NGW <= 6 (N <=
+// 192): wider stages never fit, their accumulator tile [128][N + 4] leaves no room for two ring stages (ly_layout and
+// iaf_dg_plan_create reject them before asking for a kernel)
+#define LY_MAX_NGW 6
 static LyKernel ly_kernel_for(bool padw, int mode, bool elu, int N) {
   switch ((N + 31) / 32) {
     case 1: return ly_kernel_pick<1, false>(padw, mode, elu);
@@ -361,9 +364,7 @@ static LyKernel ly_kernel_for(bool padw, int mode, bool elu, int N) {
     case 3: return ly_kernel_pick<3, false>(padw, mode, elu);
     case 4: return ly_kernel_pick<4, false>(padw, mode, elu);
     case 5: return ly_kernel_pick<5, false>(padw, mode, elu);
-    case 6: return ly_kernel_pick<6, false>(padw, mode, elu);
-    case 7: return ly_kernel_pick<7, false>(padw, mode, elu);
-    default: return ly_kernel_pick<8, false>(padw, mode, elu);
+    default: return ly_kernel_pick<LY_MAX_NGW, false>(padw, mode, elu);
   }
 }
 // the one-launch step of a one-hidden-layer stack (hidden and 2 n_z at most 64 columns: two groups per warpgroup)
@@ -375,9 +376,9 @@ static int tc_round_up(int a, int b) { return (a + b - 1) / b * b; }
 // per stage: an A window (first stage), the bias table, the partial scratch, the accumulator tile, an NB-deep ring
 static bool ly_layout(const iaf_desc_t* d, IafTcPlan* pl) {
   if (d->n_hidden < 1 || d->n_heads != 2 || d->head[0] != d->n_z || d->head[1] != d->n_z) return false;
-  if (d->n_z % 16 != 0 || 2 * d->n_z > 256) return false;
+  if (d->n_z % 16 != 0 || 2 * d->n_z > 32 * LY_MAX_NGW) return false;
   for (int i = 0; i < d->n_hidden; ++i)
-    if (d->hidden[i] % 16 != 0 || d->hidden[i] > 256) return false;
+    if (d->hidden[i] % 16 != 0 || d->hidden[i] > 32 * LY_MAX_NGW) return false;
   const int nst = d->n_hidden + 1;
   const int Wp = d->W + 1;
   const int SPS = (d->H + 1) * Wp;
@@ -692,22 +693,46 @@ struct IafDgPlan {
   __nv_bfloat16* img[2][2];  // ping-pong operand images [buffer][hi | lo]
   __nv_bfloat16* ximg[2];    // weight gradient: operand image of the current layer's input [hi | lo]
   int img_S_pad, scratch_B;
+  float* wscale;             // [IAF_MAX_STAGES]: the power of two each stage's weight images carry
   float* amax;               // [B]
   float* bstep;              // [B][5][kin[last]]: per-sample bias / pad-channel sums of the fused step prologue
   int step_optin;            // the prologue kernel's dynamic shared memory limit has been raised
   int num_sms;
 };
 
-__global__ void __launch_bounds__(256) iaf_dg_pack_kernel(const float* __restrict__ w, __nv_bfloat16* whi, __nv_bfloat16* wlo, int cin,
-                                                          int ncol) {
-  // w: effective (masked, normalised) forward weights [tap][cin][ncol] fp32.  B operand of the data gradient: K index
-  // [column / 16][tap][column % 16] (the layered kernel's K order), N index = ci; images [K/8][N][8], fp16 hi / lo.
+// Weight scale of a data-gradient stage: the power of two that brings the layer's largest effective weight into [32, 64)
+// (dg_scale_from_amax).  The lo half of the fp16 split is subnormal below |w| ~ 2^-3 (absolute step 2^-24), so a
+// small-gain layer (heads of gain 1e-3: |w| ~ 1e-4) would otherwise lose most of its 22 bits; the stage's epilogue
+// divides it out again (exact).  One block: the weights of a stage are at most 5 x 256 x 256 floats.
+__global__ void __launch_bounds__(1024) iaf_dg_wscale_kernel(const float4* __restrict__ w, int total4, float* wscale) {
+  __shared__ float red[32];
+  float m = 0.f;
+  for (int i = threadIdx.x; i < total4; i += 1024) {
+    const float4 v = __ldg(w + i);
+    m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+  }
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    m = red[threadIdx.x];
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if (threadIdx.x == 0) *wscale = dg_scale_from_amax(m);
+  }
+}
+
+__global__ void __launch_bounds__(256) iaf_dg_pack_kernel(const float* __restrict__ w, const float* __restrict__ wscale,
+                                                          __nv_bfloat16* whi, __nv_bfloat16* wlo, int cin, int ncol) {
+  // w: effective (masked, normalised) forward weights [tap][cin][ncol] fp32, times the stage's weight scale.  B operand of
+  // the data gradient: K index [column / 16][tap][column % 16] (the layered kernel's K order), N index = ci; images
+  // [K/8][N][8], fp16 hi / lo.
   const int total = IAF_NTAPS * cin * ncol;
+  const float sw = __ldg(wscale);
   for (int i = blockIdx.x * 256 + threadIdx.x; i < total; i += gridDim.x * 256) {
     const int kc = i % ncol;
     const int ci = (i / ncol) % cin;
     const int t = i / (ncol * cin);
-    const float vc = fminf(fmaxf(w[i], -65000.f), 65000.f);
+    const float vc = fminf(fmaxf(w[i] * sw, -65000.f), 65000.f);
     const __half hh = __float2half_rn(vc);
     const __half lh = __float2half_rn(vc - __half2float(hh));
     const int k = ((kc >> 4) * IAF_NTAPS + t) * 16 + (kc & 15);
@@ -792,6 +817,7 @@ void iaf_dg_plan_destroy(IafDgPlan* pl) {
     if (pl->wlo[j]) cudaFree(pl->wlo[j]);
   }
   if (pl->zeros) cudaFree(pl->zeros);
+  if (pl->wscale) cudaFree(pl->wscale);
   if (pl->amax) cudaFree(pl->amax);
   if (pl->bstep) cudaFree(pl->bstep);
   for (int a = 0; a < 2; ++a)
@@ -827,7 +853,7 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
     pl->kin[j] = kin; pl->nout[j] = N;
     pl->max_ch = std::max(pl->max_ch, std::max(kin, N));
     maxn = std::max(maxn, N);
-    if (kin % 16 || N % 16 || kin > 256 || N > 256 || N < 16) { iaf_dg_plan_destroy(pl); return IAF_ERR_UNSUPPORTED; }
+    if (kin % 16 || N % 16 || kin > 256 || N > 32 * LY_MAX_NGW || N < 16) { iaf_dg_plan_destroy(pl); return IAF_ERR_UNSUPPORTED; }
     int off = 0;
     pl->sm_bias[j] = off; off += 5 * N * 4;
     off = tc_round_up(off, 16);
@@ -849,7 +875,8 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
     }
   }
   if (cudaMalloc(&pl->zeros, sizeof(float) * 5 * maxn) != cudaSuccess ||
-      cudaMemset(pl->zeros, 0, sizeof(float) * 5 * maxn) != cudaSuccess) {
+      cudaMemset(pl->zeros, 0, sizeof(float) * 5 * maxn) != cudaSuccess ||
+      cudaMalloc(&pl->wscale, sizeof(float) * IAF_MAX_STAGES) != cudaSuccess) {
     iaf_dg_plan_destroy(pl);
     return IAF_ERR_CUDA;
   }
@@ -923,7 +950,9 @@ int iaf_dg_stage(IafDgPlan* pl, int j, const float* w_packed, int in_buf, const 
   const int kin = pl->kin[j], N = pl->nout[j];
   {
     const int total = IAF_NTAPS * N * kin;
-    iaf_dg_pack_kernel<<<std::min(592, (total + 255) / 256), 256, 0, stream>>>(w_packed, pl->whi[j], pl->wlo[j], N, kin);
+    iaf_dg_wscale_kernel<<<1, 1024, 0, stream>>>(reinterpret_cast<const float4*>(w_packed), total / 4, pl->wscale + j);
+    iaf_dg_pack_kernel<<<std::min(592, (total + 255) / 256), 256, 0, stream>>>(w_packed, pl->wscale + j, pl->whi[j],
+                                                                              pl->wlo[j], N, kin);
     if (cudaGetLastError() != cudaSuccess) return IAF_ERR_CUDA;
   }
   const int SPS = (d.H + 1) * (d.W + 1);
@@ -960,6 +989,7 @@ int iaf_dg_stage(IafDgPlan* pl, int j, const float* w_packed, int in_buf, const 
   q.n_bchunks = kin / 16;
   q.bwd = hprev ? 1 : 2;
   q.amax = pl->amax;
+  q.wscale = pl->wscale + j;
   q.TS = TC_TILE; q.TO = TC_TILE;
   LyKernel lk = ly_kernel_for(false, IAF_MODE_MULTICONV, d.nl == IAF_NL_ELU, N);
   const int grid = std::min(pl->num_sms, NT);

@@ -60,6 +60,7 @@ struct IafLyParams {
   // nl' multiplies the result (bwd 1) or is null (bwd 2: gradient at the stack input, ACCUMULATED into hid_out)
   int bwd;                     // 0 forward, 1 x nl'(h), 2 identity and accumulate
   const float* amax;           // [B] per-sample max |gradient at the heads| (the scale is 2^(5 - floor(log2 amax)))
+  const float* wscale;         // the power of two the stage's weight images carry (iaf_dg_wscale_kernel), undone here
 };
 
 // floats per row of the shared-memory accumulator tile: N + 4 keeps a warp's 16-byte row reads conflict-free
@@ -365,13 +366,15 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             uint32_t r[16];
             acc_ld16(c0, r, pitch);
             if (q.bwd) {
-              // data gradient: acc = W^T g (scaled units); x nl'(h), evaluated from the activation itself
+              // data gradient: acc = (c W)^T g (scaled units); / c (exact: a power of two), x nl'(h), evaluated from the
+              // activation itself
               const float sc = si.valid ? dg_scale_from_amax(__ldg(q.amax + si.n)) : 1.0f;
               const float inv = 1.0f / sc;
+              const float winv = 1.0f / __ldg(q.wscale);
               float vb[16];
   #pragma unroll
               for (int e = 0; e < 16; ++e) {
-                const float a = __uint_as_float(r[e]);
+                const float a = __uint_as_float(r[e]) * winv;
                 const float d = (q.bwd == 1) ? dg_nl_grad(cx[e], p.nl) : 1.0f;
                 vb[e] = si.valid ? a * d : 0.f;
               }
