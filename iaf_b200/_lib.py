@@ -15,6 +15,15 @@ PATH_NAMES = {1: "simt", 2: "tc"}
 ENTRIES = {"multiconv": 0, "step": 1, "layer": 2}
 
 OK, ERR_BAD_ARG, ERR_BAD_SHAPE, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOT_PACKED, ERR_NO_DEVICE = 0, -1, -2, -3, -4, -5, -6
+ERR_CAPTURED = -7
+
+CAPTURE_HINT = ("call every entry point you capture (forward and backward) once at the largest batch size before "
+                "capturing, and use a second IAFOperator for a batch larger than the one captured")
+
+
+class CaptureError(RuntimeError):
+    """A call would allocate scratch inside a CUDA-graph capture, or grow the scratch of an operator a graph has captured
+    (growing frees buffers the graph still uses).  Nothing was launched."""
 
 
 class IafDesc(C.Structure):
@@ -87,4 +96,6 @@ def check(status):
         raise ValueError("iaf_b200: " + msg)
     if status == ERR_UNSUPPORTED:
         raise NotImplementedError("iaf_b200: " + msg)
+    if status == ERR_CAPTURED:
+        raise CaptureError("iaf_b200: " + msg + " (" + CAPTURE_HINT + ")")
     raise RuntimeError("iaf_b200: " + msg)

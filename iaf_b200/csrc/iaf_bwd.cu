@@ -892,6 +892,14 @@ void iaf_bwd_plan_destroy(IafBwdPlan* pl) {
   delete pl;
 }
 
+// The tensor-core data gradient's scratch (operand images, per-sample scales) is sized for B by every run that sizes this
+// plan's (iaf_dg_begin / iaf_dg_begin_step): it fits exactly when this plan's does, and is first allocated with it.
+int iaf_bwd_scratch_need(const IafBwdPlan* pl, int mode, int B) {
+  int need = iaf_scratch_need(pl->scratch_B, B);
+  if (mode == IAF_MODE_LAYER) need = std::max(need, iaf_scratch_need(pl->z0_B, B));
+  return need;
+}
+
 static int bw_ensure_scratch(IafBwdPlan* pl, int B) {
   if (B <= pl->scratch_B) return IAF_OK;
   bw_free_scratch(pl);

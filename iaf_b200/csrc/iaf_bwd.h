@@ -52,3 +52,4 @@ int iaf_bwd_plan_create(IafBwdPlan** out, const iaf_desc_t* d, const int* cin, c
 int iaf_bwd_plan_uses_tc(const IafBwdPlan* p);  // 0: SIMT, 1: data gradient on tensor cores, 2: data and weight gradient
 void iaf_bwd_plan_destroy(IafBwdPlan* p);
 int iaf_bwd_run(IafBwdPlan* p, const IafBwdArgs* a, cudaStream_t stream, int* n_launches);
+int iaf_bwd_scratch_need(const IafBwdPlan* p, int mode, int B);  // IAF_SCRATCH_*: what iaf_bwd_run of `mode` at B does

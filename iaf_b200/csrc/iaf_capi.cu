@@ -89,6 +89,9 @@ struct iaf_plan {
   cudaStream_t last_stream;
   bool last_stream_valid;
   cudaEvent_t ev_handoff;
+  // a call of this plan has been captured into a CUDA graph: the graph keeps the scratch pointers it saw, so from then on
+  // no scratch may be freed or replaced (see capture_guard)
+  bool captured;
 };
 #define IAF_NSLOT 3
 
@@ -140,7 +143,34 @@ static int stream_handoff(iaf_plan* pl, cudaStream_t stream) {
   return IAF_OK;
 }
 
-static int ensure_scratch(iaf_plan* pl, int B) {
+// Scratch is allocated on first use and freed and re-allocated when the batch grows (need: IAF_SCRATCH_*).  cudaMalloc is
+// illegal inside a capture, and a graph captured earlier would replay into the freed buffers, so a call fails with
+// IAF_ERR_CAPTURED, before it issues anything, when it needs any allocation while its stream is capturing, or a
+// re-allocation once a call of the plan was captured.  Checked before stream_handoff: a refused call leaves no trace.
+static int capture_guard(iaf_plan* pl, cudaStream_t stream, int need) {
+  bool capturing = false;
+#ifndef IAF_EMU  // (the host emulation has no graphs: nothing is ever captured there)
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CK(cudaStreamIsCapturing(stream, &cs));
+  capturing = cs != cudaStreamCaptureStatusNone;
+#endif
+  if ((capturing && need != IAF_SCRATCH_FITS) || (pl->captured && need == IAF_SCRATCH_REALLOC)) return IAF_ERR_CAPTURED;
+  if (capturing) pl->captured = true;
+  return IAF_OK;
+}
+
+// what a forward call of `mode` at batch B does to the scratch
+static int fwd_need(const iaf_plan* pl, int mode, int B) {
+#ifndef IAF_EMU  // (the host emulation has no tensor-core plans)
+  if (pl->path == IAF_PATH_TC && iaf_tc_mode_supported(pl->tc, mode)) return iaf_tc_scratch_need(pl->tc, B);
+#else
+  (void)mode;
+#endif
+  return iaf_scratch_need(pl->scratch_B, B);
+}
+
+// the zero-fill is ordered on the caller's stream: a kernel launched there must not see the counters before it lands
+static int ensure_scratch(iaf_plan* pl, int B, cudaStream_t stream) {
   if (B <= pl->scratch_B) return IAF_OK;
   if (pl->partial) cudaFree(pl->partial);
   if (pl->counter) cudaFree(pl->counter);
@@ -148,7 +178,7 @@ static int ensure_scratch(iaf_plan* pl, int B) {
   const int maxbands = pl->d.H;  // worst case band_rows = 1
   CK(cudaMalloc(&pl->partial, sizeof(float) * (size_t)B * maxbands * std::max(1, pl->d.head[0])));
   CK(cudaMalloc(&pl->counter, sizeof(unsigned) * (size_t)B));
-  CK(cudaMemset(pl->counter, 0, sizeof(unsigned) * (size_t)B));
+  CK(cudaMemsetAsync(pl->counter, 0, sizeof(unsigned) * (size_t)B, stream));
   pl->scratch_B = B;
   return IAF_OK;
 }
@@ -166,6 +196,9 @@ const char* iaf_strerror(int status) {
     case IAF_ERR_CUDA: return "CUDA error (see iaf_last_cuda_error)";
     case IAF_ERR_NOT_PACKED: return "iaf_pack_weights has not been called on this plan";
     case IAF_ERR_NO_DEVICE: return "no CUDA device";
+    case IAF_ERR_CAPTURED:
+      return "the call would allocate scratch inside a CUDA-graph capture, or grow (free and re-allocate) the scratch of a "
+             "plan that a graph has captured";
     default: return "unknown status";
   }
 }
@@ -360,6 +393,7 @@ static int run(iaf_plan* pl, int mode, const float* z, const float* ctx, const f
                cudaStream_t stream, float* const* hid_out = nullptr) {
   if (!pl->packed) return IAF_ERR_NOT_PACKED;
   if (B <= 0) return IAF_ERR_BAD_ARG;
+  { int cg = capture_guard(pl, stream, fwd_need(pl, mode, B)); if (cg != IAF_OK) return cg; }
   { int hs = stream_handoff(pl, stream); if (hs != IAF_OK) return hs; }
   const iaf_desc_t& d = pl->d;
   // a plan the caller pinned to the tensor-core path never downgrades silently (see iaf_plan_path_for_entry)
@@ -379,7 +413,7 @@ static int run(iaf_plan* pl, int mode, const float* z, const float* ctx, const f
     return st;
   }
   if (!pl->simt_ok) return IAF_ERR_UNSUPPORTED;
-  int st = ensure_scratch(pl, B);
+  int st = ensure_scratch(pl, B, stream);
   if (st != IAF_OK) return st;
   IafSimtParams p;
   memset(&p, 0, sizeof(p));
@@ -448,6 +482,21 @@ int iaf_step_fwd_train(iaf_plan_t* pl, const float* z, const float* context, flo
              nullptr, logdet_out, B, (cudaStream_t)stream, hidden_out);
 }
 
+// iaf_step_bwd on a tensor-core plan recomputes z', arw_logsd and the activations with the forward's own kernels
+static bool bwd_recomputes(const iaf_plan* pl, int mode, bool have_saved) {
+  return mode == IAF_MODE_STEP && !have_saved && pl->path == IAF_PATH_TC && iaf_tc_mode_supported(pl->tc, IAF_MODE_STEP) &&
+         iaf_bwd_plan_uses_tc(pl->bwd);
+}
+
+// what a backward call of `mode` at batch B does to the backward plan and every scratch it touches
+static int bwd_need(const iaf_plan* pl, int mode, bool have_saved, int B) {
+  if (!pl->bwd) return IAF_SCRATCH_ALLOC;
+  int need = iaf_bwd_scratch_need(pl->bwd, mode, B);
+  if (bwd_recomputes(pl, mode, have_saved))
+    need = std::max(need, std::max(iaf_scratch_need(pl->rc_B, B), fwd_need(pl, IAF_MODE_STEP, B)));
+  return need;
+}
+
 static int run_bwd(iaf_plan* pl, int mode, const float* z, const float* ctx, const float* const* w,
                    const float* const* scale, const float* g_zout, const float* g_logsd, const float* g_logdet,
                    const float* const* g_heads, float* g_z, float* g_ctx, float* const* g_w, float* const* g_scale,
@@ -455,6 +504,7 @@ static int run_bwd(iaf_plan* pl, int mode, const float* z, const float* ctx, con
                    const float* logsd_saved = nullptr, const float* const* hidden_saved = nullptr) {
   if (!pl->packed) return IAF_ERR_NOT_PACKED;
   if (B <= 0) return IAF_ERR_BAD_ARG;
+  { int cg = capture_guard(pl, stream, bwd_need(pl, mode, z_out_saved != nullptr, B)); if (cg != IAF_OK) return cg; }
   { int hs = stream_handoff(pl, stream); if (hs != IAF_OK) return hs; }
   const iaf_desc_t& d = pl->d;
   const int n_layers = d.n_hidden + d.n_heads;
@@ -482,8 +532,7 @@ static int run_bwd(iaf_plan* pl, int mode, const float* z, const float* ctx, con
   a.z_out_saved = z_out_saved; a.logsd_saved = logsd_saved;
   for (int j = 0; j < d.n_hidden && hidden_saved; ++j) a.h_saved[j] = hidden_saved[j];
   a.have_saved = z_out_saved != nullptr;
-  if (mode == IAF_MODE_STEP && !z_out_saved && pl->path == IAF_PATH_TC && iaf_tc_mode_supported(pl->tc, IAF_MODE_STEP) &&
-      iaf_bwd_plan_uses_tc(pl->bwd)) {
+  if (bwd_recomputes(pl, mode, z_out_saved != nullptr)) {
     // a tensor-core plan recomputes z', arw_logsd and the activations with its own forward (one training-forward call)
     // instead of the SIMT layer convs: what iaf_step_fwd_train would have kept
     if (B > pl->rc_B) {
@@ -551,6 +600,7 @@ int iaf_layer_bwd(iaf_plan_t* pl, const float* eps, const float* post_mean, cons
   if (pl->d.n_heads != 2 || pl->d.head[0] != pl->d.n_z) return IAF_ERR_BAD_SHAPE;
   if (!pl->packed) return IAF_ERR_NOT_PACKED;
   if (B <= 0) return IAF_ERR_BAD_ARG;
+  { int cg = capture_guard(pl, (cudaStream_t)stream, bwd_need(pl, IAF_MODE_LAYER, false, B)); if (cg != IAF_OK) return cg; }
   { int hs = stream_handoff(pl, (cudaStream_t)stream); if (hs != IAF_OK) return hs; }
   const iaf_desc_t& d = pl->d;
   const bool want_params = g_w || g_scale || g_bias;

@@ -85,6 +85,13 @@ struct IafSimtParams {
 
 enum { IAF_MODE_MULTICONV = 0, IAF_MODE_STEP = 1, IAF_MODE_LAYER = 2 };
 
+// What a call at batch B would do to a set of scratch buffers sized for have_B samples (0: none yet): nothing, a first
+// allocation, or a re-allocation that frees the old buffers.  Sets combine with std::max.
+enum { IAF_SCRATCH_FITS = 0, IAF_SCRATCH_ALLOC = 1, IAF_SCRATCH_REALLOC = 2 };
+static inline int iaf_scratch_need(int have_B, int B) {
+  return B <= have_B ? IAF_SCRATCH_FITS : (have_B > 0 ? IAF_SCRATCH_REALLOC : IAF_SCRATCH_ALLOC);
+}
+
 // Raw-parameter description handed to the pack kernel.
 struct IafPackLayer {
   const float* w;      // reference layout (TF [3,3,Cin,Cout] | Theano [Cout,Cin+1,3,3])

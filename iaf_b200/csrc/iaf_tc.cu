@@ -551,14 +551,28 @@ bool iaf_tc_mode_supported(const IafTcPlan* pl, int mode) {
   return mode == IAF_MODE_STEP || mode == IAF_MODE_MULTICONV || (mode == IAF_MODE_LAYER && pl->layer_ok);
 }
 
+// tiles of a call at batch B (0: the slot stream overflows int)
+static int tc_num_tiles(const IafTcPlan* pl, int B) {
+  const int SPS = (pl->d.H + 1) * (pl->d.W + 1);
+  if ((long long)B * SPS + TC_TILE >= (1LL << 31)) return 0;
+  const int TS = pl->fused ? TC_TILE - pl->MIR : TC_TILE;  // slots a tile advances (fused: overlapped windows)
+  return (B * SPS + TS - 1) / TS;
+}
+
+int iaf_tc_scratch_need(const IafTcPlan* pl, int B) {
+  const int NT = tc_num_tiles(pl, B);
+  if (NT == 0 || (B <= pl->scratch_B && NT <= pl->scratch_NT)) return IAF_SCRATCH_FITS;  // (overflow: refused, no growth)
+  return pl->scratch_B > 0 ? IAF_SCRATCH_REALLOC : IAF_SCRATCH_ALLOC;
+}
+
 int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_launches) {
   const iaf_desc_t& d = pl->d;
   const int B = a->B;
   const int SPS = (d.H + 1) * (d.W + 1);
-  if ((long long)B * SPS + TC_TILE >= (1LL << 31)) return IAF_ERR_UNSUPPORTED;
+  const int NT = tc_num_tiles(pl, B);
+  if (NT == 0) return IAF_ERR_UNSUPPORTED;
   const int S = B * SPS;
-  const int TS = pl->fused ? TC_TILE - pl->MIR : TC_TILE;  // slots a tile advances (fused: overlapped windows)
-  const int NT = (S + TS - 1) / TS;
+  const int TS = pl->fused ? TC_TILE - pl->MIR : TC_TILE;
   if (B > pl->scratch_B || NT > pl->scratch_NT) {
     if (pl->counter) cudaFree(pl->counter);
     if (pl->tilepart) cudaFree(pl->tilepart);
@@ -572,10 +586,10 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
         if (pl->img[a2][b2]) cudaFree(pl->img[a2][b2]);
         pl->img[a2][b2] = nullptr;
         if (cudaMalloc(&pl->img[a2][b2], bytes) != cudaSuccess) return IAF_ERR_CUDA;
-        if (cudaMemset(pl->img[a2][b2], 0, bytes) != cudaSuccess) return IAF_ERR_CUDA;
+        if (cudaMemsetAsync(pl->img[a2][b2], 0, bytes, stream) != cudaSuccess) return IAF_ERR_CUDA;
       }
     if (cudaMalloc(&pl->counter, sizeof(unsigned) * (size_t)B) != cudaSuccess) return IAF_ERR_CUDA;
-    if (cudaMemset(pl->counter, 0, sizeof(unsigned) * (size_t)B) != cudaSuccess) return IAF_ERR_CUDA;
+    if (cudaMemsetAsync(pl->counter, 0, sizeof(unsigned) * (size_t)B, stream) != cudaSuccess) return IAF_ERR_CUDA;
     if (cudaMalloc(&pl->tilepart, sizeof(float) * (size_t)NT * pl->MAXS * d.n_z) != cudaSuccess) return IAF_ERR_CUDA;
     pl->scratch_B = B;
     pl->scratch_NT = NT;
@@ -685,7 +699,8 @@ struct IafDgPlan {
   int kin[IAF_MAX_STAGES], nout[IAF_MAX_STAGES];  // dgrad of layer j: input planes (= packed columns of layer j), output channels (= cin of layer j)
   __nv_bfloat16* whi[IAF_MAX_STAGES];
   __nv_bfloat16* wlo[IAF_MAX_STAGES];
-  float* zeros;  // bias table of the stages (the kernel adds it; the gradient has none)
+  float* zeros;  // bias table of the stages (the kernel adds it; the gradient has none): [5][maxn]
+  int maxn;
   int sm_bias[IAF_MAX_STAGES], sm_part[IAF_MAX_STAGES], sm_acc[IAF_MAX_STAGES], sm_b[IAF_MAX_STAGES], stage[IAF_MAX_STAGES],
       NB[IAF_MAX_STAGES];
   size_t smem[IAF_MAX_STAGES];
@@ -874,8 +889,9 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
       return IAF_ERR_CUDA;
     }
   }
+  pl->maxn = maxn;
+  // (zeros is filled on the first call's stream, by dg_ensure_scratch: the create has no stream to order it on)
   if (cudaMalloc(&pl->zeros, sizeof(float) * 5 * maxn) != cudaSuccess ||
-      cudaMemset(pl->zeros, 0, sizeof(float) * 5 * maxn) != cudaSuccess ||
       cudaMalloc(&pl->wscale, sizeof(float) * IAF_MAX_STAGES) != cudaSuccess) {
     iaf_dg_plan_destroy(pl);
     return IAF_ERR_CUDA;
@@ -894,12 +910,14 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
   return IAF_OK;
 }
 
-static int dg_ensure_scratch(IafDgPlan* pl, int B) {
+// every zero-fill goes to the caller's stream, ahead of the kernels that read it
+static int dg_ensure_scratch(IafDgPlan* pl, int B, cudaStream_t stream) {
   if (B <= pl->scratch_B) return IAF_OK;
   const int SPS = (pl->d.H + 1) * (pl->d.W + 1);
   if ((long long)B * SPS + TC_TILE >= (1LL << 31)) return IAF_ERR_UNSUPPORTED;
   const int NT = (B * SPS + TC_TILE - 1) / TC_TILE;
   pl->scratch_B = 0;  // a failure below must not leave the old size standing over freed buffers
+  if (cudaMemsetAsync(pl->zeros, 0, sizeof(float) * 5 * pl->maxn, stream) != cudaSuccess) return IAF_ERR_CUDA;
   pl->img_S_pad = (NT + 1) * TC_TILE;  // one zero tile past the end: windows of the last tile read into it
   const size_t bytes = (size_t)(pl->max_ch / 8) * pl->img_S_pad * 16;
   for (int a = 0; a < 2; ++a)
@@ -907,13 +925,13 @@ static int dg_ensure_scratch(IafDgPlan* pl, int B) {
       if (pl->img[a][b]) cudaFree(pl->img[a][b]);
       pl->img[a][b] = nullptr;
       if (cudaMalloc(&pl->img[a][b], bytes) != cudaSuccess) return IAF_ERR_CUDA;
-      if (cudaMemset(pl->img[a][b], 0, bytes) != cudaSuccess) return IAF_ERR_CUDA;
+      if (cudaMemsetAsync(pl->img[a][b], 0, bytes, stream) != cudaSuccess) return IAF_ERR_CUDA;
     }
   for (int a = 0; a < 2; ++a) {
     if (pl->ximg[a]) cudaFree(pl->ximg[a]);
     pl->ximg[a] = nullptr;
     if (cudaMalloc(&pl->ximg[a], bytes) != cudaSuccess) return IAF_ERR_CUDA;
-    if (cudaMemset(pl->ximg[a], 0, bytes) != cudaSuccess) return IAF_ERR_CUDA;
+    if (cudaMemsetAsync(pl->ximg[a], 0, bytes, stream) != cudaSuccess) return IAF_ERR_CUDA;
   }
   if (pl->amax) cudaFree(pl->amax);
   if (pl->bstep) cudaFree(pl->bstep);
@@ -927,7 +945,7 @@ static int dg_ensure_scratch(IafDgPlan* pl, int B) {
 // gradient at the heads (fp32 [B][kin[last]][HW]) -> per-sample scale + operand image 0
 int iaf_dg_begin(IafDgPlan* pl, const float* g_heads, int B, cudaStream_t stream) {
   const iaf_desc_t& d = pl->d;
-  int st = dg_ensure_scratch(pl, B);
+  int st = dg_ensure_scratch(pl, B, stream);
   if (st != IAF_OK) return st;
   IafDgImageParams q;
   memset(&q, 0, sizeof(q));
@@ -1158,7 +1176,7 @@ int iaf_dg_begin_step(IafDgPlan* pl, const float* z_out, const float* logsd, con
                       const float* g_logdet, float* g_z, float* hb, int head_pad, int B, cudaStream_t stream,
                       const float** bias_partials) {
   const iaf_desc_t& d = pl->d;
-  int st = dg_ensure_scratch(pl, B);
+  int st = dg_ensure_scratch(pl, B, stream);
   if (st != IAF_OK) return st;
   if (!pl->step_optin) {
     if (iaf_smem_optin(iaf_dg_step_kernel) != cudaSuccess) return IAF_ERR_CUDA;

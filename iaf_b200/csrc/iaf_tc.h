@@ -27,13 +27,13 @@ int iaf_tc_pack(IafTcPlan* p, const float* const* w, const float* const* scale, 
                 cudaStream_t stream);
 bool iaf_tc_mode_supported(const IafTcPlan* p, int mode);
 int iaf_tc_run(IafTcPlan* p, const IafTcArgs* a, cudaStream_t stream, int* n_launches);
+int iaf_tc_scratch_need(const IafTcPlan* p, int B);  // IAF_SCRATCH_*: what iaf_tc_run at batch B does to the scratch
 
 // Data gradient of the conv stack on the tensor cores (used by iaf_bwd.cu when the shapes allow it; IAF_BWD_TC=0 keeps
 // the exact-fp32 SIMT kernels).  cin / ncol: per stage, the forward layer's input channels and packed output columns.
 struct IafDgPlan;
 int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, const int* ncol, int n_stages);
-void iaf_dg_plan_destroy(IafDgPlan* p);
-int iaf_dg_begin(IafDgPlan* p, const float* g_heads, int B, cudaStream_t stream);
+void iaf_dg_plan_destroy(IafDgPlan* p);int iaf_dg_begin(IafDgPlan* p, const float* g_heads, int B, cudaStream_t stream);
 int iaf_dg_stage(IafDgPlan* p, int j, const float* w_packed, int in_buf, const float* hprev, float* out, int write_image,
                  int B, cudaStream_t stream);
 int iaf_wg_run(IafDgPlan* p, int j, const float* x, int g_buf, float* part, int part_stride, int ng_max, int B,

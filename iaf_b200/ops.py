@@ -122,7 +122,14 @@ class IAFOperator(object):
         """Plan for (H, W, device) with the packed weights of ``layers`` (default: the current set_weights())."""
         key = (H, W, device.index)
         ent = self._plans.get(key)
+        capturing = False
+        if device.type == "cuda":
+            with torch.cuda.device(device):
+                capturing = torch.cuda.is_current_stream_capturing()
         if ent is None:
+            if capturing:  # iaf_plan_create allocates (illegal inside a capture) and takes no stream to check
+                raise _lib.CaptureError("iaf_b200: the first call of an IAFOperator for a map size cannot run inside a "
+                                        "CUDA-graph capture (" + _lib.CAPTURE_HINT + ")")
             d = _lib.IafDesc()
             d.variant = _lib.VARIANTS[self.variant]
             d.n_z = self.n_z
@@ -138,19 +145,20 @@ class IAFOperator(object):
             handle = C.c_void_p()
             with torch.cuda.device(device):
                 _lib.check(self._lib.iaf_plan_create(C.byref(handle), C.byref(d)))
-            ent = [handle, None]
+            ent = [handle, None, False]  # handle, key of the packed weights, packed inside a capture
             self._plans[key] = ent
         if layers is None:
             layers = self._layers
         if layers is None:
             raise RuntimeError("IAFOperator.set_weights() has not been called")
         wk = self._weights_key(layers)
-        if ent[1] != wk:
+        # a pack recorded into a graph only runs when the graph is replayed: the next call outside the capture packs again
+        if ent[1] != wk or (ent[2] and not capturing):
             n = len(layers)
             arr = lambda j: (C.c_void_p * n)(*[l[j].data_ptr() for l in layers])
             with torch.cuda.device(device):
                 _lib.check(self._lib.iaf_pack_weights(ent[0], arr(0), arr(1), arr(2), _stream(device)))
-            ent[1] = wk
+            ent[1], ent[2] = wk, capturing
         return ent[0]
 
     def __del__(self):

@@ -31,7 +31,9 @@ typedef enum {
   IAF_ERR_UNSUPPORTED = -3, /* valid in the reference but outside what the kernels cover       */
   IAF_ERR_CUDA = -4,        /* a CUDA runtime call failed; see iaf_last_cuda_error()           */
   IAF_ERR_NOT_PACKED = -5,  /* iaf_step_* called before iaf_pack_weights                       */
-  IAF_ERR_NO_DEVICE = -6    /* no sm_90 device                                                 */
+  IAF_ERR_NO_DEVICE = -6,   /* no sm_90 device                                                 */
+  IAF_ERR_CAPTURED = -7     /* the call would allocate scratch while its stream is capturing into a CUDA graph, or
+                               re-allocate scratch after a call of the plan was captured; nothing was issued        */
 } iaf_status;
 
 /* which of the reference's two implementations the numerics follow (SURVEY F2) */
@@ -71,7 +73,12 @@ typedef struct iaf_desc {
 /* opaque: packed weights, scratch, launch geometry.  A plan is NOT re-entrant: its scratch serves one call at a time.
  * Calls on the same stream are ordered by the stream; when consecutive calls use different streams the library makes the
  * later stream wait for the earlier one (one event), so results stay correct -- but two streams never run the same plan
- * concurrently.  Use one plan per concurrent stream. */
+ * concurrently.  Use one plan per concurrent stream.
+ * CUDA graphs: scratch is allocated on an entry's first call and re-allocated when the batch grows; a capture can do
+ * neither.  Call every entry you capture once at the largest batch before capturing.  A call that would allocate inside
+ * a capture, or re-allocate once any call of the plan was captured, returns IAF_ERR_CAPTURED (a larger batch after a
+ * capture needs a second plan).  Replays bypass this ABI, so the stream handoff above cannot see them: order replays
+ * and direct calls of one plan yourself (same stream, or an event).  Destroy the plan only after its graphs. */
 typedef struct iaf_plan iaf_plan_t;
 
 /* Validate the description and allocate the plan (replaces the graph-construction half of

@@ -36,9 +36,16 @@ def test_library_exports_every_declared_symbol(lib):
 
 def test_version_and_strerror(lib):
     assert lib.iaf_version() >= 100
-    for st in range(0, -7, -1):
-        assert lib.iaf_strerror(st)
+    for st in range(0, -8, -1):
+        assert lib.iaf_strerror(st) and b"unknown" not in lib.iaf_strerror(st)
     assert b"unknown" in lib.iaf_strerror(-99)
+
+
+def test_capture_refusal_raises_capture_error(lib):
+    """IAF_ERR_CAPTURED reaches python as CaptureError (a RuntimeError) telling the caller how to warm up."""
+    with pytest.raises(_lib.CaptureError, match="largest batch size"):
+        _lib.check(_lib.ERR_CAPTURED)
+    assert issubclass(_lib.CaptureError, RuntimeError)
 
 
 def _desc(**kw):
