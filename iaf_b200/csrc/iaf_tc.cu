@@ -46,6 +46,8 @@ struct IafTcStage {
   const __nv_bfloat16* wlo;
   const float* bias;         // [N] packed column order
   const float* padw;         // [4][N] or nullptr
+  const float* wsinv;        // [N] packed column order: the inverse of the power of two each weight column carries
+                             // (iaf_tc_pack_kernel), undone as the epilogues read the accumulator tile; nullptr = unscaled
   float* hid_out;            // training forward: this (hidden) stage's activations, fp32 [B][N][HW]; nullptr = not kept
   int cin, N, K;
 };
@@ -126,8 +128,10 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 // SBO >> 4 (base offset 0, layout type 0 = no swizzle).  Adding n to the low word moves the start by n x 16 bytes.
 // Why fp16 pairs and not bf16 pairs: the residual of a two-term WEIGHT split is the same for every pixel and so adds
 // up coherently over the 8192 elements of a sample's log-det (bf16 + bf16 leaves 2^-17 |w|, ~2e-4 absolute against the
-// fp64 oracle over 256 samples; fp16 + fp16 leaves 2^-23 |w|).  Weight-normalised weights are bounded by their gain
-// (|w| <= exp(g), exp(3s)); see split_store8 for the activations' range.
+// fp64 oracle over 256 samples; fp16 + fp16 leaves 2^-23 |w|).  That holds only while the lo half is a normal fp16
+// number: below |w| ~ 2^-3 it is subnormal, with a fixed absolute step of 2^-24, so iaf_tc_pack_kernel scales every
+// weight column by the power of two that brings its largest |w| into [32, 64) (also keeping gains far above e^11 inside
+// the fp16 range) and the stage epilogues divide it out exactly.  See split_store8 for the activations' range.
 __device__ __forceinline__ uint32_t wg_desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
   return ((saddr >> 4) & 0x3FFFu) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
 }
@@ -164,8 +168,9 @@ __device__ __forceinline__ float tc_apply_nl(float v, int nl) {
 // split 8 floats into fp16 hi / lo (22 significant bits together) and store both 16-byte vectors.  fp16, not bf16: the
 // a_lo * w_lo product the three-MMA scheme drops and the residual of the two-term split both shrink 64x (CPU simulation
 // tools/experiments/prec_sim.py: worst per-sample log-det error on C2a 1.3e-4 with bf16 pairs, 5e-6 with fp16 pairs).
-// Range: |x| >= 65520 becomes inf and the step's outputs NaN (loud, never silently wrong); values below 6e-5 keep an
-// absolute resolution of 3e-8.
+// Range: |x| >= 65520 becomes inf and that sample's outputs NaN (loud, never silently wrong; invalid slots are zeroed by
+// a select, so the NaN stays inside its sample).  Activations are not scaled: below |x| ~ 2^-3 the lo half is subnormal
+// and x keeps an absolute resolution of about 2^-25 (3e-8) instead of 22 significant bits.
 __device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, uint8_t* lo_ptr) {
   uint32_t h[4], l[4];
 #pragma unroll
@@ -233,7 +238,7 @@ __device__ __forceinline__ SlotInfo decode_slot(const IafTcParams& p, int s, int
 // ------------------------------------------------------------------------------------------
 struct TcPackLayer {
   const float* w; const float* scale; const float* bias;
-  __nv_bfloat16* whi; __nv_bfloat16* wlo; float* bias_out; float* padw_out;
+  __nv_bfloat16* whi; __nv_bfloat16* wlo; float* bias_out; float* padw_out; float* wsinv_out;
   int cin, cout, N, zerodiag, head, is_head;
 };
 struct TcPackParams {
@@ -263,28 +268,37 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
   const int tid = threadIdx.x;
   const int n_real = L.cin * IAF_NTAPS;
   const int n_pad = (p.variant == IAF_VARIANT_THEANO) ? 4 : 0;
-  float ss = 0.f;
+  float ss = 0.f, am = 0.f;  // sum of squares (normalisation, pad channel included) and max |w| of the column's real taps
   for (int e = tid; e < n_real + n_pad; e += blockDim.x) {
     float v;
     if (e < n_real) {
       const int t = e / L.cin, ci = e % L.cin;
       v = tc_raw_weight(L, p.variant, t, ci, co);
       if (t == 0 && !tc_centre_visible(ci, co, L.cin, L.cout, L.zerodiag)) v = 0.f;
+      am = fmaxf(am, fabsf(v));
     } else {
       v = tc_raw_weight(L, p.variant, e - n_real + 1, L.cin, co);
     }
     ss = fmaf(v, v, ss);
   }
-  __shared__ float red[128];
+  __shared__ float red[128], redm[128];
   red[tid] = ss;
+  redm[tid] = am;
   __syncthreads();
   for (int s = 64; s > 0; s >>= 1) {
-    if (tid < s) red[tid] += red[tid + s];
+    if (tid < s) {
+      red[tid] += red[tid + s];
+      redm[tid] = fmaxf(redm[tid], redm[tid + s]);
+    }
     __syncthreads();
   }
   ss = red[0];
   const float factor = (p.variant == IAF_VARIANT_TF) ? expf(L.scale[co]) / sqrtf(fmaxf(ss, 1e-12f))
                                                      : expf(3.0f * L.scale[co]) / (sqrtf(ss) + 1e-8f);
+  // the column's weight scale: its largest |w| into [32, 64), so that the lo half of every sizeable weight is a normal
+  // fp16 number and the largest stays inside the fp16 range.  fl(|v| factor) is monotone in |v|: redm[0] * factor is
+  // exactly the largest |v * factor| of the loop below.  The bias and the pad-channel terms stay unscaled fp32.
+  const float wsc = dg_scale_from_amax(redm[0] * factor);
   // heads are interleaved in groups of 8: column = (c/8)*16 + head*8 + c%8
   const int col = L.is_head ? ((co >> 3) * 16 + L.head * 8 + (co & 7)) : co;
   for (int e = tid; e < n_real + n_pad; e += blockDim.x) {
@@ -292,11 +306,10 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
       const int t = e / L.cin, ci = e % L.cin;
       float v = tc_raw_weight(L, p.variant, t, ci, co);
       if (t == 0 && !tc_centre_visible(ci, co, L.cin, L.cout, L.zerodiag)) v = 0.f;
-      v *= factor;
+      const float vc = v * factor * wsc;  // (a power of two: exact)
       // K order [ci / 16][tap][ci % 16]: one K-step of the stage kernel is one 16-channel block over the five taps
       const int k = ((ci >> 4) * IAF_NTAPS + t) * 16 + (ci & 15);
-      // fp16 hi + fp16 lo (22 significant bits); saturated at the fp16 range (a gain of e^11 is not a weight-norm layer)
-      const float vc = fminf(fmaxf(v, -65000.f), 65000.f);
+      // fp16 hi + fp16 lo (22 significant bits)
       const __half hh = __float2half_rn(vc);
       const __half lh = __float2half_rn(vc - __half2float(hh));
       const __nv_bfloat16 h = __ushort_as_bfloat16(__half_as_ushort(hh));  // raw 16-bit patterns travel in the bf16-typed images
@@ -309,7 +322,10 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
       L.padw_out[(size_t)(t - 1) * L.N + col] = tc_raw_weight(L, p.variant, t, L.cin, co) * factor;
     }
   }
-  if (tid == 0) L.bias_out[col] = L.bias[co];
+  if (tid == 0) {
+    L.bias_out[col] = L.bias[co];
+    L.wsinv_out[col] = 1.0f / wsc;
+  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -323,6 +339,7 @@ struct IafTcPlan {
   __nv_bfloat16* wlo[IAF_MAX_STAGES];
   float* bias[IAF_MAX_STAGES];
   float* padw[IAF_MAX_STAGES];
+  float* wsinv[IAF_MAX_STAGES];  // [N]: inverse weight scale of each packed column
   int MIR, WIN, MAXS;
   bool layer_ok;             // the per-(sample,channel) scratch of the fused-layer mode fits
   // one launch per stage: an A window (first stage), an NB-deep ring, the bias table, the partials, the accumulator tile
@@ -459,13 +476,14 @@ int iaf_tc_plan_create(IafTcPlan** out, const iaf_desc_t* d) {
   pl->num_sms = prop.multiProcessorCount;
   for (int j = 0; j < pl->n_stages; ++j) {
     const size_t wb = (size_t)pl->K[j] * pl->N[j] * 2;
-    // bias [N] and pad-channel weights [4][N] are ONE table [5][N]
+    // bias [N] and pad-channel weights [4][N] are ONE table [5][N]; the inverse weight scales [N] follow it
     if (cudaMalloc(&pl->whi[j], wb) != cudaSuccess || cudaMalloc(&pl->wlo[j], wb) != cudaSuccess ||
-        cudaMalloc(&pl->bias[j], sizeof(float) * 5 * pl->N[j]) != cudaSuccess) {
+        cudaMalloc(&pl->bias[j], sizeof(float) * 6 * pl->N[j]) != cudaSuccess) {
       iaf_tc_plan_destroy(pl);
       return IAF_ERR_CUDA;
     }
     pl->padw[j] = pl->bias[j] + pl->N[j];
+    pl->wsinv[j] = pl->bias[j] + 5 * pl->N[j];
   }
   for (int a = 0; a < 12; ++a) {
     const int md = (a >> 2) == 0 ? IAF_MODE_MULTICONV : ((a >> 2) == 1 ? IAF_MODE_STEP : IAF_MODE_LAYER);
@@ -486,7 +504,7 @@ void iaf_tc_plan_destroy(IafTcPlan* pl) {
   for (int j = 0; j < IAF_MAX_STAGES; ++j) {
     if (pl->whi[j]) cudaFree(pl->whi[j]);
     if (pl->wlo[j]) cudaFree(pl->wlo[j]);
-    if (pl->bias[j]) cudaFree(pl->bias[j]);  // padw[j] points into the same allocation
+    if (pl->bias[j]) cudaFree(pl->bias[j]);  // padw[j] and wsinv[j] point into the same allocation
   }
   if (pl->counter) cudaFree(pl->counter);
   if (pl->tilepart) cudaFree(pl->tilepart);
@@ -515,6 +533,7 @@ int iaf_tc_pack(IafTcPlan* pl, const float* const* w, const float* const* scale,
     const int j = is_head ? d.n_hidden : i;
     L.w = w[i]; L.scale = scale[i]; L.bias = bias[i];
     L.whi = pl->whi[j]; L.wlo = pl->wlo[j]; L.bias_out = pl->bias[j]; L.padw_out = pl->padw[j];
+    L.wsinv_out = pl->wsinv[j];
     L.cin = pl->cin[j];
     L.cout = is_head ? d.head[i - d.n_hidden] : d.hidden[i];
     L.N = pl->N[j];
@@ -631,7 +650,7 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
     q.t = p;
     for (int j = 0; j < 2; ++j) {
       IafTcStage& S_ = q.t.st[j];
-      S_.whi = pl->whi[j]; S_.wlo = pl->wlo[j]; S_.bias = pl->bias[j]; S_.padw = pl->padw[j];
+      S_.whi = pl->whi[j]; S_.wlo = pl->wlo[j]; S_.bias = pl->bias[j]; S_.padw = pl->padw[j]; S_.wsinv = pl->wsinv[j];
       S_.hid_out = j == 0 ? a->hid_out[0] : nullptr;
       S_.cin = pl->cin[j]; S_.N = pl->N[j]; S_.K = pl->K[j];
     }
@@ -657,7 +676,7 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
     q.TS = TC_TILE; q.TO = TC_TILE;
     IafTcStage& S_ = q.t.st[0];
     S_.whi = pl->whi[j]; S_.wlo = pl->wlo[j]; S_.bias = pl->bias[j];
-    S_.padw = pl->padw[j];
+    S_.padw = pl->padw[j]; S_.wsinv = pl->wsinv[j];
     S_.hid_out = (j < IAF_MAX_HIDDEN && j + 1 < pl->n_stages) ? a->hid_out[j] : nullptr;
     S_.cin = pl->cin[j]; S_.N = pl->N[j]; S_.K = pl->K[j];
     q.t.sm_part = pl->ly_sm_part[j];

@@ -93,6 +93,8 @@ __device__ __forceinline__ float dg_scale_from_amax(float amax) {
 //   ring: weight chunk c sits in ring stage gchunk % NB (parity from gchunk / NB), released after its MMAs complete;
 //   otherwise resident: chunk c sits in stage c behind barrier bar0 + c (parity 0).
 //   a_in_stage: the A chunk pair of K-step c rides in the ring stage before the weights; otherwise A is a window at a_addr.
+// The tile holds the products with the weight images as packed: the per-column weight scale is undone by the epilogues
+// as they read it (acc_ld16).
 template <int NGW>
 __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float* s_acc, int N, int n_chunks, bool ring, int NB,
                                             int& gchunk, int bar0, uint32_t b_addr0, uint32_t stage_bytes,
@@ -104,11 +106,19 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
   const uint32_t sh[IAF_NTAPS] = {0u, 1u, (uint32_t)(Wp - 1), (uint32_t)Wp, (uint32_t)(Wp + 1)};  // 16-byte units
   const uint32_t a_kstep = (2u * a_plane) >> 4, b_tstep = (2u * b_plane) >> 4;
   const uint32_t a_row = (uint32_t)(rh * 64);  // 64 slots = 64 descriptor units
-  float acc[NGW][8];
+  // The two correction products (lo x hi, hi x lo: 2^-11 of hi x hi) go to their own accumulators where registers allow:
+  // added one by one to the main sum, each is rounded at the main sum's magnitude by the tensor cores' accumulation, and
+  // over K = 160 those roundings reach ~2e-7 of a unit pre-activation -- enough to put a ReLU's derivative on the wrong
+  // side of a pre-activation that small.  Summed apart and added once at the end, they cost one rounding.
+  constexpr bool SPLIT = NGW <= 2;
+  float acc[NGW][8], acl[SPLIT ? NGW : 1][8];
 #pragma unroll
   for (int k = 0; k < NGW; ++k)
 #pragma unroll
-    for (int e = 0; e < 8; ++e) acc[k][e] = 0.f;
+    for (int e = 0; e < 8; ++e) {
+      acc[k][e] = 0.f;
+      if (SPLIT) acl[SPLIT ? k : 0][e] = 0.f;
+    }
   int prev_stg = -1;
   for (int c = 0; c < n_chunks; ++c) {
     const int stg = ring ? gchunk % NB : c;
@@ -135,8 +145,9 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
 #pragma unroll
       for (int k = 0; k < NGW; ++k) {
         const uint32_t go = bt + (uint32_t)k * 32u;  // every second group: 32 columns = 512 B
-        wgmma_m64n16k16<0>(acc[k], al, mk_desc(bh0 + go));
-        wgmma_m64n16k16<0>(acc[k], ah, mk_desc(bl0 + go));
+        float* corr = SPLIT ? acl[SPLIT ? k : 0] : acc[k];
+        wgmma_m64n16k16<0>(corr, al, mk_desc(bh0 + go));
+        wgmma_m64n16k16<0>(corr, ah, mk_desc(bl0 + go));
         wgmma_m64n16k16<0>(acc[k], ah, mk_desc(bh0 + go));
       }
     }
@@ -149,6 +160,12 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
   }
   wgmma_wait<0>();
   if (ring && prev_stg >= 0 && wl == 0 && lane == 0) mbar_arrive(&bars[LB_BEMPTY + prev_stg]);
+  if (SPLIT) {
+#pragma unroll
+    for (int k = 0; k < NGW; ++k)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[k][e] += acl[SPLIT ? k : 0][e];
+  }
   // fragment -> accumulator tile: acc[k][4j + 2h + e] = row 16 wl + lane / 4 + 8h, column 16 g + 8j + 2 (lane % 4) + e
   const int pitch = ly_acc_pitch(N);
   const int r0 = rh * 64 + wl * 16 + (lane >> 2);
@@ -273,12 +290,17 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     const int sl = qd * 32 + lane;
     float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
     float* s_acc = reinterpret_cast<float*>(smem + q.sm_acc);
-    // this thread's slot row of the accumulator tile, 16 columns from c0
-    auto acc_ld16 = [&](int c0, uint32_t* r, int pitch) {
+    // this thread's slot row of the accumulator tile, 16 columns from c0, times the columns' inverse weight scales
+    // (exact: powers of two; wsinv null = unscaled images, the data gradient's)
+    auto acc_ld16 = [&](int c0, uint32_t* r, int pitch, const float* wsinv) {
       const float4* s4 = reinterpret_cast<const float4*>(s_acc + sl * pitch + c0);
 #pragma unroll
       for (int e4 = 0; e4 < 4; ++e4) {
-        const float4 v4 = s4[e4];
+        float4 v4 = s4[e4];
+        if (wsinv) {
+          const float4 w4 = __ldg(reinterpret_cast<const float4*>(wsinv + c0) + e4);
+          v4.x *= w4.x; v4.y *= w4.y; v4.z *= w4.z; v4.w *= w4.w;
+        }
         r[4 * e4] = __float_as_uint(v4.x); r[4 * e4 + 1] = __float_as_uint(v4.y);
         r[4 * e4 + 2] = __float_as_uint(v4.z); r[4 * e4 + 3] = __float_as_uint(v4.w);
       }
@@ -364,7 +386,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             for (int e = 0; e < 16; ++e) cx[e] = cxn[e];
             fetch_ctx(g + CGS);
             uint32_t r[16];
-            acc_ld16(c0, r, pitch);
+            acc_ld16(c0, r, pitch, St.wsinv);
             if (q.bwd) {
               // data gradient: acc = (c W)^T g (scaled units); / c (exact: a power of two), x nl'(h), evaluated from the
               // activation itself
@@ -400,7 +422,9 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             {
               // branch-free: bias rows come in as 16-byte vectors, the pad-channel terms (conv.py:77-83: the pad
               // channel is 1 where a tap falls outside the image) are 0/1-weighted FMAs, and an invalid slot
-              // (pad column, zero row, past the end) is multiplied to zero: that zero IS the conv's padding
+              // (pad column, zero row, past the end) is selected to zero: that zero IS the conv's padding.  A select, not
+              // a multiply: the zero row of sample n - 1 is computed from row 0 of sample n (every tap shift is
+              // forward), and NaN * 0 would carry a non-finite sample n into its neighbour's outputs
               const float4* tb4 = reinterpret_cast<const float4*>(tb + c0);
               float bsv[16];
   #pragma unroll
@@ -416,7 +440,6 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                   bsv[e] += f1 * tb[St.N + c0 + e] + f2 * tb[2 * St.N + c0 + e] + f3 * tb[3 * St.N + c0 + e] +
                             f4 * tb[4 * St.N + c0 + e];
               }
-              const float validf = si.valid ? 1.f : 0.f;
   #pragma unroll
               for (int e = 0; e < 16; ++e) {
                 const float a = __uint_as_float(r[e]) + bsv[e] + cx[e];
@@ -427,7 +450,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                 } else {
                   o = tc_apply_nl<NLT>(a, p.nl);
                 }
-                v[e] = o * validf;
+                v[e] = si.valid ? o : 0.f;
               }
             }
             if (St.hid_out && si.valid && sl < q.TO && u < p.NT) {  // training forward: keep the activations for iaf_step_bwd_saved
@@ -468,7 +491,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
               for (int e = 0; e < 8; ++e) zv[e] = __ldg(p.z + gi + (size_t)e * HW);
             }
             uint32_t r[16];
-            acc_ld16(c0, r, pitch);
+            acc_ld16(c0, r, pitch, St.wsinv);
             if (MODE == IAF_MODE_LAYER) {
   #pragma unroll
               for (int k_ = 0; k_ < NRED; ++k_) red[k_] = 0.f;

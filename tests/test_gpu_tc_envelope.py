@@ -45,6 +45,24 @@ def per_sample_fwd_err(a, ref):
     return float((d / r).max())
 
 
+def col_err(a, ref, abs_err=0.0):
+    """Worst channel of ``max_{n,y,x} |d| / max_{n,y,x} |ref|`` over axis 1: each channel judged at its own scale, so a
+    head or layer of small gain gets no absolute error floor.  ``abs_err``: an absolute error every element may carry on
+    top (subtracted from |d| first)."""
+    a, ref = _np(a), _np(ref)
+    assert np.isfinite(a).all()
+    r = np.abs(ref).max(axis=(0, 2, 3))
+    assert (r > 0).all()
+    return float((np.maximum(np.abs(a - ref) - abs_err, 0.0).max(axis=(0, 2, 3)) / r).max())
+
+
+def logdet_err(logdet, logdet_ref, logsd_ref):
+    """Worst sample of ``|d logdet_n| / sum |arw_logsd_ref[n]|``: the log-det against the size of what it sums."""
+    a, ref, ls = _np(logdet), _np(logdet_ref), _np(logsd_ref)
+    assert np.isfinite(a).all()
+    return float((np.abs(a - ref) / np.abs(ls).reshape(ls.shape[0], -1).sum(axis=1)).max())
+
+
 def bwd_err(a, ref):
     a, ref = _np(a), _np(ref)
     assert np.isfinite(a).all()
@@ -57,12 +75,13 @@ def _keys(variant):
     return ("V", "g", "b") if variant == "tf" else ("w", "s", "b")
 
 
-def make_params(variant, n_z, hidden, seed=1, spread=False, heads_gain=None):
+def make_params(variant, n_z, hidden, seed=1, spread=False, heads_gain=None, hidden0_gain=None, zero_bias=False):
     """Raw parameters (oracle.make_params).  ``spread``: gains spread like a trained model's: hidden layers tf
     g ~ U(-3, 3), theano s ~ U(-1, 1) (column gains between 0.05 and 20), heads over the lower half of that range (gains
     up to 1: with heads of gain 20 behind such hidden layers arw_logsd reaches ~90 and z' leaves the fp32 range even in
-    the fp64 reference).  ``heads_gain``: every head column's gain set to it (tf g = log(gain), theano
-    s = log(gain) / 3), the rest at the defaults."""
+    the fp64 reference).  ``heads_gain`` / ``hidden0_gain``: every column's gain of the heads / of the first hidden layer
+    set to it (tf g = log(gain), theano s = log(gain) / 3), the rest at the defaults.  ``zero_bias``: the layers whose
+    gain is set get zero biases too, so that a small output is not hidden behind its bias."""
     hid, hd = O.make_params(variant, n_z, hidden, [n_z, n_z], seed=seed)
     k = "g" if variant == "tf" else "s"
     if spread:
@@ -72,10 +91,14 @@ def make_params(variant, n_z, hidden, seed=1, spread=False, heads_gain=None):
             l[k] = rng.uniform(-lim, lim, size=l[k].shape).astype(np.float32)
         for l in hd:
             l[k] = rng.uniform(-lim, 0.0, size=l[k].shape).astype(np.float32)
-    if heads_gain is not None:
-        v = math.log(heads_gain) / (1.0 if variant == "tf" else 3.0)
-        for l in hd:
+    for gain, ls in ((heads_gain, hd), (hidden0_gain, hid[:1])):
+        if gain is None:
+            continue
+        v = math.log(gain) / (1.0 if variant == "tf" else 3.0)
+        for l in ls:
             l[k] = np.full_like(l[k], v)
+            if zero_bias:
+                l["b"] = np.zeros_like(l["b"])
     return hid, hd
 
 
@@ -444,6 +467,202 @@ def test_small_heads_gain_backward(shape, gain):
     for (name, got, ref), (_, got_s, _) in zip(pairs, pairs_s):
         assert bwd_err(got, ref) < TOL, name
         assert bwd_err(got, got_s) < TOL, name
+
+
+# Forward precision per output channel, and non-finite samples.  Shapes: the one-launch step, the per-stage step, C2b and
+# the streamed weight ring.  Every case also runs on the exact-fp32 SIMT kernel, which meets the same bounds: they ask for
+# fp32-level accuracy of each channel at its own scale.  Measured errors go to the JUnit report (record_property).
+GAIN_SHAPES = [
+    # variant, n_z, hidden, H, W, launches of one tensor-core step
+    ("tf", 32, [64], 16, 16, 1),
+    ("theano", 32, [64, 64], 8, 8, 3),
+    ("tf", 32, [160, 160], 16, 16, 3),
+    ("tf", 16, [176, 176], 16, 16, 3),
+]
+GAIN_IDS = ["one-launch", "per-stage", "c2b", "ring"]
+COL_TOL = 1e-5     # col_err
+LOGDET_TOL = 2e-6  # logdet_err
+# absolute error of the tensor-core epilogue's elu for a negative input: exp(v) - 1 with ex2.approx (2 ulp of a result
+# near 1).  It is most of an activation of ~1e-3 and is allowed on top of COL_TOL for hidden activations.
+ELU_ABS = 3e-7
+
+
+def checked_op(shape, path, hid, hd, checknan=None):
+    """Operator on ``path`` ("auto": the tensor cores, or "simt"), asserting where every entry and the backward run.
+    Returns (op, launches of one step)."""
+    from iaf_b200 import IAFOperator
+    variant, n_z, hidden, H, W, launches = shape
+    op = IAFOperator(variant, n_z, hidden, [n_z, n_z], nl="elu", path=path, checknan=checknan)
+    op.set_weights(dev_layers(variant, hid + hd))
+    want = "tc" if path == "auto" else "simt"
+    for entry in ("step", "multiconv", "layer"):
+        assert op.path_used(H, W, DEV, entry=entry) == want, entry
+    assert op.backward_path(H, W, DEV) == want
+    return op, (launches if path == "auto" else 1)
+
+
+def counted_step(op, launches, z, ctx, train=False):
+    """op.step (or the training forward, which also returns the hidden activations) through the expected kernels."""
+    l0 = op.launch_count()
+    out = op._step_train_raw(z, ctx) if train else op.step(z, ctx)
+    assert op.launch_count() - l0 == launches
+    return out
+
+
+def within(record_property, name, err, tol):
+    record_property(name, err)
+    assert err <= tol, (name, err)
+
+
+@pytest.mark.parametrize("path", ["auto", "simt"])
+@pytest.mark.parametrize("gain", [1e-2, 1e-3, 1e-4])
+@pytest.mark.parametrize("shape", GAIN_SHAPES, ids=GAIN_IDS)
+def test_small_heads_gain_forward_per_channel(shape, gain, path, record_property):
+    """Heads of gain 1e-2 .. 1e-4 with zero biases: weights of O(gain / sqrt(K)), far below the range where the fp16 lo
+    half of a weight is a normal number.  m, s and arw_logsd per channel, the log-det against sum |arw_logsd|, z' and the
+    layer entry at the usual tolerance."""
+    variant, n_z, hidden, H, W, _ = shape
+    B = 2
+    hid, hd = make_params(variant, n_z, hidden, seed=81, heads_gain=gain, zero_bias=True)
+    op, launches = checked_op(shape, path, hid, hd)
+    z, ctx = O.make_inputs(B, n_z, hidden[0], H, W, seed=82)
+    zc, cc = torch.from_numpy(z).to(DEV), torch.from_numpy(ctx).to(DEV)
+    th, thh = f64_layers(hid), f64_layers(hd)
+    zt, ct = torch.from_numpy(z).double(), torch.from_numpy(ctx).double()
+
+    z1, logsd, logdet = counted_step(op, launches, zc, cc)
+    z_ref, logsd_ref, logdet_ref = OT.iaf_step(variant, zt, ct, th, thh)
+    within(record_property, "arw_logsd", col_err(logsd, logsd_ref), COL_TOL)
+    within(record_property, "logdet", logdet_err(logdet, logdet_ref, logsd_ref), LOGDET_TOL)
+    assert fwd_err(z1, z_ref) < TOL
+    m, s = op.multiconv(zc, cc)
+    m_ref, s_ref = OT.multiconv(variant, zt, ct, th, thh)
+    within(record_property, "m", col_err(m, m_ref), COL_TOL)
+    within(record_property, "s", col_err(s, s_ref), COL_TOL)
+
+    eps, pm, pls, prm, prl, lctx = layer_inputs(B, n_z, hidden, H, W, seed=83)
+    t = lambda a: torch.from_numpy(a).to(DEV)
+    zo, kl, kl_bc, kl_cost = op.layer(t(eps), t(pm), t(pls), t(prm), t(prl), t(lctx))
+    d = lambda a: torch.from_numpy(a).double()
+    zr, klr, bcr, costr = layer_ref(variant, "elu", th, thh, d(eps), d(pm), d(pls), d(prm), d(prl), d(lctx))
+    assert fwd_err(zo, zr) < TOL and fwd_err(kl, klr) < TOL
+    assert per_sample_fwd_err(kl_bc, bcr) < TOL
+    assert per_sample_fwd_err(kl_cost[:, None], costr[:, None]) < TOL
+
+
+@pytest.mark.parametrize("path", ["auto", "simt"])
+@pytest.mark.parametrize("gain", [1e-2, 1e-3])
+@pytest.mark.parametrize("shape", GAIN_SHAPES, ids=GAIN_IDS)
+def test_small_first_hidden_gain_forward_per_channel(shape, gain, path, record_property):
+    """First hidden layer of gain 1e-2 / 1e-3 with zero bias and zero context: its activations (kept by the training
+    forward) per channel, beyond the elu's absolute error ELU_ABS, and the step's outputs at the usual tolerance.  The
+    heads see activations of ~gain here, whose own fp16 split has an absolute floor (activations are not scaled), so they
+    get no per-channel bound."""
+    variant, n_z, hidden, H, W, _ = shape
+    B = 2
+    hid, hd = make_params(variant, n_z, hidden, seed=91, hidden0_gain=gain, zero_bias=True)
+    op, launches = checked_op(shape, path, hid, hd)
+    z, _ = O.make_inputs(B, n_z, hidden[0], H, W, seed=92)
+    ctx = np.zeros((B, hidden[0], H, W), dtype=np.float32)
+    th, thh = f64_layers(hid), f64_layers(hd)
+    zt, ct = torch.from_numpy(z).double(), torch.from_numpy(ctx).double()
+
+    z1, logsd, logdet, hs = counted_step(op, launches, torch.from_numpy(z).to(DEV), torch.from_numpy(ctx).to(DEV),
+                                         train=True)
+    conv = OT.tf_ar_conv2d if variant == "tf" else OT.theano_ar_conv2d
+    h_ref = torch.nn.functional.elu(conv(zt, th[0], False) + ct)
+    record_property("hidden0_raw", col_err(hs[0], h_ref))
+    within(record_property, "hidden0", col_err(hs[0], h_ref, ELU_ABS), COL_TOL)
+    z_ref, logsd_ref, logdet_ref = OT.iaf_step(variant, zt, ct, th, thh)
+    assert fwd_err(z1, z_ref) < TOL and fwd_err(logsd, logsd_ref) < TOL
+    assert per_sample_fwd_err(logdet[:, None], logdet_ref[:, None]) < TOL
+
+
+@pytest.mark.parametrize("path", ["auto", "simt"])
+@pytest.mark.parametrize("shape", GAIN_SHAPES, ids=GAIN_IDS)
+def test_heads_column_beyond_fp16_range(shape, path, record_property):
+    """One column of the m head with gain e^15 (tf g = 15, theano s = 5): most of its weights are larger than the
+    largest fp16 number and must still come out exact."""
+    variant, n_z, hidden, H, W, _ = shape
+    B = 2
+    hid, hd = make_params(variant, n_z, hidden, seed=101)
+    c = n_z // 2 + 3
+    hd[0]["g" if variant == "tf" else "s"][c] = 15.0 if variant == "tf" else 5.0
+    op, launches = checked_op(shape, path, hid, hd)
+    z, ctx = O.make_inputs(B, n_z, hidden[0], H, W, seed=102)
+    zc, cc = torch.from_numpy(z).to(DEV), torch.from_numpy(ctx).to(DEV)
+    th, thh = f64_layers(hid), f64_layers(hd)
+    zt, ct = torch.from_numpy(z).double(), torch.from_numpy(ctx).double()
+
+    m, _ = op.multiconv(zc, cc)
+    m_ref, _ = OT.multiconv(variant, zt, ct, th, thh)
+    assert float(m_ref[:, c].abs().max()) > 65504.0  # the column really is beyond the fp16 range
+    within(record_property, "m_column", col_err(m[:, c:c + 1], m_ref[:, c:c + 1]), COL_TOL)
+    z1, _, _ = counted_step(op, launches, zc, cc)
+    z_ref, _, _ = OT.iaf_step(variant, zt, ct, th, thh)
+    within(record_property, "z", fwd_err(z1, z_ref), TOL)
+
+
+ISO_SHAPES = GAIN_SHAPES + [("tf", 16, [16], 2, 2, 1)]
+ISO_IDS = GAIN_IDS + ["2x2-b50"]
+
+
+@pytest.mark.parametrize("path", ["auto", "simt"])
+@pytest.mark.parametrize("poison", ["1e5", "nan"])
+@pytest.mark.parametrize("shape", ISO_SHAPES, ids=ISO_IDS)
+def test_non_finite_sample_stays_in_its_sample(shape, poison, path):
+    """One channel plane of one middle sample set to 1e5 (inf in the fp16 operand split of the tensor cores) or NaN:
+    every other sample's outputs of step, multiconv, layer (eps poisoned) and the step's autograd node (g_z, g_context)
+    are bit-identical to a clean run at the same batch positions.  On the tensor cores the poisoned sample's log-det is
+    non-finite (loud), and checknan="raise" raises on the poisoned batch only."""
+    variant, n_z, hidden, H, W, _ = shape
+    B = 50 if H == 2 else 3      # 2x2: 15 samples per tile
+    pn, pc = B // 2, 3
+    val = 1e5 if poison == "1e5" else float("nan")
+    hid, hd = make_params(variant, n_z, hidden, seed=111)
+    op, launches = checked_op(shape, path, hid, hd)
+    z, ctx = O.make_inputs(B, n_z, hidden[0], H, W, seed=112)
+    zp = z.copy()
+    zp[pn, pc] = val
+    t = lambda a: torch.from_numpy(a).to(DEV)
+    keep = torch.tensor([n for n in range(B) if n != pn], device=DEV)
+
+    def same(clean, bad):
+        for i, (a, b) in enumerate(zip(clean, bad)):
+            assert torch.equal(a[keep], b[keep]), i
+            assert torch.isfinite(a).all(), i
+
+    clean = counted_step(op, launches, t(z), t(ctx))
+    bad = op.step(t(zp), t(ctx))
+    same(clean, bad)
+    if path == "auto":
+        assert not bool(torch.isfinite(bad[2][pn]))
+    same(op.multiconv(t(z), t(ctx)), op.multiconv(t(zp), t(ctx)))
+
+    ins = layer_inputs(B, n_z, hidden, H, W, seed=113)
+    eps_p = ins[0].copy()
+    eps_p[pn, pc] = val
+    same(op.layer(*map(t, ins)), op.layer(t(eps_p), *map(t, ins[1:])))
+
+    r = np.random.RandomState(114)
+    gzo, gls = t(r.randn(*z.shape).astype(np.float32)), t(r.randn(*z.shape).astype(np.float32))
+    gld = t(r.randn(B).astype(np.float32))
+
+    def grads(zz):
+        zg, cg = t(zz).requires_grad_(True), t(ctx).requires_grad_(True)
+        zo, ls, ld = op.step(zg, cg)
+        ((zo * gzo).sum() + (ls * gls).sum() + (ld * gld).sum()).backward()
+        return zg.grad, cg.grad
+
+    same(grads(z), grads(zp))
+
+    opn, _ = checked_op(shape, path, hid, hd, checknan="raise")
+    opn.step(t(z), t(ctx))
+    if path == "auto" or bool(torch.isnan(bad[2].sum())):
+        with pytest.raises(FloatingPointError):
+            opn.step(t(zp), t(ctx))
+    else:
+        opn.step(t(zp), t(ctx))  # the exact-fp32 kernel may carry 1e5 through to a finite log-det
 
 
 @pytest.mark.parametrize("shape", REGIME_SHAPES, ids=["one-launch", "per-stage"])
