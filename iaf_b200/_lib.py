@@ -8,7 +8,7 @@ from .build import LIB
 IAF_MAX_HIDDEN = 4
 IAF_MAX_HEADS = 2
 
-VARIANTS = {"tf": 0, "theano": 1}
+VARIANTS = {"tf": 0, "theano": 1, "theano_flipmask": 2}  # theano_flipmask: multiconv2d(..., flipmask=True)
 NLS = {None: 0, "None": 0, "none": 0, "elu": 1, "softplus": 2, "relu": 3, "tanh": 4, "leakyrelu": 5}
 PATHS = {"auto": 0, "simt": 1, "tc": 2}
 PATH_NAMES = {1: "simt", 2: "tc"}

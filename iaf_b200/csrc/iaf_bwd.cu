@@ -675,26 +675,15 @@ struct IafWnormLayer {
 };
 struct IafWnormParams {
   IafWnormLayer layer[IAF_MAX_HIDDEN + IAF_MAX_HEADS];
-  int n_layers, variant;
+  int n_layers;
+  IafVariantFlags vf;
 };
 
-__device__ __forceinline__ bool bw_centre_visible(int ci, int co, int cin, int cout, int zd) {
-  if (cout >= cin) {
-    const int k = cout / cin, i = co / k;
-    return zd ? (ci < i) : (ci <= i);
-  }
-  const int k = cin / cout;
-  return zd ? (ci < co * k) : (ci < (co + 1) * k);
-}
-__device__ __forceinline__ size_t bw_raw_index(const IafWnormLayer& L, int variant, int ky, int kx, int ci, int co) {
-  if (variant == IAF_VARIANT_TF) return ((size_t)(ky * 3 + kx) * L.cin + ci) * L.cout + co;
-  return (((size_t)co * (L.cin + 1) + ci) * 3 + ky) * 3 + kx;
-}
-// live tap index of kernel position (ky,kx), or -1 (layers.py:134-141)
-__device__ __forceinline__ int bw_tap_of(int ky, int kx) {
-  if (ky == 1) return kx == 1 ? 0 : (kx == 2 ? 1 : -1);
-  if (ky == 2) return 2 + kx;
-  return -1;
+// gradient of the packed weight of canonical tap t, input channel ci (ci == cin: pad channel).  The flipped pad channel's
+// centre is live but never reaches an output (iaf_tap_rule): its packed gradient is 0, and it still gets -k * v below
+__device__ __forceinline__ float bw_packed_grad(const IafWnormLayer& L, size_t nw, int t, int ci, int col) {
+  if (ci < L.cin) return L.dwp[((size_t)t * L.cin + ci) * L.ncol + col];
+  return t == 0 ? 0.f : L.dwp[nw + (size_t)t * L.ncol + col];
 }
 
 __global__ void __launch_bounds__(128) iaf_bwd_wnorm_kernel(const __grid_constant__ IafWnormParams p) {
@@ -703,25 +692,18 @@ __global__ void __launch_bounds__(128) iaf_bwd_wnorm_kernel(const __grid_constan
   if (co >= L.cout) return;
   const int tid = threadIdx.x;
   const int col = L.n_heads ? bw_head_col(L.n_heads, L.head, co) : co;
-  const int cin_all = L.cin + (p.variant == IAF_VARIANT_THEANO ? 1 : 0);
+  const int cin_all = L.cin + (p.vf.pad_channel ? 1 : 0);
   const int n_ent = 9 * cin_all;
   const size_t nw = (size_t)IAF_NTAPS * L.cin * L.ncol;
 
   // pass 1: ss = sum v^2, dot = sum dW * v over the live entries of this output channel
   float ss = 0.f, dot = 0.f;
   for (int e = tid; e < n_ent; e += 128) {
-    const int ci = e / 9, ky = (e % 9) / 3, kx = e % 3;
-    const int t = bw_tap_of(ky, kx);
-    if (t < 0) continue;
-    float dv;
-    if (ci < L.cin) {
-      if (t == 0 && !bw_centre_visible(ci, co, L.cin, L.cout, L.zerodiag)) continue;
-      dv = L.dwp[((size_t)t * L.cin + ci) * L.ncol + col];
-    } else {
-      if (t == 0) continue;  // pad channel: centre tap masked (ar.py:249-262)
-      dv = L.dwp[nw + (size_t)t * L.ncol + col];
-    }
-    const float v = L.w[bw_raw_index(L, p.variant, ky, kx, ci, co)];
+    const int ci = e / 9, k = e % 9;
+    const int t = iaf_canonical_tap(k, p.vf.flipmask);
+    if (t < 0 || !iaf_tap_rule(t, ci, co, L.cin, L.cout, L.zerodiag, p.vf.flipmask).live) continue;
+    const float dv = bw_packed_grad(L, nw, t, ci, col);
+    const float v = L.w[iaf_raw_index(p.vf.theano, k, ci, co, L.cin, L.cout)];
     ss = fmaf(v, v, ss);
     dot = fmaf(dv, v, dot);
   }
@@ -738,7 +720,7 @@ __global__ void __launch_bounds__(128) iaf_bwd_wnorm_kernel(const __grid_constan
   dot = r2[0];
 
   float f, k;  // dV = f * dW - k * v
-  if (p.variant == IAF_VARIANT_TF) {
+  if (!p.vf.theano) {
     const float n2 = fmaxf(ss, 1e-12f);
     f = expf(L.scale[co]) / sqrtf(n2);
     k = ss > 1e-12f ? f * dot / n2 : 0.f;
@@ -751,19 +733,14 @@ __global__ void __launch_bounds__(128) iaf_bwd_wnorm_kernel(const __grid_constan
   }
   if (tid == 0 && L.g_bias) L.g_bias[co] = L.dwp[nw + col];
   if (!L.g_w) return;
-  // pass 2: every raw entry of this output channel; masked entries get exactly zero
+  // pass 2: every raw entry of this output channel; masked entries and the zero-diagonal rows get exactly zero
   for (int e = tid; e < n_ent; e += 128) {
-    const int ci = e / 9, ky = (e % 9) / 3, kx = e % 3;
-    const int t = bw_tap_of(ky, kx);
-    const size_t ri = bw_raw_index(L, p.variant, ky, kx, ci, co);
+    const int ci = e / 9, kk = e % 9;
+    const int t = iaf_canonical_tap(kk, p.vf.flipmask);
+    const size_t ri = iaf_raw_index(p.vf.theano, kk, ci, co, L.cin, L.cout);
     float out = 0.f;
-    bool live = t >= 0;
-    if (live && ci < L.cin && t == 0 && !bw_centre_visible(ci, co, L.cin, L.cout, L.zerodiag)) live = false;
-    if (live && ci >= L.cin && t == 0) live = false;
-    if (live) {
-      const float dv = ci < L.cin ? L.dwp[((size_t)t * L.cin + ci) * L.ncol + col] : L.dwp[nw + (size_t)t * L.ncol + col];
-      out = f * dv - k * L.w[ri];
-    }
+    if (t >= 0 && iaf_tap_rule(t, ci, co, L.cin, L.cout, L.zerodiag, p.vf.flipmask).live)
+      out = f * bw_packed_grad(L, nw, t, ci, col) - k * L.w[ri];
     L.g_w[ri] = out;
   }
 }
@@ -775,6 +752,7 @@ static int bw_round_up(int a, int b) { return (a + b - 1) / b * b; }
 
 struct IafBwdPlan {
   iaf_desc_t d;
+  IafVariantFlags vf;
   int n_stages;
   int cin[IAF_MAX_STAGES], cout[IAF_MAX_STAGES], ncol[IAF_MAX_STAGES];
   int head_pad;
@@ -823,6 +801,7 @@ int iaf_bwd_plan_create(IafBwdPlan** out, const iaf_desc_t* d, const int* cin, c
   if (!pl) return IAF_ERR_BAD_ARG;
   memset(pl, 0, sizeof(*pl));
   pl->d = *d;
+  pl->vf = iaf_variant_flags(d->variant);
   pl->n_stages = d->n_hidden + 1;
   pl->head_pad = head_pad;
   size_t wt_max = 0;
@@ -961,7 +940,7 @@ int iaf_bwd_run(IafBwdPlan* pl, const IafBwdArgs* a, cudaStream_t stream, int* n
   const iaf_desc_t& d = pl->d;
   const int B = a->B, H = d.H, W = d.W, HW = H * W;
   const int nst = pl->n_stages, last = nst - 1;
-  const int flip = d.variant == IAF_VARIANT_THEANO ? 1 : 0;
+  const int flip = pl->vf.reflect;
   int st = bw_ensure_scratch(pl, B);
   if (st != IAF_OK) return st;
   int nl_ = 0;
@@ -1009,7 +988,7 @@ int iaf_bwd_run(IafBwdPlan* pl, const IafBwdArgs* a, cudaStream_t stream, int* n
     memset(&q, 0, sizeof(q));
     q.in = hcur[j];
     q.w = a->w_packed[j]; q.bias = a->bias_packed[j];
-    q.padw = flip ? a->padw_packed[j] : nullptr;
+    q.padw = pl->vf.pad_channel ? a->padw_packed[j] : nullptr;
     q.ctx = (j == 0 && j != last) ? a->ctx : nullptr;
     q.out = j == last ? pl->hb : pl->h[j + 1];
     q.B = B; q.H = H; q.W = W; q.cin = pl->cin[j]; q.in_planes = pl->cin[j];
@@ -1077,7 +1056,7 @@ int iaf_bwd_run(IafBwdPlan* pl, const IafBwdArgs* a, cudaStream_t stream, int* n
         nl_ += 4;
       } else {
 #ifndef IAF_EMU
-        if (flip) iaf_bwd_bias_kernel<true><<<pl->ncol[j] * BW_BIAS_SEG, BW_THREADS, 0, stream>>>(Gcur, pl->bpart, B, g_planes, pl->ncol[j], H, W, flip);
+        if (pl->vf.pad_channel) iaf_bwd_bias_kernel<true><<<pl->ncol[j] * BW_BIAS_SEG, BW_THREADS, 0, stream>>>(Gcur, pl->bpart, B, g_planes, pl->ncol[j], H, W, flip);
         else iaf_bwd_bias_kernel<false><<<pl->ncol[j] * BW_BIAS_SEG, BW_THREADS, 0, stream>>>(Gcur, pl->bpart, B, g_planes, pl->ncol[j], H, W, flip);
 #endif
         if (cudaGetLastError() != cudaSuccess) return IAF_ERR_CUDA;
@@ -1157,7 +1136,7 @@ int iaf_bwd_run(IafBwdPlan* pl, const IafBwdArgs* a, cudaStream_t stream, int* n
     IafWnormParams q;
     memset(&q, 0, sizeof(q));
     q.n_layers = d.n_hidden + d.n_heads;
-    q.variant = d.variant;
+    q.vf = pl->vf;
     int max_cout = 0;
     for (int i = 0; i < q.n_layers; ++i) {
       IafWnormLayer& L = q.layer[i];

@@ -26,20 +26,11 @@ int cuda_fail(cudaError_t e, const char* what) {
 
 int round_up(int a, int b) { return (a + b - 1) / b * b; }
 
-long long centre_nnz(int cin, int cout, int zd) {
+// live centre weights of the real input channels (the pad channel never multiplies anything but the border)
+long long centre_nnz(int cin, int cout, int zd, int flipmask) {
   long long n = 0;
   for (int co = 0; co < cout; ++co)
-    for (int ci = 0; ci < cin; ++ci) {
-      bool vis;
-      if (cout >= cin) {
-        int k = cout / cin, i = co / k;
-        vis = zd ? ci < i : ci <= i;
-      } else {
-        int k = cin / cout;
-        vis = zd ? ci < co * k : ci < (co + 1) * k;
-      }
-      n += vis;
-    }
+    for (int ci = 0; ci < cin; ++ci) n += iaf_tap_rule(0, ci, co, cin, cout, zd, flipmask).live;
   return n;
 }
 
@@ -47,6 +38,7 @@ long long centre_nnz(int cin, int cout, int zd) {
 
 struct iaf_plan {
   iaf_desc_t d;
+  IafVariantFlags vf;
   int path;
   int device;
   int n_stages;                       // n_hidden + 1
@@ -185,7 +177,7 @@ static int ensure_scratch(iaf_plan* pl, int B, cudaStream_t stream) {
 
 extern "C" {
 
-int iaf_version(void) { return 100; }  // 0.1.0
+int iaf_version(void) { return 200; }  // 0.2.0
 
 const char* iaf_strerror(int status) {
   switch (status) {
@@ -210,7 +202,7 @@ int iaf_plan_create(iaf_plan_t** out, const iaf_desc_t* desc) {
   *out = nullptr;
   const iaf_desc_t& d = *desc;
   if (d.n_z <= 0 || d.H <= 0 || d.W <= 0) return IAF_ERR_BAD_ARG;
-  if (d.variant != IAF_VARIANT_TF && d.variant != IAF_VARIANT_THEANO) return IAF_ERR_BAD_ARG;
+  if (d.variant < IAF_VARIANT_TF || d.variant > IAF_VARIANT_THEANO_FLIPMASK) return IAF_ERR_BAD_ARG;
   if (d.n_hidden < 0 || d.n_hidden > IAF_MAX_HIDDEN) return IAF_ERR_UNSUPPORTED;
   if (d.n_heads < 1 || d.n_heads > IAF_MAX_HEADS) return IAF_ERR_UNSUPPORTED;
   if (d.nl < IAF_NL_NONE || d.nl > IAF_NL_LEAKYRELU) return IAF_ERR_UNSUPPORTED;
@@ -238,6 +230,7 @@ int iaf_plan_create(iaf_plan_t** out, const iaf_desc_t* desc) {
   if (!pl) return IAF_ERR_BAD_ARG;
   memset(pl, 0, sizeof(*pl));
   pl->d = d;
+  pl->vf = iaf_variant_flags(d.variant);
   // a CUDA failure from here on releases the half-built plan (struct and device buffers) before returning
 #define CKP(call)                                                    \
   do {                                                              \
@@ -353,7 +346,7 @@ int iaf_pack_weights(iaf_plan_t* pl, const float* const* w, const float* const* 
   IafPackParams pp;
   memset(&pp, 0, sizeof(pp));
   pp.n_layers = n_layers;
-  pp.variant = d.variant;
+  pp.vf = pl->vf;
   int max_cout = 0;
   for (int j = 0; j < pl->n_stages; ++j) {
     CK(cudaMemsetAsync(pl->w[j], 0, sizeof(float) * pl->w_elems[j], stream));
@@ -426,7 +419,7 @@ static int run(iaf_plan* pl, int mode, const float* z, const float* ctx, const f
   for (int j = 0; j < pl->n_stages; ++j) {
     p.stage[j].w = pl->w[j];
     p.stage[j].bias = pl->bias[j];
-    p.stage[j].padw = d.variant == IAF_VARIANT_THEANO ? pl->padw[j] : nullptr;
+    p.stage[j].padw = pl->vf.pad_channel ? pl->padw[j] : nullptr;
     p.stage[j].cin = pl->cin[j];
     p.stage[j].cout = pl->cout[j];
     p.stage[j].cout_pad = pl->cout_pad[j];
@@ -435,7 +428,7 @@ static int run(iaf_plan* pl, int mode, const float* z, const float* ctx, const f
   p.n_heads = d.n_heads; p.head_c = d.head[0]; p.head_pad = pl->head_pad;
   p.B = B; p.C = d.n_z; p.H = d.H; p.W = d.W; p.P = pl->P;
   p.band_rows = pl->band_rows; p.n_bands = pl->n_bands;
-  p.flip = d.variant == IAF_VARIANT_THEANO ? 1 : 0;
+  p.flip = pl->vf.reflect;
   p.nl = d.nl; p.mode = mode; p.scale = 0.1f;
   p.bufz_elems = pl->bufz; p.bufa_elems = pl->bufa; p.bufb_elems = pl->bufb;
   CK(iaf_launch_simt(p, pl->smem, stream));
@@ -801,10 +794,10 @@ double iaf_plan_algorithmic_flops(const iaf_plan_t* pl, int B) {
   long long nnz = 0;
   int prev = d.n_z;
   for (int i = 0; i < d.n_hidden; ++i) {
-    nnz += 4LL * prev * d.hidden[i] + centre_nnz(prev, d.hidden[i], 0);
+    nnz += 4LL * prev * d.hidden[i] + centre_nnz(prev, d.hidden[i], 0, pl->vf.flipmask);
     prev = d.hidden[i];
   }
-  for (int k = 0; k < d.n_heads; ++k) nnz += 4LL * prev * d.head[k] + centre_nnz(prev, d.head[k], 1);
+  for (int k = 0; k < d.n_heads; ++k) nnz += 4LL * prev * d.head[k] + centre_nnz(prev, d.head[k], 1, pl->vf.flipmask);
   return 2.0 * B * d.H * d.W * (double)nnz;
 }
 

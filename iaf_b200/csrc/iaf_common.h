@@ -45,6 +45,71 @@ static inline cudaError_t iaf_smem_optin(K kernel) {
 #define IAF_NTAPS 5          // live taps of the 3x3 AR mask: (ky,kx) = (1,1)c (1,2) (2,0) (2,1) (2,2)
 #define IAF_MAX_STAGES (IAF_MAX_HIDDEN + 1)
 
+// What a variant means to the kernels; every plan derives it once from its desc.  The kernels always apply the TF offsets
+// above (the "canonical frame"), the pad-channel table at the bottom / right borders of that frame.
+//   TF:               no reflection, no pad channel, TF layout and norm.
+//   THEANO:           true convolution with the mask reads the point reflection of the TF offsets: the data is reflected
+//                     on load / store (pixel p <-> HW-1-p), which also puts the pad channel's top / left border at the
+//                     canonical bottom / right.
+//   THEANO_FLIPMASK:  the mask reversed on all four axes (ar.py:263-264) reflects the taps back: true convolution with it
+//                     reads the TF offsets themselves, so there is no reflection, and the pad channel sits at the bottom
+//                     / right borders of the image.  Theano layout, norm and pad channel; the channel rule: iaf_tap_rule.
+struct IafVariantFlags {
+  int reflect;      // data point-reflected on load / store
+  int pad_channel;  // the Theano pad channel (conv.py:71-83): a [4][N] table of its taps 1..4
+  int theano;       // Theano raw layout [Cout][Cin+1][3][3] and norm exp(3s) / (sqrt(ss) + 1e-8) (ar.py:267-281,316)
+  int flipmask;     // the reversed mask (iaf_tap_rule)
+};
+static inline IafVariantFlags iaf_variant_flags(int variant) {
+  IafVariantFlags f;
+  f.reflect = variant == IAF_VARIANT_THEANO;
+  f.pad_channel = variant != IAF_VARIANT_TF;
+  f.theano = variant != IAF_VARIANT_TF;
+  f.flipmask = variant == IAF_VARIANT_THEANO_FLIPMASK;
+  return f;
+}
+
+// The AR mask, for every layout and both mask orders: the one copy of the rule of tf_utils/layers.py:115-141 and
+// graphy/nodes/ar.py:241-276.  t: canonical tap (0 = centre); ci: input channel, ci == cin the Theano pad channel; co: output
+// channel; zd: zerodiagonal (heads).  Returns k = ky*3+kx of the raw parameter entry tap t multiplies, and live: the entry
+// enters the normalised kernel -- the mask keeps it and, for heads, l2normalize's zero-diagonal rows (ar.py:273-276: the
+// centre of rows [0, cout/cin), or row 0 when cout < cin) do not clear it.
+// flipmask: the raw tap is the point reflection (2-ky, 2-kx), and the centre follows the unflipped rule of output channel
+// cout-1-co and input channel cin-ci.  So channel 0 never sees the centre, and the pad channel's centre inherits channel
+// 0's column: live, although it never reaches an output (the centre of the padded input is interior, i.e. 0) -- it only
+// enters the norm.  Unflipped, the pad centre is masked and the zero-diagonal rows are already masked.
+struct IafTap {
+  int k;
+  bool live;
+};
+__host__ __device__ __forceinline__ IafTap iaf_tap_rule(int t, int ci, int co, int cin, int cout, int zd, int flipmask) {
+  const int ky = t < 2 ? 1 : 2, kx = t == 0 ? 1 : (t == 1 ? 2 : t - 2);
+  IafTap r;
+  r.k = flipmask ? (2 - ky) * 3 + (2 - kx) : ky * 3 + kx;
+  r.live = true;
+  if (t != 0) return r;
+  const int c = flipmask ? cin - ci : ci, o = flipmask ? cout - 1 - co : co;
+  if (cout >= cin) {
+    const int k = cout / cin, i = o / k;
+    r.live = (zd ? (c < i) : (c <= i)) && !(zd && co < k);
+  } else {
+    const int k = cin / cout;
+    r.live = (zd ? (c < o * k) : (c < (o + 1) * k)) && !(zd && co == 0);
+  }
+  return r;
+}
+// canonical tap of raw kernel position k = ky*3+kx, or -1 where the mask is zero for every channel
+__host__ __device__ __forceinline__ int iaf_canonical_tap(int k, int flipmask) {
+  if (flipmask) k = 8 - k;
+  const int ky = k / 3, kx = k % 3;
+  if (ky == 1) return kx == 1 ? 0 : (kx == 2 ? 1 : -1);
+  return ky == 2 ? 2 + kx : -1;
+}
+// index of raw entry (k, ci, co) in the reference layout: TF [3,3,cin,cout] | Theano [cout,cin+1,3,3]
+__host__ __device__ __forceinline__ size_t iaf_raw_index(int theano, int k, int ci, int co, int cin, int cout) {
+  return theano ? ((size_t)co * (cin + 1) + ci) * 9 + k : ((size_t)k * cin + ci) * cout + co;
+}
+
 // One conv stage as the SIMT kernel sees it (weights already masked, normalised, scaled).
 struct IafStageDev {
   const float* w;     // [5][cin][cout_pad], cout contiguous (heads: see iaf_pack.cu for the column order)
@@ -76,7 +141,7 @@ struct IafSimtParams {
   int n_heads, head_c, head_pad;
   int B, C, H, W, P;       // P = smem row pitch = 8*ceil(W/8) + 2
   int band_rows, n_bands;
-  int flip;                // 1: Theano orientation (data point-reflected on load/store)
+  int flip;                // 1: data point-reflected on load/store (IafVariantFlags::reflect)
   int nl;
   int mode;                // 0 multiconv, 1 step, 2 layer
   float scale;             // 0.1
@@ -110,7 +175,7 @@ struct IafPackLayer {
 struct IafPackParams {
   IafPackLayer layer[IAF_MAX_HIDDEN + IAF_MAX_HEADS];
   int n_layers;
-  int variant;
+  IafVariantFlags vf;
 };
 
 cudaError_t iaf_launch_pack(const IafPackParams& p, int max_cout, cudaStream_t stream);

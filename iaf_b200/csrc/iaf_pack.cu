@@ -5,26 +5,13 @@
 //
 // Only the 5 live taps of the 3x3 AR mask are kept (tf_utils/layers.py:134-141 ==
 // graphy/nodes/ar.py:241-264): t -> (ky,kx) = (1,1) (1,2) (2,0) (2,1) (2,2); the centre tap
-// carries the MADE channel mask (layers.py:115-131).
+// carries the MADE channel mask (layers.py:115-131).  The rule itself: iaf_tap_rule (iaf_common.h).
 #include "iaf_common.h"
 
-__device__ __forceinline__ bool iaf_centre_visible(int ci, int co, int cin, int cout, int zd) {
-  if (cout >= cin) {
-    const int k = cout / cin;
-    const int i = co / k;
-    return zd ? (ci < i) : (ci <= i);
-  }
-  const int k = cin / cout;
-  return zd ? (ci < co * k) : (ci < (co + 1) * k);
-}
-
-__device__ __forceinline__ int iaf_tap_ky(int t) { return t < 2 ? 1 : 2; }
-__device__ __forceinline__ int iaf_tap_kx(int t) { return t == 0 ? 1 : (t == 1 ? 2 : t - 2); }
-
-__device__ __forceinline__ float iaf_raw_weight(const IafPackLayer& L, int variant, int t, int ci, int co) {
-  const int ky = iaf_tap_ky(t), kx = iaf_tap_kx(t);
-  if (variant == IAF_VARIANT_TF) return L.w[((size_t)(ky * 3 + kx) * L.cin + ci) * L.cout + co];
-  return L.w[(((size_t)co * (L.cin + 1) + ci) * 3 + ky) * 3 + kx];
+// raw weight of canonical tap t, input channel ci (ci == cin: pad channel), output channel co; 0 where not live
+__device__ __forceinline__ float iaf_masked_weight(const IafPackLayer& L, const IafVariantFlags& vf, int t, int ci, int co) {
+  const IafTap tp = iaf_tap_rule(t, ci, co, L.cin, L.cout, L.zerodiag, vf.flipmask);
+  return tp.live ? L.w[iaf_raw_index(vf.theano, tp.k, ci, co, L.cin, L.cout)] : 0.f;
 }
 
 __global__ void __launch_bounds__(128) iaf_pack_kernel(const __grid_constant__ IafPackParams p) {
@@ -33,7 +20,9 @@ __global__ void __launch_bounds__(128) iaf_pack_kernel(const __grid_constant__ I
   if (co >= L.cout) return;
   const int tid = threadIdx.x;
   const int n_real = L.cin * IAF_NTAPS;
-  const int n_pad = (p.variant == IAF_VARIANT_THEANO) ? 4 : 0;  // pad channel: taps 1..4 (centre masked, ar.py:249-262)
+  // pad channel: taps 1..4; flipped, also its centre, which only enters the norm (see iaf_tap_rule)
+  const int n_pad = p.vf.pad_channel ? (p.vf.flipmask ? 5 : 4) : 0;
+  const int t_pad0 = IAF_NTAPS - n_pad;
 
   // pass 1: sum of squares of the masked row
   float ss = 0.f;
@@ -41,10 +30,9 @@ __global__ void __launch_bounds__(128) iaf_pack_kernel(const __grid_constant__ I
     float v;
     if (e < n_real) {
       const int t = e / L.cin, ci = e % L.cin;
-      v = iaf_raw_weight(L, p.variant, t, ci, co);
-      if (t == 0 && !iaf_centre_visible(ci, co, L.cin, L.cout, L.zerodiag)) v = 0.f;
+      v = iaf_masked_weight(L, p.vf, t, ci, co);
     } else {
-      v = iaf_raw_weight(L, p.variant, e - n_real + 1, L.cin, co);
+      v = iaf_masked_weight(L, p.vf, t_pad0 + e - n_real, L.cin, co);
     }
     ss = fmaf(v, v, ss);
   }
@@ -57,7 +45,7 @@ __global__ void __launch_bounds__(128) iaf_pack_kernel(const __grid_constant__ I
   }
   ss = red[0];
   float factor;
-  if (p.variant == IAF_VARIANT_TF)
+  if (!p.vf.theano)
     factor = expf(L.scale[co]) / sqrtf(fmaxf(ss, 1e-12f));        // layers.py:60, l2_normalize eps
   else
     factor = expf(3.0f * L.scale[co]) / (sqrtf(ss) + 1e-8f);      // ar.py:277-281,316 (logscale_scale = 3)
@@ -66,12 +54,10 @@ __global__ void __launch_bounds__(128) iaf_pack_kernel(const __grid_constant__ I
   for (int e = tid; e < n_real + n_pad; e += blockDim.x) {
     if (e < n_real) {
       const int t = e / L.cin, ci = e % L.cin;
-      float v = iaf_raw_weight(L, p.variant, t, ci, co);
-      if (t == 0 && !iaf_centre_visible(ci, co, L.cin, L.cout, L.zerodiag)) v = 0.f;
-      L.w_out[((size_t)t * L.cin + ci) * L.cout_pad + col] = v * factor;
+      L.w_out[((size_t)t * L.cin + ci) * L.cout_pad + col] = iaf_masked_weight(L, p.vf, t, ci, co) * factor;
     } else {
-      const int t = e - n_real + 1;
-      L.padw_out[(size_t)(t - 1) * L.cout_pad + col] = iaf_raw_weight(L, p.variant, t, L.cin, co) * factor;
+      const int t = t_pad0 + e - n_real;
+      if (t > 0) L.padw_out[(size_t)(t - 1) * L.cout_pad + col] = iaf_masked_weight(L, p.vf, t, L.cin, co) * factor;
     }
   }
   if (tid == 0) L.bias_out[col] = L.bias[co];

@@ -11,7 +11,9 @@
 // set, so it is run as the TF form on the point-reflected image: loads and stores map
 // pixel p -> H*W-1-p ("flip"), nothing else changes.  Zero rows/columns around the band
 // give the SAME / pad2dwithchannel zero padding; the Theano pad channel (conv.py:71-83)
-// is a position-dependent bias added in the epilogue.
+// is a position-dependent bias added in the epilogue.  With flipmask (the mask reversed,
+// ar.py:263-264) the true convolution reads the TF offsets themselves: no reflection, the
+// pad-channel bias kept (IafVariantFlags, iaf_common.h).
 //
 // Dependencies only look forward (down/right), so a band of R output rows needs R+1 rows
 // of the last hidden layer, R+2 of the one before, ... : halo rows are recomputed, never

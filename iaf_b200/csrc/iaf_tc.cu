@@ -19,7 +19,8 @@
 //
 // Schedule: one launch per conv stage (iaf_tc_gemm.cuh); the same stage kernel runs the data
 // gradient of the backward on the point-reflected stream.
-// Orientation of the Theano variant: see iaf_simt.cu (point reflection on load/store).
+// Orientation of the Theano variants: see IafVariantFlags in iaf_common.h (point reflection on load/store, pad-channel
+// table; the flipmask variant keeps the table without the reflection).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -243,22 +244,14 @@ struct TcPackLayer {
 };
 struct TcPackParams {
   TcPackLayer layer[IAF_MAX_HIDDEN + IAF_MAX_HEADS];
-  int n_layers, variant;
+  int n_layers;
+  IafVariantFlags vf;
 };
 
-__device__ __forceinline__ bool tc_centre_visible(int ci, int co, int cin, int cout, int zd) {
-  if (cout >= cin) {
-    const int k = cout / cin, i = co / k;
-    return zd ? (ci < i) : (ci <= i);
-  }
-  const int k = cin / cout;
-  return zd ? (ci < co * k) : (ci < (co + 1) * k);
-}
-__device__ __forceinline__ float tc_raw_weight(const TcPackLayer& L, int variant, int t, int ci, int co) {
-  const int ky = t < 2 ? 1 : 2;
-  const int kx = t == 0 ? 1 : (t == 1 ? 2 : t - 2);
-  if (variant == IAF_VARIANT_TF) return L.w[((size_t)(ky * 3 + kx) * L.cin + ci) * L.cout + co];
-  return L.w[(((size_t)co * (L.cin + 1) + ci) * 3 + ky) * 3 + kx];
+// raw weight of canonical tap t, input channel ci (ci == cin: pad channel), output channel co; 0 where not live
+__device__ __forceinline__ float tc_masked_weight(const TcPackLayer& L, const IafVariantFlags& vf, int t, int ci, int co) {
+  const IafTap tp = iaf_tap_rule(t, ci, co, L.cin, L.cout, L.zerodiag, vf.flipmask);
+  return tp.live ? L.w[iaf_raw_index(vf.theano, tp.k, ci, co, L.cin, L.cout)] : 0.f;
 }
 
 __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant__ TcPackParams p) {
@@ -267,17 +260,18 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
   if (co >= L.cout) return;
   const int tid = threadIdx.x;
   const int n_real = L.cin * IAF_NTAPS;
-  const int n_pad = (p.variant == IAF_VARIANT_THEANO) ? 4 : 0;
+  // pad channel: taps 1..4; flipped, also its centre, which only enters the norm (see iaf_tap_rule)
+  const int n_pad = p.vf.pad_channel ? (p.vf.flipmask ? 5 : 4) : 0;
+  const int t_pad0 = IAF_NTAPS - n_pad;
   float ss = 0.f, am = 0.f;  // sum of squares (normalisation, pad channel included) and max |w| of the column's real taps
   for (int e = tid; e < n_real + n_pad; e += blockDim.x) {
     float v;
     if (e < n_real) {
       const int t = e / L.cin, ci = e % L.cin;
-      v = tc_raw_weight(L, p.variant, t, ci, co);
-      if (t == 0 && !tc_centre_visible(ci, co, L.cin, L.cout, L.zerodiag)) v = 0.f;
+      v = tc_masked_weight(L, p.vf, t, ci, co);
       am = fmaxf(am, fabsf(v));
     } else {
-      v = tc_raw_weight(L, p.variant, e - n_real + 1, L.cin, co);
+      v = tc_masked_weight(L, p.vf, t_pad0 + e - n_real, L.cin, co);
     }
     ss = fmaf(v, v, ss);
   }
@@ -293,8 +287,8 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
     __syncthreads();
   }
   ss = red[0];
-  const float factor = (p.variant == IAF_VARIANT_TF) ? expf(L.scale[co]) / sqrtf(fmaxf(ss, 1e-12f))
-                                                     : expf(3.0f * L.scale[co]) / (sqrtf(ss) + 1e-8f);
+  const float factor = !p.vf.theano ? expf(L.scale[co]) / sqrtf(fmaxf(ss, 1e-12f))
+                                    : expf(3.0f * L.scale[co]) / (sqrtf(ss) + 1e-8f);
   // the column's weight scale: its largest |w| into [32, 64), so that the lo half of every sizeable weight is a normal
   // fp16 number and the largest stays inside the fp16 range.  fl(|v| factor) is monotone in |v|: redm[0] * factor is
   // exactly the largest |v * factor| of the loop below.  The bias and the pad-channel terms stay unscaled fp32.
@@ -304,8 +298,7 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
   for (int e = tid; e < n_real + n_pad; e += blockDim.x) {
     if (e < n_real) {
       const int t = e / L.cin, ci = e % L.cin;
-      float v = tc_raw_weight(L, p.variant, t, ci, co);
-      if (t == 0 && !tc_centre_visible(ci, co, L.cin, L.cout, L.zerodiag)) v = 0.f;
+      const float v = tc_masked_weight(L, p.vf, t, ci, co);
       const float vc = v * factor * wsc;  // (a power of two: exact)
       // K order [ci / 16][tap][ci % 16]: one K-step of the stage kernel is one 16-channel block over the five taps
       const int k = ((ci >> 4) * IAF_NTAPS + t) * 16 + (ci & 15);
@@ -318,8 +311,8 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
       L.whi[o] = h;
       L.wlo[o] = l;
     } else {
-      const int t = e - n_real + 1;
-      L.padw_out[(size_t)(t - 1) * L.N + col] = tc_raw_weight(L, p.variant, t, L.cin, co) * factor;
+      const int t = t_pad0 + e - n_real;
+      if (t > 0) L.padw_out[(size_t)(t - 1) * L.N + col] = tc_masked_weight(L, p.vf, t, L.cin, co) * factor;
     }
   }
   if (tid == 0) {
@@ -333,6 +326,7 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
 // ------------------------------------------------------------------------------------------
 struct IafTcPlan {
   iaf_desc_t d;
+  IafVariantFlags vf;
   int n_stages;
   int cin[IAF_MAX_STAGES], N[IAF_MAX_STAGES], K[IAF_MAX_STAGES];
   __nv_bfloat16* whi[IAF_MAX_STAGES];
@@ -465,6 +459,7 @@ int iaf_tc_plan_create(IafTcPlan** out, const iaf_desc_t* d) {
   if (!pl) return IAF_ERR_BAD_ARG;
   memset(pl, 0, sizeof(*pl));
   pl->d = *d;
+  pl->vf = iaf_variant_flags(d->variant);
   if (!ly_layout(d, pl)) { delete pl; return IAF_ERR_UNSUPPORTED; }
   // IAF_TC_FUSED=0 (development): one-hidden-layer stacks on the per-stage kernel too, for A/B against the fused one
   const char* fe = getenv("IAF_TC_FUSED");
@@ -519,7 +514,7 @@ int iaf_tc_pack(IafTcPlan* pl, const float* const* w, const float* const* scale,
   TcPackParams pp;
   memset(&pp, 0, sizeof(pp));
   pp.n_layers = d.n_hidden + d.n_heads;
-  pp.variant = d.variant;
+  pp.vf = pl->vf;
   int max_cout = 0;
   for (int j = 0; j < pl->n_stages; ++j) {
     const size_t wb = (size_t)pl->K[j] * pl->N[j] * 2;
@@ -626,13 +621,13 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
   p.B = B; p.C = d.n_z; p.H = d.H; p.W = d.W; p.Wp = d.W + 1; p.SPS = SPS; p.HW = d.H * d.W;
   p.S = S; p.NT = NT;
   p.MIR = pl->MIR; p.WIN = pl->WIN; p.MAXS = pl->MAXS;
-  p.flip = d.variant == IAF_VARIANT_THEANO ? 1 : 0;
+  p.flip = pl->vf.reflect;
   p.nl = d.nl; p.scale = 0.1f;
   p.mg_sps = (unsigned)((1ULL << 32) / (unsigned)SPS) + 1u;
   p.mg_wp = (unsigned)((1ULL << 32) / (unsigned)p.Wp) + 1u;
   p.mg_win = (unsigned)((1ULL << 32) / (unsigned)p.WIN) + 1u;
   const int grid = std::min(pl->num_sms, NT);
-  const bool padw = d.variant == IAF_VARIANT_THEANO, elu = d.nl == IAF_NL_ELU;
+  const bool padw = pl->vf.pad_channel, elu = d.nl == IAF_NL_ELU;
   auto launch = [&](LyKernel lk, const IafLyParams& q, size_t smem) {
     const char* pe = getenv("IAF_PDL");
     cudaLaunchConfig_t cfg;
@@ -714,6 +709,7 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
 // ------------------------------------------------------------------------------------------
 struct IafDgPlan {
   iaf_desc_t d;
+  int grad_flip;  // the gradient stream: the point reflection of the forward's (1 - IafVariantFlags::reflect)
   int n_stages;
   int kin[IAF_MAX_STAGES], nout[IAF_MAX_STAGES];  // dgrad of layer j: input planes (= packed columns of layer j), output channels (= cin of layer j)
   __nv_bfloat16* whi[IAF_MAX_STAGES];
@@ -878,6 +874,7 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
   if (!pl) return IAF_ERR_BAD_ARG;
   memset(pl, 0, sizeof(*pl));
   pl->d = *d;
+  pl->grad_flip = iaf_variant_flags(d->variant).reflect ? 0 : 1;
   pl->n_stages = n_stages;
   pl->MIR = MIR; pl->WIN = TC_TILE + MIR; pl->MAXS = (TC_TILE - 1) / SPS + 2;
   pl->num_sms = prop.multiProcessorCount;
@@ -971,7 +968,7 @@ int iaf_dg_begin(IafDgPlan* pl, const float* g_heads, int B, cudaStream_t stream
   q.g = g_heads; q.amax = pl->amax; q.o_hi = pl->img[0][0]; q.o_lo = pl->img[0][1];
   q.planes = pl->kin[pl->n_stages - 1]; q.H = d.H; q.W = d.W; q.Wp = d.W + 1; q.SPS = (d.H + 1) * (d.W + 1);
   q.HW = d.H * d.W; q.S_pad = pl->img_S_pad;
-  q.flip = d.variant == IAF_VARIANT_THEANO ? 0 : 1;  // the data gradient runs on the point-reflected stream of the forward
+  q.flip = pl->grad_flip;  // the data gradient runs on the point-reflected stream of the forward
   q.xmode = 0; q.B = B;
   // gridDim.y splits the image planes; every y-block recomputes the sample's max (L2 hits) and writes the same value
   q.S_end = ((B * q.SPS + TC_TILE - 1) / TC_TILE + 1) * TC_TILE;
@@ -1007,7 +1004,7 @@ int iaf_dg_stage(IafDgPlan* pl, int j, const float* w_packed, int in_buf, const 
   p.B = B; p.C = d.n_z; p.H = d.H; p.W = d.W; p.Wp = d.W + 1; p.SPS = SPS; p.HW = d.H * d.W;
   p.S = S; p.NT = NT;
   p.MIR = pl->MIR; p.WIN = pl->WIN; p.MAXS = pl->MAXS; p.sm_part = pl->sm_part[j];
-  p.flip = d.variant == IAF_VARIANT_THEANO ? 0 : 1;
+  p.flip = pl->grad_flip;
   p.nl = d.nl; p.scale = 0.1f;
   p.mg_sps = (unsigned)((1ULL << 32) / (unsigned)SPS) + 1u;
   p.mg_wp = (unsigned)((1ULL << 32) / (unsigned)p.Wp) + 1u;
@@ -1046,7 +1043,7 @@ int iaf_wg_run(IafDgPlan* pl, int j, const float* x, int g_buf, float* part, int
     memset(&q, 0, sizeof(q));
     q.g = x; q.amax = pl->amax; q.o_hi = pl->ximg[0]; q.o_lo = pl->ximg[1];
     q.planes = cin; q.H = d.H; q.W = d.W; q.Wp = d.W + 1; q.SPS = SPS; q.HW = d.H * d.W; q.S_pad = pl->img_S_pad;
-    q.flip = d.variant == IAF_VARIANT_THEANO ? 0 : 1;
+    q.flip = pl->grad_flip;
     q.xmode = 1; q.B = B;
     q.S_end = ((B * SPS + TC_TILE - 1) / TC_TILE + 1) * TC_TILE;
     iaf_dg_image_kernel<<<dim3(B + 1, std::max(1, cin / 32)), 256, 0, stream>>>(q);
@@ -1210,8 +1207,8 @@ int iaf_dg_begin_step(IafDgPlan* pl, const float* z_out, const float* logsd, con
   q.H = d.H; q.W = d.W; q.Wp = d.W + 1; q.SPS = (d.H + 1) * (d.W + 1); q.HW = d.H * d.W;
   q.S_pad = pl->img_S_pad;
   q.S_end = ((B * q.SPS + TC_TILE - 1) / TC_TILE + 1) * TC_TILE;
-  q.fwd_flip = d.variant == IAF_VARIANT_THEANO ? 1 : 0;
-  q.img_flip = q.fwd_flip ? 0 : 1;
+  q.img_flip = pl->grad_flip;
+  q.fwd_flip = q.img_flip ? 0 : 1;
   q.scale = 0.1f;
   iaf_dg_step_kernel<<<B + 1, 256, (size_t)q.cp * q.HW * 4, stream>>>(q);
   if (bias_partials) *bias_partials = pl->bstep;

@@ -1,7 +1,8 @@
 """ELBO forward of the Theano front-end around the IAF operator (SURVEY 8f-2, configs C1 / C4):
 `cvae1.f_encode_decode` (models.py:435-497) with `cvae_layer.up` / `cvae_layer.down_q` (models.py:133-328) for
 ``posterior='down_iaf2_nl'`` (the README configs, train.py:55-75) and ``posterior='up_iaf2_nl'`` (the bottom-up
-placement of the same operator, models.py:169-178), ``prior='diag'``, ``px='logistic'``, ``downsample_type='nn'``,
+placement of the same operator, models.py:169-178) and ``posterior='down_iaf2_nl2'`` (two steps, the second with
+``flipmask=True``: models.py:93-98, 286-291), ``prior='diag'``, ``px='logistic'``, ``downsample_type='nn'``,
 restated in PyTorch so that bits/dim can be compared between the CUDA operator and the oracle
 operator on identical weights, inputs and noise.
 
@@ -11,7 +12,11 @@ up_iaf2_nl the plain step ``iaf_layer.step(name, z, context) -> (z', arw_logsd)`
 only known later, so the KL is assembled top-down from the stored sample and log q); the rest is plumbing on stock
 torch ops.  Parameters are a dict under the reference's Theano names (graphy/nodes/conv.py:156-173, ar.py:288-296): ``x_enc_{w,b,s}``, ``x_dec_{w,b,s}``, ``logsd_x``,
 ``h_top``, ``{i}_{j}_up_conv1_{ds}_*``, ``{i}_{j}_up_conv2_*``, ``{i}_{j}_down_conv1_*``, ``{i}_{j}_down_conv2_{ds}_*``,
-``{i}_{j}_posterior_conv1_{k}_*`` and ``{i}_{j}_posterior_conv1_out_{k}_*``.
+``{i}_{j}_posterior_conv1_{k}_*`` and ``{i}_{j}_posterior_conv1_out_{k}_*`` (down_iaf2_nl2 also
+``{i}_{j}_posterior_conv2_{k}_*`` and ``{i}_{j}_posterior_conv2_out_{k}_*``).  For down_iaf2_nl2 the block is
+sample -> step(conv1) -> step(conv2, reversed order) -> KL with both ``arw_logsd`` in log q, assembled by
+:func:`iaf_b200.elbo.stochastic_layer` around the two calls ``iaf_layer.step(name, z, context, conv)``, conv = 1, 2.
+Any other posterior name raises ``ValueError``.
 """
 import math
 
@@ -20,6 +25,15 @@ import torch
 import torch.nn.functional as F
 
 LOGSCALE_SCALE = 3.0  # graphy/nodes/conv.py:19 (conv.py:16-22: logscale=True, bn=False, maxweight=0)
+POSTERIORS = ("down_iaf2_nl", "up_iaf2_nl", "down_iaf2_nl2")
+
+
+def posterior_of(hps):
+    """The posterior of ``hps`` (default down_iaf2_nl); any other reference posterior is refused, not approximated."""
+    p = hps.get("posterior", "down_iaf2_nl")
+    if p not in POSTERIORS:
+        raise ValueError("posterior %r is not implemented (available: %s)" % (p, ", ".join(POSTERIORS)))
+    return p
 
 
 def pad2dwithchannel(x, k):
@@ -88,7 +102,7 @@ def layer_up(w, name, h_in, hps, downsample, eps=None, iaf_layer=None):
     h_det, qz_mean, qz_logsd, up_context = torch.split(h, [nh2, nz, nz, nh2], dim=1)
     if downsample:
         h_in = downsample_nn(h_in)
-    if hps.get("posterior", "down_iaf2_nl") == "up_iaf2_nl":
+    if posterior_of(hps) == "up_iaf2_nl":
         z0 = qz_mean + torch.exp(qz_logsd) * eps                       # gaussian_diag(qz_mean, 2 qz_logsd).sample
         logqs = gaussian_logps(qz_mean, 2 * qz_logsd, z0)
         z, arw_logsd = iaf_layer.step(name, z0.contiguous(), up_context.contiguous())
@@ -103,7 +117,8 @@ def layer_down_q(w, name, h_in, up_state, eps, iaf_layer, hps, downsample):
     nz, nh2, nl = hps["n_z"], hps["n_h2"], hps["nl"]
     ds = 2 if downsample else 1
     h = conv2d(w, name + "_down_conv1", nonlinearity(h_in, nl))
-    if hps.get("posterior", "down_iaf2_nl") == "up_iaf2_nl":            # models.py:215-217, 287-290
+    posterior = posterior_of(hps)
+    if posterior == "up_iaf2_nl":                                      # models.py:215-217, 287-290
         h_det, pz_mean, pz_logsd = torch.split(h, [nh2, nz, nz], dim=1)
         z, logqs = up_state
         kl = logqs - gaussian_logps(pz_mean, 2 * pz_logsd, z)
@@ -116,8 +131,19 @@ def layer_down_q(w, name, h_in, up_state, eps, iaf_layer, hps, downsample):
     h_det, pz_mean, pz_logsd, rz_mean, rz_logsd, down_context = torch.split(h, [nh2, nz, nz, nz, nz, nh2], dim=1)
     qz_mean, qz_logsd, up_context = up_state
     # posterior N(qz.mean + rz_mean, qz.logvar + 2 rz_logsd) with qz.logvar = 2 qz_logsd (models.py:139,275)
-    z, kl_bc, kl_sum = iaf_layer(name, eps, (qz_mean + rz_mean).contiguous(), (qz_logsd + rz_logsd).contiguous(),
-                                 pz_mean.contiguous(), pz_logsd.contiguous(), (up_context + down_context).contiguous())
+    stats = ((qz_mean + rz_mean).contiguous(), (qz_logsd + rz_logsd).contiguous(), pz_mean.contiguous(),
+             pz_logsd.contiguous(), (up_context + down_context).contiguous())
+    if posterior == "down_iaf2_nl2":
+        # models.py:281-291: step(conv1), then step(conv2) in the reversed order; both arw_logsd go into logqs
+        from .elbo import stochastic_layer
+
+        def two_steps(z, c):
+            z, a1 = iaf_layer.step(name, z, c, 1)
+            z, a2 = iaf_layer.step(name, z.contiguous(), c, 2)
+            return z, a1 + a2
+        z, kl_bc, kl_sum = stochastic_layer(two_steps, eps, *stats)
+    else:
+        z, kl_bc, kl_sum = iaf_layer(name, eps, *stats)
     hh = torch.cat([h_det, z], dim=1)
     if downsample:
         h_in = upsample_nn(h_in)
@@ -174,7 +200,8 @@ def make_params(hps, seed=0, dtype=np.float32):
     """Seeded synthetic parameters under the reference's Theano names and shapes (no checkpoint exists offline)."""
     rng = np.random.RandomState(seed)
     nz, nh1, nh2, depths = hps["n_z"], hps["n_h1"], hps["n_h2"], hps["depths"]
-    up_post = hps.get("posterior", "down_iaf2_nl") == "up_iaf2_nl"
+    posterior = posterior_of(hps)
+    up_post = posterior == "up_iaf2_nl"
     w = {}
 
     def conv(name, cin, cout, k, pad_channel=True):
@@ -199,24 +226,34 @@ def make_params(hps, seed=0, dtype=np.float32):
                 conv("%s_posterior_conv1_%d" % (n, k), sizes[k], sizes[k + 1], 3)
             for k in range(2):
                 conv("%s_posterior_conv1_out_%d" % (n, k), sizes[-1], nz, 3)
+            if posterior == "down_iaf2_nl2":                           # models.py:98
+                for k in range(hps["depth_ar"]):
+                    conv("%s_posterior_conv2_%d" % (n, k), sizes[k], sizes[k + 1], 3)
+                for k in range(2):
+                    conv("%s_posterior_conv2_out_%d" % (n, k), sizes[-1], nz, 3)
     return w
 
 
 class CudaIAF(object):
-    """iaf_layer callable backed by the fused CUDA operator, Theano variant (one IAFOperator per layer name)."""
+    """iaf_layer callable backed by the fused CUDA operator, Theano variant: one IAFOperator per layer name and
+    posterior conv (conv 2, down_iaf2_nl2's second step, is the flipmask operator)."""
 
     def __init__(self, w, hps, path="auto"):
         from .ops import IAFOperator
         self.w, self.hps, self.path, self.IAFOperator, self.ops = w, hps, path, IAFOperator, {}
 
-    def _op(self, name, device):
-        op = self.ops.get(name)
+    def _new_op(self, conv):
+        nz, nh2, dar = self.hps["n_z"], self.hps["n_h2"], self.hps["depth_ar"]
+        return self.IAFOperator("theano", nz, dar * [nh2], [nz, nz], nl=self.hps["nl"], path=self.path,
+                                flipmask=conv == 2)                    # models.py:92,97-98
+
+    def _op(self, name, device, conv=1):
+        op = self.ops.get((name, conv))
         if op is None:
             from .weights import theano_layers
-            nz, nh2, dar = self.hps["n_z"], self.hps["n_h2"], self.hps["depth_ar"]
-            op = self.IAFOperator("theano", nz, dar * [nh2], [nz, nz], nl=self.hps["nl"], path=self.path)   # models.py:92
-            op.set_weights(theano_layers(self.w, name + "_posterior_conv1", dar, device=device))
-            self.ops[name] = op
+            op = self._new_op(conv)
+            op.set_weights(theano_layers(self.w, "%s_posterior_conv%d" % (name, conv), self.hps["depth_ar"], device=device))
+            self.ops[(name, conv)] = op
         return op
 
     def invalidate(self):
@@ -230,9 +267,9 @@ class CudaIAF(object):
                                                                 context, want_kl=False)
         return z, kl_bc, kl_cost
 
-    def step(self, name, z, context):
-        """up_iaf2_nl: the bare step (models.py:170-173) -> (z', arw_logsd)."""
-        z_new, arw_logsd, _ = self._op(name, z.device).step(z, context)
+    def step(self, name, z, context, conv=1):
+        """The bare step of posterior conv ``conv`` (models.py:170-173; 281-291) -> (z', arw_logsd)."""
+        z_new, arw_logsd, _ = self._op(name, z.device, conv).step(z, context)
         return z_new, arw_logsd
 
 
@@ -241,15 +278,15 @@ class CudaIAFTrain(CudaIAF):
     reference, graphy/misc/optim.py:99-123): the posterior sample, logqs, prior logps and the KL sums are torch ops
     (models.py:273-298) around ``IAFOperator.step``, whose autograd node runs iaf_step_fwd_train / iaf_step_bwd_saved
     (SURVEY 8f-4).  The parameter tensors are re-bound on every call so gradients flow to the entries of ``w``
-    (``{name}_posterior_conv1_{k}_w/_s/_b``), with masked taps at exactly zero (ar.py:369-373)."""
+    (``{name}_posterior_conv{1,2}_{k}_w/_s/_b``), with masked taps at exactly zero (ar.py:369-373)."""
 
-    def _op(self, name, device):
-        op = self.ops.get(name)
-        nz, nh2, dar = self.hps["n_z"], self.hps["n_h2"], self.hps["depth_ar"]
+    def _op(self, name, device, conv=1):
+        op = self.ops.get((name, conv))
+        dar = self.hps["depth_ar"]
         if op is None:
-            op = self.IAFOperator("theano", nz, dar * [nh2], [nz, nz], nl=self.hps["nl"], path=self.path)   # models.py:92
-            self.ops[name] = op
-        pre = name + "_posterior_conv1"
+            op = self._new_op(conv)
+            self.ops[(name, conv)] = op
+        pre = "%s_posterior_conv%d" % (name, conv)
         names = ["%s_%d" % (pre, i) for i in range(dar)] + ["%s_out_%d" % (pre, k) for k in range(2)]
         # the live tensors of w (float32, on the device): not detached, so their .grad is filled by backward()
         op.set_weights([(self.w[n + "_w"], self.w[n + "_s"], self.w[n + "_b"]) for n in names])

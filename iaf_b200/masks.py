@@ -28,11 +28,14 @@ def tf_conv_ar_mask(n_in, n_out, zerodiagonal):
     return m
 
 
-def theano_conv_ar_mask(n_in, n_out, size_kernel=(3, 3), zerodiagonal=True):
-    """[n_out, n_in+1, 3, 3] including the pad channel (never sees the centre tap)."""
+def theano_conv_ar_mask(n_in, n_out, size_kernel=(3, 3), zerodiagonal=True, flipmask=False):
+    """[n_out, n_in+1, 3, 3] including the pad channel (never sees the centre tap).  flipmask: the mask reversed on all
+    four axes, pad channel included (ar.py:263-264); the pad channel then inherits channel 0's centre column."""
     assert tuple(size_kernel) == (3, 3)
     m = np.zeros((n_out, n_in + 1, 3, 3), np.float32)
     m[:, :, 1, 2] = 1
     m[:, :, 2, :] = 1
     m[:, :n_in, 1, 1] = centre_visible(n_in, n_out, zerodiagonal).T
+    if flipmask:
+        m = np.ascontiguousarray(m[::-1, ::-1, ::-1, ::-1])
     return m

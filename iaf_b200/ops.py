@@ -51,17 +51,22 @@ class IAFOperator(object):
     variant: "tf" (tf_utils/layers.py numerics) or "theano" (graphy/nodes/ar.py numerics).
     layers:  list of (w, scale, bias) tensors, hidden layers first then heads, in the
              reference's layouts: tf V [3,3,Cin,Cout], g, b; theano w [Cout,Cin+1,3,3], s, b.
+    flipmask: (theano only) the reversed autoregressive order of ``multiconv2d(..., flipmask=True)``
+             (ar.py:263-264), e.g. the second step of posterior='down_iaf2_nl2' (models.py:98).
     """
 
-    def __init__(self, variant, n_z, hidden, heads, nl="elu", path="auto", checknan=None):
+    def __init__(self, variant, n_z, hidden, heads, nl="elu", path="auto", checknan=None, flipmask=False):
         """checknan="raise": the reference driver's NaN guard (graphy/function.py:107-110 raises "NaN detected" when the sum
         of a minibatch's outputs is NaN; train.py:211, tf_train.py:283-285 stop likewise): after a step, the per-sample
         logdet (a sum over every element the kernel produced) is checked on the host.  Off by default: it synchronises."""
         if checknan not in (None, "raise"):
             raise ValueError("checknan must be None or 'raise'")
         self.checknan = checknan
-        if variant not in _lib.VARIANTS:
+        if variant not in ("tf", "theano"):
             raise ValueError("variant must be 'tf' or 'theano'")
+        if flipmask and variant != "theano":
+            raise ValueError("flipmask is a Theano-front-end option (graphy/nodes/ar.py); tf_utils/layers.py has none")
+        self.flipmask = bool(flipmask)
         if nl not in _lib.NLS:
             raise NotImplementedError("nonlinearity %r is not available in the fused kernel" % (nl,))
         if path not in _lib.PATHS:
@@ -131,7 +136,7 @@ class IAFOperator(object):
                 raise _lib.CaptureError("iaf_b200: the first call of an IAFOperator for a map size cannot run inside a "
                                         "CUDA-graph capture (" + _lib.CAPTURE_HINT + ")")
             d = _lib.IafDesc()
-            d.variant = _lib.VARIANTS[self.variant]
+            d.variant = _lib.VARIANTS["theano_flipmask" if self.flipmask else self.variant]
             d.n_z = self.n_z
             d.n_hidden = len(self.hidden)
             for i, h in enumerate(self.hidden):
@@ -585,22 +590,21 @@ def multiconv2d(name, n_in, n_h, n_out, size_kernel=(3, 3), flipmask=False, nl="
         n_out = [n_out]
     if tuple(size_kernel) != (3, 3):
         raise NotImplementedError("only the 3x3 kernel the reference uses (train.py:63) is implemented")
-    if flipmask:
-        raise NotImplementedError("flipmask=True is never used on the down_iaf2_nl / up_iaf2_nl path (models.py:92)")
+    flipmask = bool(flipmask)  # ar.py:263-264: the reversed order (second step of down_iaf2_nl2, models.py:98)
     sizes = [n_in] + list(n_h)
     names, masks = [], []
     specs = [(name + "_" + str(i), sizes[i], sizes[i + 1], False) for i in range(len(n_h))]
     specs += [(name + "_out_" + str(i), sizes[-1], n_out[i], True) for i in range(len(n_out))]
     for lname, cin, cout, zd in specs:
         assert cin % cout == 0 or cout % cin == 0  # ar.py:250,257
-        mask = theano_conv_ar_mask(cin, cout, (3, 3), zd)
+        mask = theano_conv_ar_mask(cin, cout, (3, 3), zd, flipmask)
         if lname + "_w" not in w:  # ar.py:288, 293-296
             w[lname + "_w"] = torch.from_numpy(mask * 0.05 * np.random.randn(cout, cin + 1, 3, 3)).float().to(device)
             w[lname + "_b"] = torch.zeros(cout, device=device)
             w[lname + "_s"] = torch.zeros(cout, device=device)
         names.append(lname)
         masks.append(mask)
-    op = IAFOperator("theano", n_in, n_h, n_out, nl=nl, path=path)
+    op = IAFOperator("theano", n_in, n_h, n_out, nl=nl, path=path, flipmask=flipmask)
 
     def f(h, context, w, return_hiddens=False):
         if return_hiddens:
@@ -613,7 +617,8 @@ def multiconv2d(name, n_in, n_h, n_out, size_kernel=(3, 3), flipmask=False, nl="
 
     def postup(updates, w):
         """ar.py:369-373: re-apply the mask to an updated weight.  ``updates`` maps parameter
-        name -> new value (Theano keys by shared variable; names are the eager equivalent)."""
+        name -> new value (Theano keys by shared variable; names are the eager equivalent).
+        The mask only: l2normalize's zero-diagonal rows (ar.py:273-276) stay in the parameter."""
         for n, m in zip(names, masks):
             if n + "_w" in updates:
                 u = updates[n + "_w"]

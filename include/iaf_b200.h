@@ -38,8 +38,11 @@ typedef enum {
 
 /* which of the reference's two implementations the numerics follow (SURVEY F2) */
 typedef enum {
-  IAF_VARIANT_TF = 0,    /* tf_utils/layers.py: SAME zero pad, cross-correlation, exp(g)*rsqrt(max(ss,1e-12)) */
-  IAF_VARIANT_THEANO = 1 /* graphy/nodes/ar.py: pad channel, true convolution, exp(3s)/(sqrt(ss)+1e-8)        */
+  IAF_VARIANT_TF = 0,             /* tf_utils/layers.py: SAME zero pad, cross-correlation, exp(g)*rsqrt(max(ss,1e-12)) */
+  IAF_VARIANT_THEANO = 1,         /* graphy/nodes/ar.py: pad channel, true convolution, exp(3s)/(sqrt(ss)+1e-8)        */
+  IAF_VARIANT_THEANO_FLIPMASK = 2 /* the same with flipmask=True (ar.py:263-264): the mask reversed on all four axes,
+                                     pad channel included -- the reversed autoregressive order of the second step of
+                                     posterior='down_iaf2_nl2' (models.py:98,286-291).  Same parameter layouts.        */
 } iaf_variant;
 
 /* graphy/nodes/__init__.py:158-177 (parameter-free entries); tf.nn.elu */
@@ -55,8 +58,8 @@ typedef enum {
  * Static description of one masked-AR conv stack; the arguments of
  *   multiconv2d(name, n_in, n_h, n_out, size_kernel, flipmask, nl, w)   graphy/nodes/ar.py:378
  *   ar_multiconv2d(name, x, context, n_h, n_out, nl)                     tf_utils/layers.py:159
- * size_kernel is fixed to 3x3 (the only size either caller uses: train.py:63, layers.py:145)
- * and flipmask to False (models.py:92).
+ * size_kernel is fixed to 3x3 (the only size either caller uses: train.py:63, layers.py:145);
+ * flipmask is variant IAF_VARIANT_THEANO_FLIPMASK (the TF front-end has no flipmask).
  */
 typedef struct iaf_desc {
   int variant;                /* iaf_variant                                               */
