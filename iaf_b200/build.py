@@ -16,26 +16,27 @@ def _nvcc():
     return shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 
 
-def _stale():
-    if not os.path.exists(LIB):
+def _stale(lib):
+    if not os.path.exists(lib):
         return True
-    t = os.path.getmtime(LIB)
+    t = os.path.getmtime(lib)
     deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "iaf_b200.h")]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False):
-    """Compile the CUDA sources into iaf_b200/lib/libiaf_b200.so.  Returns the path."""
-    if not force and not _stale():
-        return LIB
-    os.makedirs(LIBDIR, exist_ok=True)
-    cmd = [_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB] + SOURCES
+def build(force=False, verbose=False, lib=LIB, defines=()):
+    """Compile the CUDA sources into `lib` (default iaf_b200/lib/libiaf_b200.so) with -D`defines`.  Returns the path."""
+    if not force and not _stale(lib):
+        return lib
+    os.makedirs(os.path.dirname(lib), exist_ok=True)
+    cmd = ([_nvcc()] + NVCC_FLAGS + ["-D" + d for d in defines] + (["-Xptxas", "-v"] if verbose else []) +
+           ["-o", lib] + SOURCES)
     r = subprocess.run(cmd, cwd=CSRC, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + " ".join(cmd) + "\n" + r.stdout + r.stderr)
     if verbose:
         print(r.stderr)
-    return LIB
+    return lib
 
 
 if __name__ == "__main__":

@@ -36,7 +36,7 @@
 #define TC_WTHREADS (TC_WORKERS * 32)
 #define TC_TILE 128
 #ifdef IAF_TC_TIMELINE
-#define TC_SMEM_LIMIT (227 * 1024 - 512 - 2560)  // room for the static event buffers
+#define TC_SMEM_LIMIT (227 * 1024 - 512 - 9472)  // room for the static event buffers (4 x TL_MAX x 24 B + counts)
 #else
 #define TC_SMEM_LIMIT (227 * 1024 - 512)  // opt-in maximum minus the kernels' static shared memory (barriers: < 512 B)
 #endif
@@ -118,6 +118,79 @@ __device__ __forceinline__ void wgmma_m64n16k16(float* d, uint64_t a_desc, uint6
       : "l"(a_desc), "l"(b_desc), "r"(1), "n"(MN)
       : "memory");
 }
+// The same, N = 16 NGW columns in one instruction (K-major operands): the A tile is fetched once for all N columns
+// instead of once per 16.  Fragment: d[4j + 2h + e] = row 16 w + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e, j < 2 NGW.
+template <int NGW>
+__device__ __forceinline__ void wgmma_m64nNk16(float* d, uint64_t a_desc, uint64_t b_desc);
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<1>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a_desc), "l"(b_desc), "r"(1)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<2>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a_desc), "l"(b_desc), "r"(1)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<3>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(a_desc), "l"(b_desc), "r"(1)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<4>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(1)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<5>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, %40, %41, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+      : "l"(a_desc), "l"(b_desc), "r"(1)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<6>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(a_desc), "l"(b_desc), "r"(1)
+      : "memory");
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -186,10 +259,13 @@ __device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, ui
   *reinterpret_cast<uint4*>(lo_ptr) = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
-// Optional in-kernel timeline (compile with -DIAF_TC_TIMELINE; development aid only): CTA 0 records
-// (tag, tile, clock) triples for the control lane and lane 0 of the first warp of each worker group.
+// Optional in-kernel timeline (compile with -DIAF_TC_TIMELINE; development aid only, tools/tl_run.py): CTA 0 of the
+// launch that sets tl_enable records (tag, tile or chunk, clock) triples per role.  Role 1, lane 0 of worker warp 0, after
+// the worker barrier that closes each phase: 0 tile start (the previous tile's last epilogue done), 10 z window built,
+// 20 (hidden) MMAs done, 30 (hidden) epilogue done, 40 heads MMAs done (fused), 99 kernel end.  Role 2, the producer:
+// 60 / 61 before / after waiting for a ring stage to be released (k = the weight chunk it will refill).
 #ifdef IAF_TC_TIMELINE
-#define TL_MAX 26
+#define TL_MAX 96
 __device__ long long g_tl[4][TL_MAX][3];
 __device__ int g_tl_n[4];
 // events are staged in shared memory (a global counter would cost an L2 round trip per event)

@@ -8,8 +8,8 @@
 //   * the weights are NOT resident (unless they fit the ring): the producer warp streams them in chunks of LY_KC
 //     K-steps through an NB-deep shared-memory ring (cp.async.bulk + expect_tx on an mbarrier); every worker warpgroup
 //     releases a ring stage once its wgmma reads of it have completed;
-//   * the 16 worker warps are four warpgroups: warpgroup w issues the wgmma m64n16k16 instructions for rows
-//     [64 (w & 1), +64) of the tile and every second 16-column group (starting at w >> 1), accumulating in registers.
+//   * the 16 worker warps are four warpgroups: warpgroup w issues one wgmma m64nNk16 per K-step, tap and product for
+//     rows [64 (w & 1), +64) of the tile and one contiguous half of its columns (w >> 1), accumulating in registers.
 //     The accumulators then go through a shared-memory tile [128][N + 4] so that the epilogue keeps one thread per slot
 //     (coalesced global traffic along pixels);
 //   * hidden stages write their output operand image back to global memory (16-byte stores), the heads stage applies
@@ -23,9 +23,10 @@
 #define LY_THREADS (LY_WTHREADS + 64)
 #define LY_KC 5        // K-steps (of 16) per weight chunk
 #define LY_MAX_NB 6
-// Bytes every layout of the stage kernel reserves past its last weight image: a padded column group (16 g >= N, see
+// Bytes every layout of the stage kernel reserves past its last weight image: the column span of the second half (see
 // ly_mma_tile) of the last K plane reads up to 16 * (32 * NGW - N) bytes past the plane's end -- 256 for the per-stage
-// instantiations, 512 for the fused one (NGW = 2, N = 32) -- and that read must stay inside the CTA's allocation.
+// instantiations (NGW = ceil(N / 32)), 768 for the fused one (NGW = 2, N down to 16: hidden [16]) -- and that read must
+// stay inside the CTA's allocation.
 #define LY_B_SLACK 1024
 
 enum { LB_BFULL = 0, LB_BEMPTY = LY_MAX_NB, LB_PART = 2 * LY_MAX_NB,
@@ -84,22 +85,26 @@ __device__ __forceinline__ float dg_scale_from_amax(float amax) {
   return __uint_as_float((uint32_t)(127 + 5 - e) << 23);
 }
 
-// The MMAs of one stage for one tile.  Warpgroup w (of the four worker warpgroups) computes rows [64 (w & 1), +64) and the
-// 16-column groups g = (w >> 1) + 2k, k < NGW: D[64 x 16] += A_t[64 x 16] B_t[16 x 16] over K-steps, taps and the three
-// split products, accumulating in registers, then writes its fragments into the accumulator tile.  NGW is a compile-time
-// count (groups past the stage's columns compute on whatever follows in shared memory -- the next K plane, the next
-// image, or the LY_B_SLACK bytes every layout reserves past its last one -- and are not stored), so every wgmma
-// is issued unconditionally and ptxas keeps them asynchronous.
-//   ring: weight chunk c sits in ring stage gchunk % NB (parity from gchunk / NB), released after its MMAs complete;
+// The MMAs of one stage for one tile.  Warpgroup w (of the four worker warpgroups) computes rows [64 (w & 1), +64) and
+// the 16 NGW contiguous columns from 16 NGW (w >> 1): D[64 x 16 NGW] += A_t[64 x 16] B_t[16 x 16 NGW] over K-steps, taps
+// and the three split products, one wgmma each, accumulating in registers, then writes its fragments into the
+// accumulator tile.  In the B image [K/8][N][8] a span of contiguous columns is one K-major descriptor (8-column groups
+// 128 B apart, the two K halves one plane apart).  NGW is a compile-time count: a span past the stage's columns computes
+// on whatever follows in shared memory -- the next K plane, the next image, or the LY_B_SLACK bytes every layout
+// reserves past its last one -- and is not stored, so every wgmma is issued unconditionally and ptxas keeps them
+// asynchronous.
+//   ring: the tile's weight chunks are the CTA's gchunk, gchunk + 1, ... (every tile streams all n_chunks); chunk g sits
+//   in ring stage g % NB (parity from g / NB), released after its MMAs complete;
 //   otherwise resident: chunk c sits in stage c behind barrier bar0 + c (parity 0).
 //   a_in_stage: the A chunk pair of K-step c rides in the ring stage before the weights; otherwise A is a window at a_addr.
 // The tile holds the products with the weight images as packed: the per-column weight scale is undone by the epilogues
 // as they read it (acc_ld16).
 template <int NGW>
 __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float* s_acc, int N, int n_chunks, bool ring, int NB,
-                                            int& gchunk, int bar0, uint32_t b_addr0, uint32_t stage_bytes,
+                                            int gchunk, int bar0, uint32_t b_addr0, uint32_t stage_bytes,
                                             uint32_t b_chunk_bytes, bool a_in_stage, uint32_t a_addr, uint32_t a_plane,
                                             uint32_t a_lo_off, int Wp) {
+  constexpr int NA = 8 * NGW;  // accumulators per thread: 64 x 16 NGW over the 128 threads of the warpgroup
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2, rh = wg & 1, gh = wg >> 1, wl = warp & 3;
   const uint32_t b_plane = (uint32_t)N * 16u;
@@ -111,18 +116,17 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
   // over K = 160 those roundings reach ~2e-7 of a unit pre-activation -- enough to put a ReLU's derivative on the wrong
   // side of a pre-activation that small.  Summed apart and added once at the end, they cost one rounding.
   constexpr bool SPLIT = NGW <= 2;
-  float acc[NGW][8], acl[SPLIT ? NGW : 1][8];
+  float acc[NA], acl[SPLIT ? NA : 1];
 #pragma unroll
-  for (int k = 0; k < NGW; ++k)
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      acc[k][e] = 0.f;
-      if (SPLIT) acl[SPLIT ? k : 0][e] = 0.f;
-    }
+  for (int e = 0; e < NA; ++e) {
+    acc[e] = 0.f;
+    if (SPLIT) acl[SPLIT ? e : 0] = 0.f;
+  }
+  float* corr = SPLIT ? acl : acc;
   int prev_stg = -1;
   for (int c = 0; c < n_chunks; ++c) {
-    const int stg = ring ? gchunk % NB : c;
-    mbar_wait(&bars[bar0 + stg], ring ? (uint32_t)((gchunk / NB) & 1) : 0u);
+    const int stg = ring ? (int)((uint32_t)gchunk % (uint32_t)NB) : c;
+    mbar_wait(&bars[bar0 + stg], ring ? ((uint32_t)gchunk / (uint32_t)NB) & 1u : 0u);
     const uint32_t sbase = b_addr0 + (uint32_t)stg * stage_bytes;
     uint32_t ah0, al0, bbase;
     if (a_in_stage) {
@@ -135,21 +139,16 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
       bbase = sbase;
     }
     ah0 += a_row; al0 += a_row;
-    const uint32_t bh0 = wg_desc_lo(bbase, b_plane) + (uint32_t)gh * 16u;  // 16 columns = 256 B
-    const uint32_t bl0 = wg_desc_lo(bbase + b_chunk_bytes, b_plane) + (uint32_t)gh * 16u;
+    const uint32_t bh0 = wg_desc_lo(bbase, b_plane) + (uint32_t)(gh * 16 * NGW);  // 16 NGW columns x 16 B
+    const uint32_t bl0 = wg_desc_lo(bbase + b_chunk_bytes, b_plane) + (uint32_t)(gh * 16 * NGW);
     wgmma_fence();
 #pragma unroll 1
     for (int t = 0; t < IAF_NTAPS; ++t) {
       const uint64_t ah = mk_desc(ah0 + sh[t]), al = mk_desc(al0 + sh[t]);
       const uint32_t bt = (uint32_t)t * b_tstep;
-#pragma unroll
-      for (int k = 0; k < NGW; ++k) {
-        const uint32_t go = bt + (uint32_t)k * 32u;  // every second group: 32 columns = 512 B
-        float* corr = SPLIT ? acl[SPLIT ? k : 0] : acc[k];
-        wgmma_m64n16k16<0>(corr, al, mk_desc(bh0 + go));
-        wgmma_m64n16k16<0>(corr, ah, mk_desc(bl0 + go));
-        wgmma_m64n16k16<0>(acc[k], ah, mk_desc(bh0 + go));
-      }
+      wgmma_m64nNk16<NGW>(corr, al, mk_desc(bh0 + bt));
+      wgmma_m64nNk16<NGW>(corr, ah, mk_desc(bl0 + bt));
+      wgmma_m64nNk16<NGW>(acc, ah, mk_desc(bh0 + bt));
     }
     wgmma_commit();
     // keep this K-step's group in flight; the previous one has completed, so its ring stage can be refilled
@@ -162,24 +161,19 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
   if (ring && prev_stg >= 0 && wl == 0 && lane == 0) mbar_arrive(&bars[LB_BEMPTY + prev_stg]);
   if (SPLIT) {
 #pragma unroll
-    for (int k = 0; k < NGW; ++k)
-#pragma unroll
-      for (int e = 0; e < 8; ++e) acc[k][e] += acl[SPLIT ? k : 0][e];
+    for (int e = 0; e < NA; ++e) acc[e] += acl[SPLIT ? e : 0];
   }
-  // fragment -> accumulator tile: acc[k][4j + 2h + e] = row 16 wl + lane / 4 + 8h, column 16 g + 8j + 2 (lane % 4) + e
+  // fragment -> accumulator tile: acc[4j + 2h + e] = row 16 wl + lane / 4 + 8h, column 16 NGW gh + 8j + 2 (lane % 4) + e
   const int pitch = ly_acc_pitch(N);
   const int r0 = rh * 64 + wl * 16 + (lane >> 2);
 #pragma unroll
-  for (int k = 0; k < NGW; ++k) {
-    const int g = gh + 2 * k;
-    if (16 * g < N) {
-      const int col = g * 16 + 2 * (lane & 3);
+  for (int j = 0; j < 2 * NGW; ++j) {
+    const int c8 = 16 * NGW * gh + 8 * j;
+    if (c8 < N) {
+      const int col = c8 + 2 * (lane & 3);
 #pragma unroll
-      for (int j = 0; j < 2; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          *reinterpret_cast<float2*>(s_acc + (r0 + 8 * h) * pitch + col + 8 * j) =
-              make_float2(acc[k][4 * j + 2 * h], acc[k][4 * j + 2 * h + 1]);
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(s_acc + (r0 + 8 * h) * pitch + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
     }
   }
 }
@@ -200,7 +194,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   const int a_plane = p.WIN * 16;          // bytes per chunk plane of the A window
   const int a_lo_off = nchunk * a_plane;
   // tiles of this CTA: u = blockIdx.x + i * gridDim.x
-  const int n_my = (p.NT - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int n_my = (int)((uint32_t)(p.NT - (int)blockIdx.x + (int)gridDim.x - 1) / gridDim.x);
   const bool resident = FUSED || q.n_bchunks <= q.NB;
 
   // programmatic dependent launch: everything up to the barrier init overlaps the previous grid
@@ -259,7 +253,11 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
           if (resident && i >= 1 && !q.in_mode) continue;  // weights already resident, A comes from the workers
           const int stg = gchunk % q.NB;
           const int use = gchunk / q.NB;
-          if (use >= 1) mbar_wait(&bars[LB_BEMPTY + stg], (uint32_t)((use - 1) & 1));
+          if (use >= 1) {
+            TL(2, 60, gchunk);
+            mbar_wait(&bars[LB_BEMPTY + stg], (uint32_t)((use - 1) & 1));
+            TL(2, 61, gchunk);
+          }
           uint8_t* dst = smem + q.sm_b + stg * q.stage_bytes;
           const size_t bo = (size_t)c * q.b_chunk_bytes;
           if (q.in_mode) {
@@ -336,22 +334,22 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       fence_proxy_async();  // generic-proxy stores -> the wgmma (async proxy) reads of the window
     };
 
-    int gchunk = 0;
     for (int i = 0; i < n_my; ++i) {
       const int u = (int)blockIdx.x + i * (int)gridDim.x;
       // the previous tile's epilogue is done with the accumulator tile and its MMAs with the A window
       worker_bar_sync();
+      if (warp == 0 && lane == 0) TL(1, 0, i);
       if (!q.in_mode) {
         load_window(i);
         worker_bar_sync();
+        if (warp == 0 && lane == 0) TL(1, 10, i);
       }
-      if (warp == 0 && lane == 0) TL(1, 10, i);
-      ly_mma_tile<NGW>(smem, bars, s_acc, St0.N, q.n_bchunks, !resident || q.in_mode, q.NB, gchunk, LB_BFULL,
+      ly_mma_tile<NGW>(smem, bars, s_acc, St0.N, q.n_bchunks, !resident || q.in_mode, q.NB, i * q.n_bchunks, LB_BFULL,
                        smem_u32(smem + q.sm_b), (uint32_t)(FUSED ? 2 * q.b_chunk_bytes : q.stage_bytes),
                        (uint32_t)q.b_chunk_bytes, q.in_mode != 0, smem_u32(smem + q.sm_a), (uint32_t)a_plane,
                        (uint32_t)a_lo_off, p.Wp);
       worker_bar_sync();
-      if (warp == 0 && lane == 0) TL(1, 50, i);
+      if (warp == 0 && lane == 0) TL(1, 20, i);
       const SlotInfo si_all = decode_slot(p, u * q.TS + sl, HW);
       const bool bx0 = (si_all.x == 0), bxW = (si_all.x == p.W - 1), byH = (si_all.y == p.H - 1);
 
@@ -571,12 +569,13 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
         hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
         fence_proxy_async();
         worker_bar_sync();
+        if (warp == 0 && lane == 0) TL(1, 30, i);
         const IafTcStage& St1 = p.st[1];
-        int g1 = 0;
-        ly_mma_tile<NGW>(smem, bars, s_acc, St1.N, q.n_bchunks1, false, 1, g1, LB_BFULL + q.n_bchunks,
+        ly_mma_tile<NGW>(smem, bars, s_acc, St1.N, q.n_bchunks1, false, 1, 0, LB_BFULL + q.n_bchunks,
                          smem_u32(smem + q.sm_b1), (uint32_t)(2 * q.b_chunk_bytes1), (uint32_t)q.b_chunk_bytes1, false,
                          smem_u32(smem + q.sm_h), (uint32_t)h_plane, (uint32_t)((St1.cin >> 3) * h_plane), p.Wp);
         worker_bar_sync();
+        if (warp == 0 && lane == 0) TL(1, 40, i);
         SlotInfo si_out = si_all;
         si_out.valid = si_all.valid && sl < q.TO;
         heads_epi(St1, reinterpret_cast<const float*>(smem + q.sm_bias1), St1.N >> 4, ly_acc_pitch(St1.N), si_out);
@@ -643,5 +642,9 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   }
 
   __syncthreads();
-  if (q.tl_enable) { TL_FLUSH }
+  if (q.tl_enable) {
+    if (tid == 0) TL(1, 99, n_my);
+    __syncwarp();
+    TL_FLUSH
+  }
 }
