@@ -145,6 +145,44 @@ def test_nl2_training_gradients_over_the_emulated_abi(monkeypatch):
 
 
 @pytest.mark.gpu
+def test_nl2_training_gradients_on_the_tensor_cores():
+    """d(cost)/d(every parameter) through CudaIAFTrain on the GPU, at a shape where both convs of every layer run the
+    tensor-core forward and backward (the second one flipped), against fp64 autograd through the oracle block."""
+    hps = dict(HPS, n_z=16, n_h1=32, n_h2=32, depths=[1, 1], depth_ar=1, image_size=16)
+    w32, x, n32 = _setup(hps, 2, 7, torch.float32, "cuda")
+    w64, _, n64 = _setup(hps, 2, 7, torch.float64, "cpu")
+    for w in (w32, w64):
+        for v in w.values():
+            v.requires_grad_(True)
+    iaf = ET.CudaIAFTrain(w32, hps)
+    got = ET.forward(w32, x, n32, iaf, hps)
+    got["cost"].sum().backward()
+    assert sorted(iaf.ops) == [("0_0", 1), ("0_0", 2), ("1_0", 1), ("1_0", 2)]
+    for (name, conv), op in iaf.ops.items():
+        s = hps["image_size"] // 2 ** (int(name[0]) + 1)
+        assert op.flipmask == (conv == 2), (name, conv)
+        assert op.path_used(s, s, "cuda:0", "step") == "tc", (name, conv)
+        assert op.backward_path(s, s, "cuda:0") == "tc", (name, conv)
+    ref = ET.forward(w64, x.cpu(), n64, TorchIAFTheanoNL2(w64, hps), hps)
+    np.testing.assert_allclose(got["cost"].detach().cpu().numpy(), ref["cost"].detach().numpy(), rtol=2e-5)
+    ref["cost"].sum().backward()
+    checked = 0
+    for k in w64:
+        g, r = w32[k].grad, w64[k].grad
+        if r is None:
+            assert g is None, k
+            continue
+        g = g.cpu()
+        err = float((g.double() - r).abs().max()) / max(float(r.abs().max()), 1e-12)
+        assert err < 5e-4, (k, err)   # fp32 torch plumbing around the operator
+        if "_posterior_conv2_" in k and k.endswith("_w"):
+            mask = conv_ar_mask(g.shape[1] - 1, g.shape[0], "_out_" in k, True)
+            assert bool((g.numpy()[mask == 0] == 0).all()), k   # masked taps: exactly zero (ar.py:369-373)
+            checked += 1
+    assert checked == 3 * len(hps["depths"])
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("name", ["0_1", "1_0"])
 def test_nl2_layer_on_the_gpu(name):
     got, ref = _layer(name, ET.CudaIAF, torch.float32, "cuda")
