@@ -32,15 +32,13 @@
 
 #include "iaf_tc.h"
 
-#define TC_WORKERS 16  // worker warps of the stage kernel (four warpgroups)
-#define TC_WTHREADS (TC_WORKERS * 32)
 #define TC_TILE 128
 #ifdef IAF_TC_TIMELINE
 #define TC_SMEM_LIMIT (227 * 1024 - 512 - 9472)  // room for the static event buffers (4 x TL_MAX x 24 B + counts)
 #else
 #define TC_SMEM_LIMIT (227 * 1024 - 512)  // opt-in maximum minus the kernels' static shared memory (barriers: < 512 B)
 #endif
-#define TC_ZITEMS 2  // z-window (slot, chunk) items per worker thread
+#define TC_ZITEMS 4  // z-window (slot, chunk) items per epilogue thread of the stage kernel
 
 struct IafTcStage {
   const __nv_bfloat16* whi;  // global packed [K/8][N][8]
@@ -104,7 +102,6 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ void worker_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(TC_WTHREADS) : "memory"); }
 // Hopper warpgroup MMA (wgmma), all four warps of a warpgroup converged.  D[64 x 16] += A[64 x 16] * B[16 x 16]: fp16
 // operands from shared-memory descriptors (both K-major, or both MN-major with MN = 1), fp32 accumulators in registers.
 // Fragment of a thread (warp w of the warpgroup): d[4j + 2h + e] = row 16 w + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e.
@@ -118,19 +115,11 @@ __device__ __forceinline__ void wgmma_m64n16k16(float* d, uint64_t a_desc, uint6
       : "l"(a_desc), "l"(b_desc), "r"(1), "n"(MN)
       : "memory");
 }
-// The same, N = 16 NGW columns in one instruction (K-major operands): the A tile is fetched once for all N columns
-// instead of once per 16.  Fragment: d[4j + 2h + e] = row 16 w + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e, j < 2 NGW.
-template <int NGW>
+// The same, N = 16 G columns in one instruction (K-major operands): the A tile is fetched once for all N columns
+// instead of once per 16.  Fragment: d[4j + 2h + e] = row 16 w + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e, j < 2 G.
+// The stage kernel issues G = 2, 4, 5, 6, 8 (see ly_mma_tile).
+template <int G>
 __device__ __forceinline__ void wgmma_m64nNk16(float* d, uint64_t a_desc, uint64_t b_desc);
-template <>
-__device__ __forceinline__ void wgmma_m64nNk16<1>(float* d, uint64_t a_desc, uint64_t b_desc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a_desc), "l"(b_desc), "r"(1)
-      : "memory");
-}
 template <>
 __device__ __forceinline__ void wgmma_m64nNk16<2>(float* d, uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
@@ -138,17 +127,6 @@ __device__ __forceinline__ void wgmma_m64nNk16<2>(float* d, uint64_t a_desc, uin
       "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a_desc), "l"(b_desc), "r"(1)
-      : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_m64nNk16<3>(float* d, uint64_t a_desc, uint64_t b_desc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
       : "l"(a_desc), "l"(b_desc), "r"(1)
       : "memory");
 }
@@ -188,6 +166,22 @@ __device__ __forceinline__ void wgmma_m64nNk16<6>(float* d, uint64_t a_desc, uin
         "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
         "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
         "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(a_desc), "l"(b_desc), "r"(1)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<8>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(a_desc), "l"(b_desc), "r"(1)
       : "memory");
 }
@@ -260,10 +254,12 @@ __device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, ui
 }
 
 // Optional in-kernel timeline (compile with -DIAF_TC_TIMELINE; development aid only, tools/tl_run.py): CTA 0 of the
-// launch that sets tl_enable records (tag, tile or chunk, clock) triples per role.  Role 1, lane 0 of worker warp 0, after
-// the worker barrier that closes each phase: 0 tile start (the previous tile's last epilogue done), 10 z window built,
-// 20 (hidden) MMAs done, 30 (hidden) epilogue done, 40 heads MMAs done (fused), 99 kernel end.  Role 2, the producer:
-// 60 / 61 before / after waiting for a ring stage to be released (k = the weight chunk it will refill).
+// launch that sets tl_enable records (tag, tile or chunk, clock) triples per role, each at the end of a phase of its own
+// warp (other warps of the role may still be in it).  Role 0, lane 0 of MMA warp 0: 15 / 35 the (hidden) / heads MMAs'
+// operands ready, 20 / 40 their MMAs done, 21 / 41 their fragments in the accumulator tile (after waiting for the
+// epilogues to free it).  Role 1, lane 0 of epilogue warp 0: 10 z window built, 25 / 45 (hidden) / heads accumulators
+// ready, 30 (hidden) epilogue done, 50 heads epilogue done (fused), 99 kernel end.  Role 2, the producer: 60 / 61 before
+// / after waiting for a ring stage to be released (k = the weight chunk it will refill).
 #ifdef IAF_TC_TIMELINE
 #define TL_MAX 96
 __device__ long long g_tl[4][TL_MAX][3];
@@ -440,7 +436,7 @@ static LyKernel ly_kernel_pick(bool padw, int mode, bool elu) {
   LY_PICK(IAF_MODE_LAYER)
 #undef LY_PICK
 }
-// the stage kernel for a stage of N output columns: NGW = ceil(N / 32) 16-column groups per warpgroup.  NGW <= 6 (N <=
+// the stage kernel for a stage of N output columns: NGW = ceil(N / 32), an MMA warpgroup's span of 32 NGW columns.  NGW <= 6 (N <=
 // 192): wider stages never fit, their accumulator tile [128][N + 4] leaves no room for two ring stages (ly_layout and
 // iaf_dg_plan_create reject them before asking for a kernel)
 #define LY_MAX_NGW 6
@@ -454,7 +450,7 @@ static LyKernel ly_kernel_for(bool padw, int mode, bool elu, int N) {
     default: return ly_kernel_pick<LY_MAX_NGW, false>(padw, mode, elu);
   }
 }
-// the one-launch step of a one-hidden-layer stack (hidden and 2 n_z at most 64 columns: two groups per warpgroup)
+// the one-launch step of a one-hidden-layer stack (hidden and 2 n_z at most 64 columns: one m64n64 span)
 #define FZ_NGW 2
 static LyKernel fz_kernel_for(bool padw, int mode, bool elu) { return ly_kernel_pick<FZ_NGW, true>(padw, mode, elu); }
 
@@ -476,7 +472,7 @@ static bool ly_layout(const iaf_desc_t* d, IafTcPlan* pl) {
   q->n_stages = nst;
   q->MIR = MIR; q->WIN = TC_TILE + MIR;
   q->MAXS = (TC_TILE - 1) / SPS + 2;
-  if ((d->n_z / 8) * q->WIN > TC_ZITEMS * LY_WTHREADS) return false;
+  if ((d->n_z / 8) * q->WIN > TC_ZITEMS * LY_ETHREADS) return false;
   int prev = d->n_z;
   q->layer_ok = true;
   for (int j = 0; j < nst; ++j) {
@@ -490,7 +486,7 @@ static bool ly_layout(const iaf_desc_t* d, IafTcPlan* pl) {
     q->ly_sm_bias[j] = off; off += 5 * q->N[j] * 4;
     off = tc_round_up(off, 16);
     q->ly_sm_part[j] = off;
-    off += std::max(2 * LY_WORKERS * q->MAXS * 4, 2 * 4 * q->MAXS * d->n_z * 4);
+    off += std::max(2 * LY_PART_SETS * q->MAXS * 4, 2 * 4 * q->MAXS * d->n_z * 4);
     off = tc_round_up(off, 16);
     q->ly_sm_acc[j] = off; off += TC_TILE * ly_acc_pitch(q->N[j]) * 4;
     off = tc_round_up(off, 128);
@@ -518,7 +514,7 @@ static bool fz_layout(const iaf_desc_t* d, IafTcPlan* q) {
   q->fz_sm_h = off; off += 2 * (q->N[0] / 8) * (TC_TILE + q->MIR) * 16;
   for (int j = 0; j < 2; ++j) { q->fz_sm_bias[j] = off; off += 5 * q->N[j] * 4; }
   off = tc_round_up(off, 16);
-  q->fz_sm_part = off; off += std::max(2 * LY_WORKERS * q->MAXS * 4, 2 * 4 * q->MAXS * d->n_z * 4);
+  q->fz_sm_part = off; off += std::max(2 * LY_PART_SETS * q->MAXS * 4, 2 * 4 * q->MAXS * d->n_z * 4);
   off = tc_round_up(off, 16);
   q->fz_sm_acc = off; off += TC_TILE * ly_acc_pitch(std::max(q->N[0], q->N[1])) * 4;
   off = tc_round_up(off, 128);
@@ -964,7 +960,7 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
     int off = 0;
     pl->sm_bias[j] = off; off += 5 * N * 4;
     off = tc_round_up(off, 16);
-    pl->sm_part[j] = off; off += 2 * LY_WORKERS * pl->MAXS * 4;
+    pl->sm_part[j] = off; off += 2 * LY_PART_SETS * pl->MAXS * 4;
     off = tc_round_up(off, 16);
     pl->sm_acc[j] = off; off += TC_TILE * ly_acc_pitch(N) * 4;
     off = tc_round_up(off, 128);

@@ -6,32 +6,54 @@
 //     [channel chunk][slot][8] (hi and lo), so that a tile's A chunk pair is a few contiguous runs that the producer warp
 //     fetches with 1-D bulk copies;
 //   * the weights are NOT resident (unless they fit the ring): the producer warp streams them in chunks of LY_KC
-//     K-steps through an NB-deep shared-memory ring (cp.async.bulk + expect_tx on an mbarrier); every worker warpgroup
-//     releases a ring stage once its wgmma reads of it have completed;
-//   * the 16 worker warps are four warpgroups: warpgroup w issues one wgmma m64nNk16 per K-step, tap and product for
-//     rows [64 (w & 1), +64) of the tile and one contiguous half of its columns (w >> 1), accumulating in registers.
-//     The accumulators then go through a shared-memory tile [128][N + 4] so that the epilogue keeps one thread per slot
-//     (coalesced global traffic along pixels);
+//     K-steps through an NB-deep shared-memory ring (cp.async.bulk + expect_tx on an mbarrier); both MMA warpgroups
+//     release a ring stage once their wgmma reads of it have completed;
+//   * five warpgroups with their own jobs: warpgroups 0 and 1 issue the MMAs, warpgroup r for rows [64 r, +64) of the
+//     tile and ALL of the stage's columns (one wgmma m64nNk16 per K-step, tap and product; two of half the width for
+//     stages of 129-160 columns; two passes over K for 161-192), accumulating in registers; warpgroups 2 and 3 build the first stage's z window and
+//     run the epilogues; in warpgroup 4, warp 16 is the producer and warp 17 the reducer.  setmaxnreg moves registers
+//     from warpgroup 4 to the MMA warpgroups;
+//   * the accumulators go through a shared-memory tile [128][N + 4] so that the epilogue keeps one thread per slot
+//     (coalesced global traffic along pixels).  The tile, the z window and the fused kernel's hidden operand buffer
+//     are handed between the MMA and epilogue warpgroups through full / empty mbarrier pairs, so an epilogue runs
+//     while the MMAs of the next tile (or stage) are in flight: the MMA warpgroups' registers are the second buffer;
 //   * hidden stages write their output operand image back to global memory (16-byte stores), the heads stage applies
 //     the affine update; per-sample sums go through the reducer warp in fixed order.
 #pragma once
 
-#define LY_WORKERS 16
-#define LY_WTHREADS (LY_WORKERS * 32)
-#define LY_TMA_WARP LY_WORKERS
-#define LY_RED_WARP (LY_WORKERS + 1)
-#define LY_THREADS (LY_WTHREADS + 64)
+#define LY_MMA_WARPS 8                   // warpgroups 0, 1: the MMAs
+#define LY_EPI_WARP0 8                   // warpgroups 2, 3: z window and epilogues
+#define LY_EPI_WARPS 8
+#define LY_ETHREADS (LY_EPI_WARPS * 32)
+#define LY_TMA_WARP 16                   // warpgroup 4: the producer, the reducer and two idle warps
+#define LY_RED_WARP 17
+#define LY_THREADS 640
+// registers per thread after setmaxnreg.  The launch gives each of the 640 threads 96 (61,440 in all); warpgroup 4
+// returns 48 of them and the MMA warpgroups take 24 more, for up to 80 accumulators (64 x 160 fp32 over 128 threads, or
+// 2 x 64 x 64 when the correction products are summed apart) beside their descriptors and counters.  The epilogue
+// warpgroups keep 96.  ptxas compiles the code after setmaxnreg.inc to the raised count, but each single wgmma must
+// still fit the launch's 96: hence two instructions of half the width for 160 columns (ly_mma_tile).  96 accumulators
+// (a 192-column span) do not fit in 120: stages of 161-192 columns run two passes over K of 96 columns each.
+#define LY_REGS_AUX 48
+#define LY_REGS_MMA 120
+// per-sample partials of one tile (step and multiconv modes): one per (set of column groups g with the same g % 4,
+// quarter of the tile's slots), summed by the reducer warp in that fixed order
+#define LY_PART_SETS 16
 #define LY_KC 5        // K-steps (of 16) per weight chunk
 #define LY_MAX_NB 6
-// Bytes every layout of the stage kernel reserves past its last weight image: the column span of the second half (see
-// ly_mma_tile) of the last K plane reads up to 16 * (32 * NGW - N) bytes past the plane's end -- 256 for the per-stage
-// instantiations (NGW = ceil(N / 32)), 768 for the fused one (NGW = 2, N down to 16: hidden [16]) -- and that read must
-// stay inside the CTA's allocation.
+// Bytes every layout of the stage kernel reserves past its last weight image: the column span of an MMA warpgroup (see
+// ly_mma_tile), 32 NGW columns, of the last K plane reads up to 16 * (32 * NGW - N) bytes past the plane's end -- 256 for
+// the per-stage instantiations (NGW = ceil(N / 32)), 768 for the fused one (NGW = 2, N down to 16: hidden [16]) -- and
+// that read must stay inside the CTA's allocation.  (The previous layout's second column half ended at the same byte.)
 #define LY_B_SLACK 1024
 
 enum { LB_BFULL = 0, LB_BEMPTY = LY_MAX_NB, LB_PART = 2 * LY_MAX_NB,
        LB_PART_EMPTY = 2 + 2 * LY_MAX_NB,  // + tile parity: the reducer warp has consumed the partials
-       LB_COUNT = 4 + 2 * LY_MAX_NB };
+       // MMA <-> epilogue handoffs, one phase per use (parity = use & 1): the accumulator tile (written by the MMA warps,
+       // read by the epilogue warps), the z window (written by the epilogue warps, read by the MMA warpgroups) and the
+       // fused kernel's hidden operand buffer (likewise)
+       LB_ACC_FULL = 4 + 2 * LY_MAX_NB, LB_ACC_EMPTY, LB_WIN_FULL, LB_WIN_EMPTY, LB_H_FULL, LB_H_EMPTY,
+       LB_COUNT };
 
 struct IafLyParams {
   IafTcParams t;               // geometry, pointers, slot decoding (t.st[0] describes THIS stage)
@@ -85,28 +107,35 @@ __device__ __forceinline__ float dg_scale_from_amax(float amax) {
   return __uint_as_float((uint32_t)(127 + 5 - e) << 23);
 }
 
-// The MMAs of one stage for one tile.  Warpgroup w (of the four worker warpgroups) computes rows [64 (w & 1), +64) and
-// the 16 NGW contiguous columns from 16 NGW (w >> 1): D[64 x 16 NGW] += A_t[64 x 16] B_t[16 x 16 NGW] over K-steps, taps
-// and the three split products, one wgmma each, accumulating in registers, then writes its fragments into the
-// accumulator tile.  In the B image [K/8][N][8] a span of contiguous columns is one K-major descriptor (8-column groups
-// 128 B apart, the two K halves one plane apart).  NGW is a compile-time count: a span past the stage's columns computes
-// on whatever follows in shared memory -- the next K plane, the next image, or the LY_B_SLACK bytes every layout
-// reserves past its last one -- and is not stored, so every wgmma is issued unconditionally and ptxas keeps them
-// asynchronous.
+// The MMAs of one stage (or one pass over it) for one tile, run by the two MMA warpgroups.  Warpgroup r computes rows
+// [64 r, +64) and the 16 SPG columns from col0: D[64 x 16 SPG] += A_t[64 x 16] B_t[16 x 16 SPG] over K-steps, taps and
+// the three split products, accumulating in registers (acc; returned with the correction sum added).  Each product is
+// one wgmma over the span (NI = 1), or for 160 columns two of half the span (NI = 2): an m64n160 instruction needs more
+// registers than the launch's 96 by itself, although all 80 accumulators fit after setmaxnreg.  The halves' fragments sit
+// side by side in acc exactly as one instruction's would.  In the B image [K/8][N][8] a span of contiguous columns is one
+// K-major descriptor (8-column groups 128 B apart, the two K halves one plane apart).  NGW is a compile-time count: a span
+// past the stage's columns computes on whatever follows in shared memory -- the next K plane, the next image, or the
+// LY_B_SLACK bytes every layout reserves past its last one -- and is not stored, so every wgmma is issued
+// unconditionally and ptxas keeps them asynchronous.
 //   ring: the tile's weight chunks are the CTA's gchunk, gchunk + 1, ... (every tile streams all n_chunks); chunk g sits
 //   in ring stage g % NB (parity from g / NB), released after its MMAs complete;
 //   otherwise resident: chunk c sits in stage c behind barrier bar0 + c (parity 0).
-//   a_in_stage: the A chunk pair of K-step c rides in the ring stage before the weights; otherwise A is a window at a_addr.
-// The tile holds the products with the weight images as packed: the per-column weight scale is undone by the epilogues
-// as they read it (acc_ld16).
-template <int NGW>
-__device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float* s_acc, int N, int n_chunks, bool ring, int NB,
+//   a_in_stage: the A chunk pair of K-step c rides in the ring stage before the weights; otherwise A is a window at a_addr,
+//   and barrier a_release (if >= 0) is arrived on once the MMAs have read it.
+// the two MMA warpgroups converge here before a stage's MMAs: without a barrier between the per-thread mbarrier waits
+// and the accumulator set-up, ptxas treats the wgmma sequence as divergent code and serializes every wgmma
+__device__ __forceinline__ void mma_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(LY_MMA_WARPS * 32) : "memory"); }
+
+template <int SPG, bool SPLIT>
+__device__ __forceinline__ void ly_mma_tile(float* acc, uint64_t* bars, int N, int col0, int n_chunks, bool ring, int NB,
                                             int gchunk, int bar0, uint32_t b_addr0, uint32_t stage_bytes,
                                             uint32_t b_chunk_bytes, bool a_in_stage, uint32_t a_addr, uint32_t a_plane,
-                                            uint32_t a_lo_off, int Wp) {
-  constexpr int NA = 8 * NGW;  // accumulators per thread: 64 x 16 NGW over the 128 threads of the warpgroup
+                                            uint32_t a_lo_off, int Wp, int a_release) {
+  constexpr int NA = 8 * SPG;          // accumulators per thread: 64 x 16 SPG over the 128 threads of the warpgroup
+  constexpr int NI = SPG > 8 ? 2 : 1;  // wgmma instructions per product
+  constexpr int GI = SPG / NI;         // 16-column groups per instruction
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int wg = warp >> 2, rh = wg & 1, gh = wg >> 1, wl = warp & 3;
+  const int rh = warp >> 2, wl = warp & 3;
   const uint32_t b_plane = (uint32_t)N * 16u;
   const uint32_t sh[IAF_NTAPS] = {0u, 1u, (uint32_t)(Wp - 1), (uint32_t)Wp, (uint32_t)(Wp + 1)};  // 16-byte units
   const uint32_t a_kstep = (2u * a_plane) >> 4, b_tstep = (2u * b_plane) >> 4;
@@ -114,9 +143,9 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
   // The two correction products (lo x hi, hi x lo: 2^-11 of hi x hi) go to their own accumulators where registers allow:
   // added one by one to the main sum, each is rounded at the main sum's magnitude by the tensor cores' accumulation, and
   // over K = 160 those roundings reach ~2e-7 of a unit pre-activation -- enough to put a ReLU's derivative on the wrong
-  // side of a pre-activation that small.  Summed apart and added once at the end, they cost one rounding.
-  constexpr bool SPLIT = NGW <= 2;
-  float acc[NA], acl[SPLIT ? NA : 1];
+  // side of a pre-activation that small.  Summed apart and added once at the end, they cost one rounding.  Stages of at
+  // most 64 columns do so.
+  float acl[SPLIT ? NA : 1];
 #pragma unroll
   for (int e = 0; e < NA; ++e) {
     acc[e] = 0.f;
@@ -139,16 +168,20 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
       bbase = sbase;
     }
     ah0 += a_row; al0 += a_row;
-    const uint32_t bh0 = wg_desc_lo(bbase, b_plane) + (uint32_t)(gh * 16 * NGW);  // 16 NGW columns x 16 B
-    const uint32_t bl0 = wg_desc_lo(bbase + b_chunk_bytes, b_plane) + (uint32_t)(gh * 16 * NGW);
+    const uint32_t bh0 = wg_desc_lo(bbase, b_plane) + (uint32_t)col0;  // 16 B per column
+    const uint32_t bl0 = wg_desc_lo(bbase + b_chunk_bytes, b_plane) + (uint32_t)col0;
     wgmma_fence();
 #pragma unroll 1
     for (int t = 0; t < IAF_NTAPS; ++t) {
       const uint64_t ah = mk_desc(ah0 + sh[t]), al = mk_desc(al0 + sh[t]);
       const uint32_t bt = (uint32_t)t * b_tstep;
-      wgmma_m64nNk16<NGW>(corr, al, mk_desc(bh0 + bt));
-      wgmma_m64nNk16<NGW>(corr, ah, mk_desc(bl0 + bt));
-      wgmma_m64nNk16<NGW>(acc, ah, mk_desc(bh0 + bt));
+#pragma unroll
+      for (int h = 0; h < NI; ++h) {  // instruction h: columns [16 GI h, +16 GI), 16 B per column in the descriptor
+        const uint32_t bc = bt + (uint32_t)(16 * GI * h);
+        wgmma_m64nNk16<GI>(corr + 8 * GI * h, al, mk_desc(bh0 + bc));
+        wgmma_m64nNk16<GI>(corr + 8 * GI * h, ah, mk_desc(bl0 + bc));
+        wgmma_m64nNk16<GI>(acc + 8 * GI * h, ah, mk_desc(bh0 + bc));
+      }
     }
     wgmma_commit();
     // keep this K-step's group in flight; the previous one has completed, so its ring stage can be refilled
@@ -158,17 +191,29 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
     if (ring) ++gchunk;
   }
   wgmma_wait<0>();
-  if (ring && prev_stg >= 0 && wl == 0 && lane == 0) mbar_arrive(&bars[LB_BEMPTY + prev_stg]);
+  if (wl == 0 && lane == 0) {
+    if (ring && prev_stg >= 0) mbar_arrive(&bars[LB_BEMPTY + prev_stg]);
+    if (a_release >= 0) mbar_arrive(&bars[a_release]);
+  }
   if (SPLIT) {
 #pragma unroll
     for (int e = 0; e < NA; ++e) acc[e] += acl[SPLIT ? e : 0];
   }
-  // fragment -> accumulator tile: acc[4j + 2h + e] = row 16 wl + lane / 4 + 8h, column 16 NGW gh + 8j + 2 (lane % 4) + e
+}
+
+// The MMA warpgroups' fragments -> columns [col0, +16 SPG) of the accumulator tile, for its k-th use in this launch: the
+// first pass waits until the epilogue warps have read use k - 1, the last hands use k over.  acc[4j + 2h + e] = row
+// 64 r + 16 wl + lane / 4 + 8h, column col0 + 8j + 2 (lane % 4) + e.
+template <int SPG>
+__device__ __forceinline__ void ly_acc_store(const float* acc, uint64_t* bars, float* s_acc, int N, int col0, int k,
+                                             bool first, bool last) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (first && k >= 1) mbar_wait(&bars[LB_ACC_EMPTY], (uint32_t)((k - 1) & 1));
   const int pitch = ly_acc_pitch(N);
-  const int r0 = rh * 64 + wl * 16 + (lane >> 2);
+  const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-  for (int j = 0; j < 2 * NGW; ++j) {
-    const int c8 = 16 * NGW * gh + 8 * j;
+  for (int j = 0; j < 2 * SPG; ++j) {
+    const int c8 = col0 + 8 * j;
     if (c8 < N) {
       const int col = c8 + 2 * (lane & 3);
 #pragma unroll
@@ -176,9 +221,12 @@ __device__ __forceinline__ void ly_mma_tile(uint8_t* smem, uint64_t* bars, float
         *reinterpret_cast<float2*>(s_acc + (r0 + 8 * h) * pitch + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
     }
   }
+  if (!last) return;
+  __syncwarp();
+  if (lane == 0) mbar_arrive(&bars[LB_ACC_FULL]);
 }
 
-// NGW: 16-column groups per warpgroup of the stage, ceil(N / 32).  FUSED: the whole step of a one-hidden-layer stack in one
+// NGW: ceil(N / 32); an MMA warpgroup covers the stage's columns as 2 NGW groups of 16.  FUSED: the whole step of a one-hidden-layer stack in one
 // launch (NGW covers both stages), tiles of TS = TC_TILE - MIR output slots whose 128 hidden rows overlap the next tile's.
 template <bool PADW, int MODE, int NLT, int NGW, bool FUSED>
 __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_constant__ IafLyParams q) {
@@ -196,27 +244,41 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   // tiles of this CTA: u = blockIdx.x + i * gridDim.x
   const int n_my = (int)((uint32_t)(p.NT - (int)blockIdx.x + (int)gridDim.x - 1) / gridDim.x);
   const bool resident = FUSED || q.n_bchunks <= q.NB;
+  const bool ring = !resident || q.in_mode;
+  // an MMA warpgroup's span: all 32 NGW columns, or for NGW = 6 two passes over K of 96 columns each (the ring streams
+  // the tile's chunks once per pass)
+  constexpr int NP = NGW > 5 ? 2 : 1;
+  constexpr int SPG = 2 * NGW / NP;
+  constexpr bool SPLIT = NGW <= 2;
 
   // programmatic dependent launch: everything up to the barrier init overlaps the previous grid
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  const bool epi = warp >= LY_EPI_WARP0 && warp < LY_EPI_WARP0 + LY_EPI_WARPS;
+  const int et = tid - LY_EPI_WARP0 * 32, ew = warp - LY_EPI_WARP0;  // epilogue thread / warp index
   if (warp == LY_TMA_WARP) {
     if (lane == 0) {
       for (int i = 0; i < 2; ++i) {
-        mbar_init(&bars[LB_PART + i], LY_WORKERS);
+        mbar_init(&bars[LB_PART + i], LY_EPI_WARPS);
         mbar_init(&bars[LB_PART_EMPTY + i], 1);
       }
       for (int i = 0; i < LY_MAX_NB; ++i) {
         mbar_init(&bars[LB_BFULL + i], 1);
-        mbar_init(&bars[LB_BEMPTY + i], LY_WORKERS / 4);  // every worker warpgroup releases the stage
+        mbar_init(&bars[LB_BEMPTY + i], 2);  // both MMA warpgroups release the stage
       }
+      mbar_init(&bars[LB_ACC_FULL], LY_MMA_WARPS);
+      mbar_init(&bars[LB_ACC_EMPTY], LY_EPI_WARPS);
+      mbar_init(&bars[LB_WIN_FULL], LY_EPI_WARPS);
+      mbar_init(&bars[LB_WIN_EMPTY], 2);
+      mbar_init(&bars[LB_H_FULL], LY_EPI_WARPS);
+      mbar_init(&bars[LB_H_EMPTY], 2);
       fence_barrier_init();
     }
-  } else if (warp < LY_WORKERS) {
+  } else if (epi) {
     asm volatile("griddepcontrol.wait;" ::: "memory");
     for (int s = 0; s < (FUSED ? 2 : 1); ++s) {
       const IafTcStage& S = p.st[s];
       float* tb = reinterpret_cast<float*>(smem + (s ? q.sm_bias1 : q.sm_bias));
-      for (int i = tid; i < 5 * S.N; i += LY_WTHREADS) {
+      for (int i = et; i < 5 * S.N; i += LY_ETHREADS) {
         float v = 0.f;
         if (i < S.N) v = __ldg(S.bias + i);
         else if (PADW) v = __ldg(S.padw + (i - S.N));
@@ -224,67 +286,162 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       }
     }
   }
-  if (warp >= LY_WORKERS) asm volatile("griddepcontrol.wait;" ::: "memory");  // producer / reducer warps
+  if (!epi) asm volatile("griddepcontrol.wait;" ::: "memory");
   __syncthreads();
 
-  if (warp == LY_TMA_WARP) {
-    // ===================== producer: A windows (operand-image input) and the weight ring =====================
-    if (lane == 0 && FUSED) {
-      // both stages' weights, resident: hidden chunk c behind barrier c, heads chunk c behind barrier n_bchunks + c
-      for (int s = 0; s < 2; ++s) {
-        const IafTcStage& S = p.st[s];
-        const int nb = s ? q.n_bchunks1 : q.n_bchunks, bcb = s ? q.b_chunk_bytes1 : q.b_chunk_bytes;
-        uint8_t* base = smem + (s ? q.sm_b1 : q.sm_b);
-        for (int c = 0; c < nb; ++c) {
-          uint64_t* bar = &bars[LB_BFULL + (s ? q.n_bchunks : 0) + c];
-          const size_t bo = (size_t)c * bcb;
-          mbar_expect_tx(bar, (uint32_t)(2 * bcb));
-          bulk_g2s(base + 2 * c * bcb, reinterpret_cast<const uint8_t*>(S.whi) + bo, (uint32_t)bcb, bar);
-          bulk_g2s(base + 2 * c * bcb + bcb, reinterpret_cast<const uint8_t*>(S.wlo) + bo, (uint32_t)bcb, bar);
+  if (warp >= LY_TMA_WARP) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(LY_REGS_AUX));
+    if (warp == LY_TMA_WARP) {
+      // ===================== producer: A windows (operand-image input) and the weight ring =====================
+      if (lane == 0 && FUSED) {
+        // both stages' weights, resident: hidden chunk c behind barrier c, heads chunk c behind barrier n_bchunks + c
+        for (int s = 0; s < 2; ++s) {
+          const IafTcStage& S = p.st[s];
+          const int nb = s ? q.n_bchunks1 : q.n_bchunks, bcb = s ? q.b_chunk_bytes1 : q.b_chunk_bytes;
+          uint8_t* base = smem + (s ? q.sm_b1 : q.sm_b);
+          for (int c = 0; c < nb; ++c) {
+            uint64_t* bar = &bars[LB_BFULL + (s ? q.n_bchunks : 0) + c];
+            const size_t bo = (size_t)c * bcb;
+            mbar_expect_tx(bar, (uint32_t)(2 * bcb));
+            bulk_g2s(base + 2 * c * bcb, reinterpret_cast<const uint8_t*>(S.whi) + bo, (uint32_t)bcb, bar);
+            bulk_g2s(base + 2 * c * bcb + bcb, reinterpret_cast<const uint8_t*>(S.wlo) + bo, (uint32_t)bcb, bar);
+          }
+        }
+      } else if (lane == 0) {
+        int gchunk = 0;
+        for (int i = 0; i < n_my; ++i) {
+          const int u = (int)blockIdx.x + i * (int)gridDim.x;
+          // K order is [K-step within a tap][tap]: weight chunk c and A chunk pair (2c, 2c+1) are consumed together,
+          // so both stream through shared memory at the pace of the MMAs
+          for (int cp = 0; cp < (ring ? NP : 1) * q.n_bchunks; ++cp) {
+            if (resident && i >= 1 && !q.in_mode) continue;  // weights already resident, A comes from the epilogue warps
+            const int c = cp % q.n_bchunks;
+            const int stg = gchunk % q.NB;
+            const int use = gchunk / q.NB;
+            if (use >= 1) {
+              TL(2, 60, gchunk);
+              mbar_wait(&bars[LB_BEMPTY + stg], (uint32_t)((use - 1) & 1));
+              TL(2, 61, gchunk);
+            }
+            uint8_t* dst = smem + q.sm_b + stg * q.stage_bytes;
+            const size_t bo = (size_t)c * q.b_chunk_bytes;
+            if (q.in_mode) {
+              // one ring stage = A chunk pair (hi c0, hi c1, lo c0, lo c1) + the weight chunk (hi, lo) of K-step c
+              mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)(4 * a_plane + 2 * q.b_chunk_bytes));
+  #pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const size_t go = ((size_t)(2 * c + h) * q.S_pad + (size_t)u * TC_TILE) * 8;
+                bulk_g2s(dst + h * a_plane, q.a_hi + go, (uint32_t)a_plane, &bars[LB_BFULL + stg]);
+                bulk_g2s(dst + (2 + h) * a_plane, q.a_lo + go, (uint32_t)a_plane, &bars[LB_BFULL + stg]);
+              }
+              dst += 4 * a_plane;
+            } else {
+              mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)(2 * q.b_chunk_bytes));
+            }
+            bulk_g2s(dst, reinterpret_cast<const uint8_t*>(St0.whi) + bo, (uint32_t)q.b_chunk_bytes, &bars[LB_BFULL + stg]);
+            bulk_g2s(dst + q.b_chunk_bytes, reinterpret_cast<const uint8_t*>(St0.wlo) + bo, (uint32_t)q.b_chunk_bytes,
+                     &bars[LB_BFULL + stg]);
+            ++gchunk;
+          }
         }
       }
-    } else if (lane == 0) {
-      int gchunk = 0;
+      __syncwarp();
+    } else if (warp == LY_RED_WARP && (FUSED || q.is_heads) && (p.persample_out || p.bc_out) && MODE != IAF_MODE_MULTICONV) {
+      // ===================== reducer warp: per-tile partials -> per-sample outputs, off the workers' critical path ==========
+      float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
+      constexpr bool LAY = (MODE == IAF_MODE_LAYER);
       for (int i = 0; i < n_my; ++i) {
         const int u = (int)blockIdx.x + i * (int)gridDim.x;
-        // K order is [K-step within a tap][tap]: weight chunk c and A chunk pair (2c, 2c+1) are consumed together,
-        // so both stream through shared memory at the pace of the MMAs
-        for (int c = 0; c < q.n_bchunks; ++c) {
-          if (resident && i >= 1 && !q.in_mode) continue;  // weights already resident, A comes from the workers
-          const int stg = gchunk % q.NB;
-          const int use = gchunk / q.NB;
-          if (use >= 1) {
-            TL(2, 60, gchunk);
-            mbar_wait(&bars[LB_BEMPTY + stg], (uint32_t)((use - 1) & 1));
-            TL(2, 61, gchunk);
-          }
-          uint8_t* dst = smem + q.sm_b + stg * q.stage_bytes;
-          const size_t bo = (size_t)c * q.b_chunk_bytes;
-          if (q.in_mode) {
-            // one ring stage = A chunk pair (hi c0, hi c1, lo c0, lo c1) + the weight chunk (hi, lo) of K-step c
-            mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)(4 * a_plane + 2 * q.b_chunk_bytes));
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const size_t go = ((size_t)(2 * c + h) * q.S_pad + (size_t)u * TC_TILE) * 8;
-              bulk_g2s(dst + h * a_plane, q.a_hi + go, (uint32_t)a_plane, &bars[LB_BFULL + stg]);
-              bulk_g2s(dst + (2 + h) * a_plane, q.a_lo + go, (uint32_t)a_plane, &bars[LB_BFULL + stg]);
-            }
-            dst += 4 * a_plane;
-          } else {
-            mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)(2 * q.b_chunk_bytes));
-          }
-          bulk_g2s(dst, reinterpret_cast<const uint8_t*>(St0.whi) + bo, (uint32_t)q.b_chunk_bytes, &bars[LB_BFULL + stg]);
-          bulk_g2s(dst + q.b_chunk_bytes, reinterpret_cast<const uint8_t*>(St0.wlo) + bo, (uint32_t)q.b_chunk_bytes,
-                   &bars[LB_BFULL + stg]);
-          ++gchunk;
+        const int pb = i & 1;
+        const int tile_s0 = u * q.TS;
+        const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
+        const int n_last = min(p.B - 1, fast_div(tile_s0 + q.TS - 1, p.SPS, p.mg_sps));
+        const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
+        {
+              mbar_wait(&bars[LB_PART + pb], (uint32_t)((i >> 1) & 1));
+              const int cred = LAY ? p.C : 1;
+              for (int k_ = lane; k_ < ns * cred; k_ += 32) {
+                float tot = 0.f;
+                if (LAY) {
+                  const int nl_ = k_ / p.C, c = k_ - nl_ * p.C;
+                  for (int qq = 0; qq < 4; ++qq) tot += s_part[((pb * 4 + qq) * p.MAXS + nl_) * p.C + c];
+                } else {
+                  for (int w = 0; w < LY_PART_SETS; ++w) tot += s_part[(pb * LY_PART_SETS + w) * p.MAXS + k_];
+                }
+                p.tilepart[((size_t)u * p.MAXS) * cred + k_] = tot;
+                __threadfence();
+              }
+              __syncwarp();
+              for (int k_ = lane; k_ < ns; k_ += 32) {
+                const int n = n_first + k_;
+                const int a = n * p.SPS, bb = a + p.SPS - 1;
+                const int ta = a / q.TS, tbk = bb / q.TS;
+                const unsigned expected = (unsigned)(tbk - ta + 1);
+                __threadfence();
+                if (atomicAdd(p.counter + n, 1u) == expected - 1u) {
+                  __threadfence();
+                  p.counter[n] = 0u;
+                  float cost = 0.f;
+                  for (int c = 0; c < cred; ++c) {
+                    float tot = 0.f;
+                    for (int tt = ta; tt <= tbk; ++tt) {
+                      const int nf = fast_div(tt * q.TS, p.SPS, p.mg_sps);
+                      tot += __ldcg(p.tilepart + ((size_t)tt * p.MAXS + (n - nf)) * cred + c);
+                    }
+                    if (LAY && p.bc_out) p.bc_out[(size_t)n * p.C + c] = tot;
+                    cost += tot;
+                  }
+                  if (p.persample_out) p.persample_out[n] = LAY ? cost : -cost;
+                }
+              }
         }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars[LB_PART_EMPTY + pb]);
       }
     }
-    __syncwarp();
-  } else if (warp < LY_WORKERS) {
-    // ===================== workers: (first stage) z -> operand window; MMAs; epilogues =====================
-    const int qd = warp & 3, cg = warp >> 2;
-    constexpr int CGS = LY_WORKERS / 4;
+    // warps 18 and 19 have nothing to do: they wait at the closing barrier with their 40 registers
+  } else if (warp < LY_MMA_WARPS) {
+    // ===================== MMA warpgroups: a tile's MMAs run while the epilogue warps finish the previous one =======
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(LY_REGS_MMA));
+    float acc[8 * SPG];
+    const bool tl0 = warp == 0 && lane == 0;
+    for (int i = 0; i < n_my; ++i) {
+      if (!q.in_mode) mbar_wait(&bars[LB_WIN_FULL], (uint32_t)(i & 1));
+      mma_bar_sync();
+      if (tl0) TL(0, 15, i);
+#pragma unroll 1
+      for (int ps = 0; ps < NP; ++ps) {
+        if (ps) mma_bar_sync();
+        ly_mma_tile<SPG, SPLIT>(acc, bars, St0.N, 16 * SPG * ps, q.n_bchunks, ring, q.NB, (i * NP + ps) * q.n_bchunks,
+                                LB_BFULL, smem_u32(smem + q.sm_b), (uint32_t)(FUSED ? 2 * q.b_chunk_bytes : q.stage_bytes),
+                                (uint32_t)q.b_chunk_bytes, q.in_mode != 0, smem_u32(smem + q.sm_a), (uint32_t)a_plane,
+                                (uint32_t)a_lo_off, p.Wp, (q.in_mode || ps + 1 < NP) ? -1 : (int)LB_WIN_EMPTY);
+        if (tl0 && ps + 1 == NP) TL(0, 20, i);
+        ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St0.N, 16 * SPG * ps, FUSED ? 2 * i : i,
+                          ps == 0, ps + 1 == NP);
+      }
+      if (tl0) TL(0, 21, i);
+      if (FUSED) {
+        const IafTcStage& St1 = p.st[1];
+        const int h_plane = (TC_TILE + p.MIR) * 16;
+        mbar_wait(&bars[LB_H_FULL], (uint32_t)(i & 1));
+        mma_bar_sync();
+        if (tl0) TL(0, 35, i);
+        ly_mma_tile<SPG, SPLIT>(acc, bars, St1.N, 0, q.n_bchunks1, false, 1, 0, LB_BFULL + q.n_bchunks,
+                                smem_u32(smem + q.sm_b1), (uint32_t)(2 * q.b_chunk_bytes1), (uint32_t)q.b_chunk_bytes1,
+                                false, smem_u32(smem + q.sm_h), (uint32_t)h_plane, (uint32_t)((St1.cin >> 3) * h_plane),
+                                p.Wp, LB_H_EMPTY);
+        if (tl0) TL(0, 40, i);
+        ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St1.N, 0, 2 * i + 1, true, true);
+        if (tl0) TL(0, 41, i);
+      }
+    }
+  } else {
+    // ===================== epilogue warps: (first stage) z -> operand window; epilogues =====================
+    const int qd = ew & 3, cg = ew >> 2;  // quarter of the tile's slots, first of the column groups g = cg + CGS k
+    constexpr int CGS = LY_EPI_WARPS / 4;
+    // the step-mode partials keep one per (g % 4, quarter): each warp covers two of the four column-group sets
+    static_assert(CGS == 2 && LY_PART_SETS == 4 * 2 * CGS, "per-sample partial sets and epilogue warps out of step");
     const int sl = qd * 32 + lane;
     float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
     float* s_acc = reinterpret_cast<float*>(smem + q.sm_acc);
@@ -305,11 +462,13 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     };
     const int h_plane = (TC_TILE + p.MIR) * 16;  // fused: bytes per chunk plane of the hidden operand buffer
 
-    auto load_window = [&](int i) {  // fp32 z -> fp16 hi/lo A window of this CTA's i-th tile
+    // fp32 z -> fp16 hi/lo A window of this CTA's i-th tile, once the MMAs have read tile i - 1's; handed to the MMAs
+    auto build_window = [&](int i) {
+      if (i >= 1) mbar_wait(&bars[LB_WIN_EMPTY], (uint32_t)((i - 1) & 1));
       const int u = (int)blockIdx.x + i * (int)gridDim.x;
 #pragma unroll
       for (int it = 0; it < TC_ZITEMS; ++it) {
-        const int idx = tid + it * LY_WTHREADS;
+        const int idx = et + it * LY_ETHREADS;
         if (idx < p.WIN * nchunk) {
           const int ch = fast_div(idx, p.WIN, p.mg_win);
           const int s_ = idx - ch * p.WIN;
@@ -332,24 +491,25 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
         }
       }
       fence_proxy_async();  // generic-proxy stores -> the wgmma (async proxy) reads of the window
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars[LB_WIN_FULL]);
+      if (ew == 0 && lane == 0) TL(1, 10, i);
     };
+    // this warp is done reading the accumulator tile
+    auto acc_release = [&]() {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars[LB_ACC_EMPTY]);
+    };
+
+    if (!q.in_mode) build_window(0);
 
     for (int i = 0; i < n_my; ++i) {
       const int u = (int)blockIdx.x + i * (int)gridDim.x;
-      // the previous tile's epilogue is done with the accumulator tile and its MMAs with the A window
-      worker_bar_sync();
-      if (warp == 0 && lane == 0) TL(1, 0, i);
-      if (!q.in_mode) {
-        load_window(i);
-        worker_bar_sync();
-        if (warp == 0 && lane == 0) TL(1, 10, i);
-      }
-      ly_mma_tile<NGW>(smem, bars, s_acc, St0.N, q.n_bchunks, !resident || q.in_mode, q.NB, i * q.n_bchunks, LB_BFULL,
-                       smem_u32(smem + q.sm_b), (uint32_t)(FUSED ? 2 * q.b_chunk_bytes : q.stage_bytes),
-                       (uint32_t)q.b_chunk_bytes, q.in_mode != 0, smem_u32(smem + q.sm_a), (uint32_t)a_plane,
-                       (uint32_t)a_lo_off, p.Wp);
-      worker_bar_sync();
-      if (warp == 0 && lane == 0) TL(1, 20, i);
+      // per stage: the next tile's window goes to the MMAs before this tile's epilogue, which then runs under them
+      if (!FUSED && !q.in_mode && i + 1 < n_my) build_window(i + 1);
+      // the accumulator tile's uses: one per tile, or (fused) 2i for the hidden stage and 2i + 1 for the heads
+      mbar_wait(&bars[LB_ACC_FULL], FUSED ? 0u : (uint32_t)(i & 1));
+      if (ew == 0 && lane == 0) TL(1, 25, i);
       const SlotInfo si_all = decode_slot(p, u * q.TS + sl, HW);
       const bool bx0 = (si_all.x == 0), bxW = (si_all.x == p.W - 1), byH = (si_all.y == p.H - 1);
 
@@ -471,6 +631,10 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
           float red[NRED];
   #pragma unroll
           for (int k_ = 0; k_ < NRED; ++k_) red[k_] = 0.f;
+          // step mode: the running sums of this thread's two column-group sets g % 4 = cg and cg + 2 (red[0] holds
+          // the current group's set while it is summed), so each partial adds the same terms in the same order as
+          // one warp per set would
+          float rs0 = 0.f, rs1 = 0.f;
           const int tile_s0 = u * q.TS;
           const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
           const int n_last = min(p.B - 1, fast_div(tile_s0 + q.TS - 1, p.SPS, p.mg_sps));
@@ -490,9 +654,12 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             }
             uint32_t r[16];
             acc_ld16(c0, r, pitch, St.wsinv);
+            const bool set_hi = ((g - cg) / CGS) & 1;
             if (MODE == IAF_MODE_LAYER) {
   #pragma unroll
               for (int k_ = 0; k_ < NRED; ++k_) red[k_] = 0.f;
+            } else {
+              red[0] = set_hi ? rs1 : rs0;
             }
             if (si.valid) {
   #pragma unroll
@@ -535,6 +702,10 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                 }
               }
             }
+            if (MODE != IAF_MODE_LAYER) {
+              if (set_hi) rs1 = red[0];
+              else rs0 = red[0];
+            }
             if (MODE == IAF_MODE_LAYER) {
               for (int nl_ = 0; nl_ < ns; ++nl_) {
   #pragma unroll
@@ -553,10 +724,13 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             if (!LAY) {
               if (i >= 2) mbar_wait(&bars[LB_PART_EMPTY + pb], (uint32_t)(((i >> 1) - 1) & 1));
               for (int nl_ = 0; nl_ < ns; ++nl_) {
-                float x = (si.valid && si.n == n_first + nl_) ? red[0] : 0.f;
   #pragma unroll
-                for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-                if (lane == 0) s_part[(pb * LY_WORKERS + warp) * p.MAXS + nl_] = x;
+                for (int h2 = 0; h2 < 2; ++h2) {
+                  float x = (si.valid && si.n == n_first + nl_) ? (h2 ? rs1 : rs0) : 0.f;
+  #pragma unroll
+                  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+                  if (lane == 0) s_part[(pb * LY_PART_SETS + (cg + CGS * h2) * 4 + qd) * p.MAXS + nl_] = x;
+                }
               }
             }
             __syncwarp();
@@ -566,78 +740,30 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
 
       const float* tb0 = reinterpret_cast<const float*>(smem + q.sm_bias);
       if (FUSED) {
+        // the hidden epilogue refills the hidden operand buffer once the heads MMAs of tile i - 1 have read it
+        if (i >= 1) mbar_wait(&bars[LB_H_EMPTY], (uint32_t)((i - 1) & 1));
         hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
-        fence_proxy_async();
-        worker_bar_sync();
-        if (warp == 0 && lane == 0) TL(1, 30, i);
+        fence_proxy_async();  // generic-proxy stores -> the heads' wgmma reads of the buffer
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars[LB_H_FULL]);
+        acc_release();
+        if (ew == 0 && lane == 0) TL(1, 30, i);
+        // the next tile's window is built under the heads MMAs, the heads epilogue runs under the next hidden MMAs
+        if (i + 1 < n_my) build_window(i + 1);
+        mbar_wait(&bars[LB_ACC_FULL], 1u);
+        if (ew == 0 && lane == 0) TL(1, 45, i);
         const IafTcStage& St1 = p.st[1];
-        ly_mma_tile<NGW>(smem, bars, s_acc, St1.N, q.n_bchunks1, false, 1, 0, LB_BFULL + q.n_bchunks,
-                         smem_u32(smem + q.sm_b1), (uint32_t)(2 * q.b_chunk_bytes1), (uint32_t)q.b_chunk_bytes1, false,
-                         smem_u32(smem + q.sm_h), (uint32_t)h_plane, (uint32_t)((St1.cin >> 3) * h_plane), p.Wp);
-        worker_bar_sync();
-        if (warp == 0 && lane == 0) TL(1, 40, i);
         SlotInfo si_out = si_all;
         si_out.valid = si_all.valid && sl < q.TO;
         heads_epi(St1, reinterpret_cast<const float*>(smem + q.sm_bias1), St1.N >> 4, ly_acc_pitch(St1.N), si_out);
-      } else if (!q.is_heads) {
-        hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
+        acc_release();
+        if (ew == 0 && lane == 0) TL(1, 50, i);
       } else {
-        heads_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
+        if (!q.is_heads) hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
+        else heads_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
+        acc_release();
+        if (ew == 0 && lane == 0) TL(1, 30, i);
       }
-    }
-  }
-
-  if (warp == LY_RED_WARP && (FUSED || q.is_heads) && (p.persample_out || p.bc_out) && MODE != IAF_MODE_MULTICONV) {
-    // ===================== reducer warp: per-tile partials -> per-sample outputs, off the workers' critical path ==========
-    float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
-    constexpr bool LAY = (MODE == IAF_MODE_LAYER);
-    for (int i = 0; i < n_my; ++i) {
-      const int u = (int)blockIdx.x + i * (int)gridDim.x;
-      const int pb = i & 1;
-      const int tile_s0 = u * q.TS;
-      const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
-      const int n_last = min(p.B - 1, fast_div(tile_s0 + q.TS - 1, p.SPS, p.mg_sps));
-      const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
-      {
-            mbar_wait(&bars[LB_PART + pb], (uint32_t)((i >> 1) & 1));
-            const int cred = LAY ? p.C : 1;
-            for (int k_ = lane; k_ < ns * cred; k_ += 32) {
-              float tot = 0.f;
-              if (LAY) {
-                const int nl_ = k_ / p.C, c = k_ - nl_ * p.C;
-                for (int qq = 0; qq < 4; ++qq) tot += s_part[((pb * 4 + qq) * p.MAXS + nl_) * p.C + c];
-              } else {
-                for (int w = 0; w < LY_WORKERS; ++w) tot += s_part[(pb * LY_WORKERS + w) * p.MAXS + k_];
-              }
-              p.tilepart[((size_t)u * p.MAXS) * cred + k_] = tot;
-              __threadfence();
-            }
-            __syncwarp();
-            for (int k_ = lane; k_ < ns; k_ += 32) {
-              const int n = n_first + k_;
-              const int a = n * p.SPS, bb = a + p.SPS - 1;
-              const int ta = a / q.TS, tbk = bb / q.TS;
-              const unsigned expected = (unsigned)(tbk - ta + 1);
-              __threadfence();
-              if (atomicAdd(p.counter + n, 1u) == expected - 1u) {
-                __threadfence();
-                p.counter[n] = 0u;
-                float cost = 0.f;
-                for (int c = 0; c < cred; ++c) {
-                  float tot = 0.f;
-                  for (int tt = ta; tt <= tbk; ++tt) {
-                    const int nf = fast_div(tt * q.TS, p.SPS, p.mg_sps);
-                    tot += __ldcg(p.tilepart + ((size_t)tt * p.MAXS + (n - nf)) * cred + c);
-                  }
-                  if (LAY && p.bc_out) p.bc_out[(size_t)n * p.C + c] = tot;
-                  cost += tot;
-                }
-                if (p.persample_out) p.persample_out[n] = LAY ? cost : -cost;
-              }
-            }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[LB_PART_EMPTY + pb]);
     }
   }
 

@@ -22,8 +22,10 @@ L.LIB = B.LIB
 import torch  # noqa: E402
 from bench import make_workload  # noqa: E402
 
-PHASE = {0: "tile start", 10: "window built", 20: "MMAs done", 30: "hidden epilogue done", 40: "heads MMAs done",
-         99: "end"}
+PHASE = {15: "MMA operands ready", 20: "MMAs done", 21: "acc tile written", 35: "heads operands ready",
+         40: "heads MMAs done", 41: "heads acc written", 10: "window built", 25: "acc ready", 30: "(hidden) epilogue done",
+         45: "heads acc ready", 50: "heads epilogue done", 99: "end"}
+ROLE = {0: "MMA warpgroups", 1: "epilogue warps"}
 
 
 def run(name, stage):
@@ -58,12 +60,15 @@ def run(name, stage):
     ev.sort()
     print("=== %s, stage %s: %d events ===" % (name, "last" if stage is None else stage, len(ev)))
     for t, role, tag, k in ev:
-        print("%9d  role%d  %-22s k=%d" % (t, role, PHASE.get(tag, {60: "ring wait", 61: "ring released"}.get(tag, tag)), k))
-    # phase cycles: role 1 events are phase ends, in order; each phase lasts from the previous event to its own
-    w = [e for e in ev if e[1] == 1]
-    print("--- cycles per phase (worker warp 0, after the closing barrier) ---")
-    for (t0, _, g0, k0), (t1, _, g1, k1) in zip(w, w[1:]):
-        print("tile %d  %-22s -> %-22s %7d" % (k0 if g1 in (0, 99) else k1, PHASE.get(g0), PHASE.get(g1), t1 - t0))
+        print("%9d  role%d  %-24s k=%d" % (t, role, PHASE.get(tag, {60: "ring wait", 61: "ring released"}.get(tag, tag)), k))
+    # phase cycles per role: its events are phase ends, in order; each phase lasts from the previous event to its own.
+    # The two roles run concurrently, so their phases of neighbouring tiles overlap in time (compare the t column).
+    for role in (0, 1):
+        w = [e for e in ev if e[1] == role]
+        print("--- %s: cycles per phase (lane 0 of its first warp) ---" % ROLE[role])
+        for (t0, _, g0, k0), (t1, _, g1, k1) in zip(w, w[1:]):
+            print("tile %d  %-24s -> %-24s %7d  (ends at %d)" % (k1 if g1 != 99 else k0, PHASE.get(g0), PHASE.get(g1),
+                                                                t1 - t0, t1))
     waits = [(e[0], e[2], e[3]) for e in ev if e[1] == 2]
     tot = sum(b[0] - a[0] for a, b in zip(waits, waits[1:]) if a[1] == 60 and b[1] == 61)
     if waits:
