@@ -816,7 +816,7 @@ int iaf_bwd_plan_create(IafBwdPlan** out, const iaf_desc_t* d, const int* cin, c
     int dev = 0;
     cudaDeviceProp prop;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) { iaf_bwd_plan_destroy(pl); return IAF_ERR_CUDA; }
-    pl->num_sms = prop.multiProcessorCount;
+    pl->num_sms = iaf_plan_num_sms(prop.multiProcessorCount);
   }
   pl->nseg = (d->W + BW_PX - 1) / BW_PX;
   pl->P = BW_PX * pl->nseg + 2;

@@ -40,6 +40,7 @@ static inline cudaError_t iaf_smem_optin(K kernel) {
 #endif
 }
 #include <stdint.h>
+#include <stdlib.h>
 #include "../../include/iaf_b200.h"
 
 #define IAF_NTAPS 5          // live taps of the 3x3 AR mask: (ky,kx) = (1,1)c (1,2) (2,0) (2,1) (2,2)
@@ -155,6 +156,18 @@ enum { IAF_MODE_MULTICONV = 0, IAF_MODE_STEP = 1, IAF_MODE_LAYER = 2 };
 enum { IAF_SCRATCH_FITS = 0, IAF_SCRATCH_ALLOC = 1, IAF_SCRATCH_REALLOC = 2 };
 static inline int iaf_scratch_need(int have_B, int B) {
   return B <= have_B ? IAF_SCRATCH_FITS : (have_B > 0 ? IAF_SCRATCH_REALLOC : IAF_SCRATCH_ALLOC);
+}
+
+// The SM count a plan sizes its persistent grids and split-K groups for: the device's, or min(n, it) when IAF_NUM_SMS=n
+// (a whole number >= 1; any other value is ignored) is in the environment when the plan is created.  Development: with a
+// small n a small batch runs many tiles per CTA, the regime of the full-size workloads.
+static inline int iaf_plan_num_sms(int device_sms) {
+  const char* e = getenv("IAF_NUM_SMS");
+  if (!e || !*e) return device_sms;
+  char* end = nullptr;
+  const long n = strtol(e, &end, 10);
+  if (*end != '\0' || n < 1) return device_sms;
+  return n < device_sms ? (int)n : device_sms;
 }
 
 // Raw-parameter description handed to the pack kernel.

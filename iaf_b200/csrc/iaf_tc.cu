@@ -540,7 +540,7 @@ int iaf_tc_plan_create(IafTcPlan** out, const iaf_desc_t* d) {
   cudaDeviceProp prop;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) { delete pl; return IAF_ERR_CUDA; }
   if (prop.major != 9) { delete pl; return IAF_ERR_UNSUPPORTED; }  // wgmma: sm_90a
-  pl->num_sms = prop.multiProcessorCount;
+  pl->num_sms = iaf_plan_num_sms(prop.multiProcessorCount);
   for (int j = 0; j < pl->n_stages; ++j) {
     const size_t wb = (size_t)pl->K[j] * pl->N[j] * 2;
     // bias [N] and pad-channel weights [4][N] are ONE table [5][N]; the inverse weight scales [N] follow it
@@ -949,7 +949,7 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
   pl->grad_flip = iaf_variant_flags(d->variant).reflect ? 0 : 1;
   pl->n_stages = n_stages;
   pl->MIR = MIR; pl->WIN = TC_TILE + MIR; pl->MAXS = (TC_TILE - 1) / SPS + 2;
-  pl->num_sms = prop.multiProcessorCount;
+  pl->num_sms = iaf_plan_num_sms(prop.multiProcessorCount);
   int maxn = 0;
   for (int j = 0; j < n_stages; ++j) {
     const int kin = ncol[j], N = cin[j];

@@ -237,6 +237,11 @@ int iaf_plan_path_for_entry(const iaf_plan_t* plan, int entry);
 /* Which kernels the plan's BACKWARD entries run (creates the backward plan on first use): 0 = exact-fp32 SIMT kernels,
  * 1 = data gradient on the tensor cores, 2 = data and weight gradient on the tensor cores (plans whose forward is on the
  * tensor-core path, channel counts in multiples of 16; IAF_BWD_TC=0 / IAF_BWD_WG_TC=0 in the environment switch them off).
+ * IAF_NUM_SMS=n in the environment (development; a whole number >= 1, anything else is ignored) makes the plans created
+ * from then on schedule for min(n, the device's SM count) SMs: the persistent grids of the tensor-core forward and
+ * data-gradient stages and the split-K groups of the weight gradients.  A small batch then runs many tiles per CTA, as
+ * the full-size workloads do.  Forward outputs and input gradients do not depend on it; parameter gradients may change
+ * in the last bits (their split-K grouping follows the SM count).
  * The reference differentiates the same graph it runs forward (graphy/nodes/ar.py:304-329 through theano.grad). */
 int iaf_plan_bwd_path(iaf_plan_t* plan);
 uint64_t iaf_plan_launch_count(const iaf_plan_t* plan); /* kernels launched through this plan so far    */
