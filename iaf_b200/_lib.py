@@ -12,7 +12,7 @@ VARIANTS = {"tf": 0, "theano": 1, "theano_flipmask": 2}  # theano_flipmask: mult
 NLS = {None: 0, "None": 0, "none": 0, "elu": 1, "softplus": 2, "relu": 3, "tanh": 4, "leakyrelu": 5}
 PATHS = {"auto": 0, "simt": 1, "tc": 2}
 PATH_NAMES = {1: "simt", 2: "tc"}
-ENTRIES = {"multiconv": 0, "step": 1, "layer": 2}
+ENTRIES = {"multiconv": 0, "step": 1, "layer": 2, "ar_logp": 3}
 
 OK, ERR_BAD_ARG, ERR_BAD_SHAPE, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOT_PACKED, ERR_NO_DEVICE = 0, -1, -2, -3, -4, -5, -6
 ERR_CAPTURED = -7
@@ -55,6 +55,10 @@ SYMBOLS = {
                                           C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.c_int, _P]),
     "iaf_multiconv_bwd": (C.c_int, [_P, _P, _P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), _P, _P, C.POINTER(_P),
                                     C.POINTER(_P), C.POINTER(_P), C.c_int, _P]),
+    "iaf_ar_logp_fwd": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, _P]),
+    "iaf_ar_logp_fwd_train": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.POINTER(_P), C.c_int, _P]),
+    "iaf_ar_logp_bwd_saved": (C.c_int, [_P, _P, _P, _P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), _P, _P, _P, _P, _P,
+                                        C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.c_int, _P]),
     "iaf_strerror": (C.c_char_p, [C.c_int]),
     "iaf_last_cuda_error": (C.c_char_p, []),
     "iaf_version": (C.c_int, []),

@@ -282,13 +282,25 @@ __global__ void __launch_bounds__(BW_THREADS) iaf_bwd_transpose_kernel(const flo
 __device__ __forceinline__ int bw_head_col(int n_heads, int k, int c) { return n_heads == 2 ? ((c >> 2) * 8 + 4 * k + (c & 3)) : c; }
 
 // step: hb holds the raw heads (m, s) on entry and (g_m, g_s) on exit; g_z receives the direct term
+// LOGP (the MADE prior's density, logps = -0.5 log 2pi - arw_logsd - 0.5 z'^2): the step's backward with the upstream
+//   G = g_logps + g_logp_bc[b,c] + g_logp[b],  g_z' = -z' G,  g_arw_logsd = -G
 struct IafAffineBwdParams {
   const float* z; const float* g_zout; const float* g_logsd; const float* g_logdet;
   const float* z_out; const float* logsd;  // kept by the training forward; when given, hb is write-only
   float* hb; float* g_z;
   int B, C, HW, cp, head_pad;
   float scale;
+  const float* g_logps; const float* g_logp_bc; const float* g_logp;  // LOGP: nullable
 };
+__device__ __forceinline__ float bw_logp_upstream(const float* g_logps, const float* g_logp_bc, const float* g_logp,
+                                                  size_t e, int n, int c, int C) {
+  float G = 0.f;
+  if (g_logps) G += __ldg(g_logps + e);
+  if (g_logp_bc) G += __ldg(g_logp_bc + (size_t)n * C + c);
+  if (g_logp) G += __ldg(g_logp + n);
+  return G;
+}
+template <bool LOGP>
 __global__ void __launch_bounds__(BW_THREADS) iaf_bwd_affine_kernel(const __grid_constant__ IafAffineBwdParams p) {
   const size_t total = (size_t)p.B * p.head_pad * p.HW;
   for (size_t i = (size_t)blockIdx.x * BW_THREADS + threadIdx.x; i < total; i += (size_t)gridDim.x * BW_THREADS) {
@@ -313,10 +325,17 @@ __global__ void __launch_bounds__(BW_THREADS) iaf_bwd_affine_kernel(const __grid
       ex = expf(-p.scale * s);
       zn = (__ldg(p.z + e) - p.scale * m) * ex;
     }
-    const float gzo = __ldg(p.g_zout + e);
-    float gs = -p.scale * zn * gzo;
-    if (p.g_logsd) gs += p.scale * __ldg(p.g_logsd + e);
-    if (p.g_logdet) gs -= p.scale * __ldg(p.g_logdet + n);
+    float gzo, gs;
+    if (LOGP) {
+      const float G = bw_logp_upstream(p.g_logps, p.g_logp_bc, p.g_logp, e, n, c, p.C);
+      gzo = -zn * G;
+      gs = -p.scale * zn * gzo - p.scale * G;
+    } else {
+      gzo = __ldg(p.g_zout + e);
+      gs = -p.scale * zn * gzo;
+      if (p.g_logsd) gs += p.scale * __ldg(p.g_logsd + e);
+      if (p.g_logdet) gs -= p.scale * __ldg(p.g_logdet + n);
+    }
     p.hb[om] = -p.scale * ex * gzo;
     p.hb[os] = gs;
     p.g_z[e] = ex * gzo;
@@ -1001,24 +1020,36 @@ int iaf_bwd_run(IafBwdPlan* pl, const IafBwdArgs* a, cudaStream_t stream, int* n
   }
 
   // ---- 2. gradient at the heads ----
-  const bool fused_step = pl->dg && pl->wg_tc && a->mode == IAF_MODE_STEP && saved && iaf_dg_step_supported(pl->dg);
+  // the MADE prior's density (IAF_MODE_LOGP) is the step with another upstream: same kernels, same path selection
+  const bool logp = a->mode == IAF_MODE_LOGP;
+  const bool steplike = a->mode == IAF_MODE_STEP || logp;
+  const bool fused_step = pl->dg && pl->wg_tc && steplike && saved && iaf_dg_step_supported(pl->dg);
   const float* step_bias = nullptr;
   if (layer) {
     IAF_LAUNCH(iaf_bwd_layer_affine_kernel, ew_grid((size_t)B * pl->head_pad * HW), BW_THREADS, 0, stream, lq);
-  } else if (a->mode == IAF_MODE_STEP && fused_step) {
+  } else if (steplike && fused_step) {
     // tensor-core backward with kept activations: affine backward, per-sample scale, heads' bias sums and gradient image in
     // one launch (iaf_dg_step_kernel); the fp32 heads gradient is not needed by anything downstream
-    if ((st = iaf_dg_begin_step(pl->dg, a->z_out_saved, a->logsd_saved, a->g_zout, a->g_logsd, a->g_logdet, a->g_z, nullptr,
-                                pl->head_pad, B, stream, &step_bias)) != IAF_OK)
-      return st;
-  } else if (a->mode == IAF_MODE_STEP) {
+    if (logp) {
+#ifndef IAF_EMU  // (the host emulation has no tensor-core plans: fused_step is never set there)
+      st = iaf_dg_begin_step_logp(pl->dg, a->z_out_saved, a->logsd_saved, a->g_logps, a->g_logp_bc, a->g_logp, a->g_z,
+                                  nullptr, pl->head_pad, B, stream, &step_bias);
+#endif
+    } else {
+      st = iaf_dg_begin_step(pl->dg, a->z_out_saved, a->logsd_saved, a->g_zout, a->g_logsd, a->g_logdet, a->g_z, nullptr,
+                             pl->head_pad, B, stream, &step_bias);
+    }
+    if (st != IAF_OK) return st;
+  } else if (steplike) {
     IafAffineBwdParams q;
     memset(&q, 0, sizeof(q));
     q.z = a->z; q.g_zout = a->g_zout; q.g_logsd = a->g_logsd; q.g_logdet = a->g_logdet;
+    q.g_logps = a->g_logps; q.g_logp_bc = a->g_logp_bc; q.g_logp = a->g_logp;
     q.z_out = saved ? a->z_out_saved : nullptr; q.logsd = saved ? a->logsd_saved : nullptr;
     q.hb = pl->hb; q.g_z = a->g_z;
     q.B = B; q.C = d.n_z; q.HW = HW; q.cp = pl->ncol[last]; q.head_pad = pl->head_pad; q.scale = 0.1f;
-    IAF_LAUNCH(iaf_bwd_affine_kernel, ew_grid((size_t)B * pl->head_pad * HW), BW_THREADS, 0, stream, q);
+    if (logp) IAF_LAUNCH(iaf_bwd_affine_kernel<true>, ew_grid((size_t)B * pl->head_pad * HW), BW_THREADS, 0, stream, q);
+    else IAF_LAUNCH(iaf_bwd_affine_kernel<false>, ew_grid((size_t)B * pl->head_pad * HW), BW_THREADS, 0, stream, q);
   } else {
     IafScatterParams q;
     memset(&q, 0, sizeof(q));

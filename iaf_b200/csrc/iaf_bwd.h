@@ -9,7 +9,7 @@
 struct IafBwdPlan;
 
 struct IafBwdArgs {
-  int mode;  // IAF_MODE_STEP | IAF_MODE_MULTICONV | IAF_MODE_LAYER
+  int mode;  // IAF_MODE_STEP | IAF_MODE_MULTICONV | IAF_MODE_LAYER | IAF_MODE_LOGP (kept activations only)
   int B;
   const float* z;
   const float* ctx;
@@ -25,6 +25,9 @@ struct IafBwdArgs {
   const float* g_logsd;  // step: [B,n_z,H,W] or nullptr
   const float* g_logdet; // step: [B] or nullptr
   const float* g_heads[IAF_MAX_HEADS];  // multiconv: gradient of each head output
+  const float* g_logps;                 // logp: [B,n_z,H,W] or nullptr
+  const float* g_logp_bc;               // logp: [B,n_z] or nullptr
+  const float* g_logp;                  // logp: [B] or nullptr
   // activations kept by the training forward (iaf_step_fwd_train): when have_saved the recompute is skipped
   int have_saved;
   const float* z_out_saved;              // z'

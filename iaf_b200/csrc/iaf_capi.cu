@@ -177,7 +177,7 @@ static int ensure_scratch(iaf_plan* pl, int B, cudaStream_t stream) {
 
 extern "C" {
 
-int iaf_version(void) { return 200; }  // 0.2.0
+int iaf_version(void) { return 201; }  // 0.2.1
 
 const char* iaf_strerror(int status) {
   switch (status) {
@@ -383,7 +383,7 @@ int iaf_pack_weights(iaf_plan_t* pl, const float* const* w, const float* const* 
 static int run(iaf_plan* pl, int mode, const float* z, const float* ctx, const float* post_mean,
                const float* post_logsd, const float* prior_mean, const float* prior_logsd, float* z_out,
                float* elem_out, float* m_out, float* s_out, float* bc_out, float* persample_out, int B,
-               cudaStream_t stream, float* const* hid_out = nullptr) {
+               cudaStream_t stream, float* const* hid_out = nullptr, float* logps_out = nullptr) {
   if (!pl->packed) return IAF_ERR_NOT_PACKED;
   if (B <= 0) return IAF_ERR_BAD_ARG;
   { int cg = capture_guard(pl, stream, fwd_need(pl, mode, B)); if (cg != IAF_OK) return cg; }
@@ -397,7 +397,7 @@ static int run(iaf_plan* pl, int mode, const float* z, const float* ctx, const f
     a.mode = mode; a.z = z; a.ctx = ctx; a.post_mean = post_mean; a.post_logsd = post_logsd;
     a.prior_mean = prior_mean; a.prior_logsd = prior_logsd; a.z_out = z_out; a.elem_out = elem_out;
     if (mode == IAF_MODE_MULTICONV) { a.z_out = m_out; a.elem_out = s_out; }  // raw heads travel in the same slots
-    a.bc_out = bc_out; a.persample_out = persample_out; a.B = B;
+    a.bc_out = bc_out; a.persample_out = persample_out; a.logps_out = logps_out; a.B = B;
     for (int j = 0; j < d.n_hidden && hid_out; ++j) a.hid_out[j] = hid_out[j];
     int nl = 0;
     int st = iaf_tc_run(pl->tc, &a, stream, &nl);
@@ -413,7 +413,7 @@ static int run(iaf_plan* pl, int mode, const float* z, const float* ctx, const f
   p.z = z; p.ctx = ctx; p.post_mean = post_mean; p.post_logsd = post_logsd;
   p.prior_mean = prior_mean; p.prior_logsd = prior_logsd;
   p.z_out = z_out; p.logsd_out = elem_out; p.m_out = m_out; p.s_out = s_out;
-  p.bc_out = bc_out; p.persample_out = persample_out;
+  p.bc_out = bc_out; p.persample_out = persample_out; p.logps_out = logps_out;
   p.partial = pl->partial; p.counter = pl->counter;
   for (int j = 0; j < d.n_hidden && hid_out; ++j) p.hid_out[j] = hid_out[j];
   for (int j = 0; j < pl->n_stages; ++j) {
@@ -475,6 +475,28 @@ int iaf_step_fwd_train(iaf_plan_t* pl, const float* z, const float* context, flo
              nullptr, logdet_out, B, (cudaStream_t)stream, hidden_out);
 }
 
+// The MADE prior's density (models.py:36-38, 304-309): the step's stack and affine update with the logp epilogue
+int iaf_ar_logp_fwd(iaf_plan_t* pl, const float* z, const float* context, float* logps_out, float* logp_bc_out,
+                    float* logp_out, int B, void* stream) {
+  if (!pl || !z) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_hidden > 0 && !context) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_heads != 2 || pl->d.head[0] != pl->d.n_z) return IAF_ERR_BAD_SHAPE;
+  return run(pl, IAF_MODE_LOGP, z, context, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+             logp_bc_out, logp_out, B, (cudaStream_t)stream, nullptr, logps_out);
+}
+
+int iaf_ar_logp_fwd_train(iaf_plan_t* pl, const float* z, const float* context, float* logps_out, float* logp_bc_out,
+                          float* logp_out, float* z_out, float* logsd_out, float* const* hidden_out, int B,
+                          void* stream) {
+  if (!pl || !z || !z_out || !logsd_out) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_hidden > 0 && (!context || !hidden_out)) return IAF_ERR_BAD_ARG;
+  for (int j = 0; j < pl->d.n_hidden; ++j)
+    if (!hidden_out[j]) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_heads != 2 || pl->d.head[0] != pl->d.n_z) return IAF_ERR_BAD_SHAPE;
+  return run(pl, IAF_MODE_LOGP, z, context, nullptr, nullptr, nullptr, nullptr, z_out, logsd_out, nullptr, nullptr,
+             logp_bc_out, logp_out, B, (cudaStream_t)stream, hidden_out, logps_out);
+}
+
 // iaf_step_bwd on a tensor-core plan recomputes z', arw_logsd and the activations with the forward's own kernels
 static bool bwd_recomputes(const iaf_plan* pl, int mode, bool have_saved) {
   return mode == IAF_MODE_STEP && !have_saved && pl->path == IAF_PATH_TC && iaf_tc_mode_supported(pl->tc, IAF_MODE_STEP) &&
@@ -494,7 +516,8 @@ static int run_bwd(iaf_plan* pl, int mode, const float* z, const float* ctx, con
                    const float* const* scale, const float* g_zout, const float* g_logsd, const float* g_logdet,
                    const float* const* g_heads, float* g_z, float* g_ctx, float* const* g_w, float* const* g_scale,
                    float* const* g_bias, int B, cudaStream_t stream, const float* z_out_saved = nullptr,
-                   const float* logsd_saved = nullptr, const float* const* hidden_saved = nullptr) {
+                   const float* logsd_saved = nullptr, const float* const* hidden_saved = nullptr,
+                   const float* g_logps = nullptr, const float* g_logp_bc = nullptr, const float* g_logp = nullptr) {
   if (!pl->packed) return IAF_ERR_NOT_PACKED;
   if (B <= 0) return IAF_ERR_BAD_ARG;
   { int cg = capture_guard(pl, stream, bwd_need(pl, mode, z_out_saved != nullptr, B)); if (cg != IAF_OK) return cg; }
@@ -519,6 +542,7 @@ static int run_bwd(iaf_plan* pl, int mode, const float* z, const float* ctx, con
   }
   a.w_raw = w; a.scale_raw = scale;
   a.g_zout = g_zout; a.g_logsd = g_logsd; a.g_logdet = g_logdet;
+  a.g_logps = g_logps; a.g_logp_bc = g_logp_bc; a.g_logp = g_logp;
   if (g_heads) { a.g_heads[0] = g_heads[0]; a.g_heads[1] = d.n_heads == 2 ? g_heads[1] : nullptr; }
   a.g_z = g_z; a.g_ctx = d.n_hidden > 0 ? g_ctx : nullptr;
   a.g_w = g_w; a.g_scale = g_scale; a.g_bias = g_bias;
@@ -579,6 +603,20 @@ int iaf_step_bwd_saved(iaf_plan_t* pl, const float* z, const float* z_out, const
   if (pl->d.n_heads != 2 || pl->d.head[0] != pl->d.n_z) return IAF_ERR_BAD_SHAPE;
   return run_bwd(pl, IAF_MODE_STEP, z, nullptr, w, scale, g_z_out, g_logsd, g_logdet, nullptr, g_z, g_context, g_w,
                  g_scale, g_bias, B, (cudaStream_t)stream, z_out, logsd, hidden);
+}
+
+int iaf_ar_logp_bwd_saved(iaf_plan_t* pl, const float* z, const float* z_out, const float* logsd,
+                          const float* const* hidden, const float* const* w, const float* const* scale,
+                          const float* g_logps, const float* g_logp_bc, const float* g_logp, float* g_z,
+                          float* g_context, float* const* g_w, float* const* g_scale, float* const* g_bias, int B,
+                          void* stream) {
+  if (!pl || !z || !z_out || !logsd || !g_z) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_hidden > 0 && !hidden) return IAF_ERR_BAD_ARG;
+  for (int j = 0; j < pl->d.n_hidden; ++j)
+    if (!hidden[j]) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_heads != 2 || pl->d.head[0] != pl->d.n_z) return IAF_ERR_BAD_SHAPE;
+  return run_bwd(pl, IAF_MODE_LOGP, z, nullptr, w, scale, nullptr, nullptr, nullptr, nullptr, g_z, g_context, g_w, g_scale,
+                 g_bias, B, (cudaStream_t)stream, z_out, logsd, hidden, g_logps, g_logp_bc, g_logp);
 }
 
 int iaf_layer_bwd(iaf_plan_t* pl, const float* eps, const float* post_mean, const float* post_logsd,
@@ -764,7 +802,7 @@ int iaf_host_wait(iaf_plan_t* pl) {
 int iaf_plan_path(const iaf_plan_t* pl) { return pl ? pl->path : IAF_ERR_BAD_ARG; }
 
 int iaf_plan_path_for_entry(const iaf_plan_t* pl, int entry) {
-  if (!pl || entry < IAF_MODE_MULTICONV || entry > IAF_MODE_LAYER) return IAF_ERR_BAD_ARG;
+  if (!pl || entry < IAF_MODE_MULTICONV || entry > IAF_MODE_LOGP) return IAF_ERR_BAD_ARG;  // iaf_entry == IAF_MODE_*
   if (pl->path == IAF_PATH_TC && iaf_tc_mode_supported(pl->tc, entry)) return IAF_PATH_TC;
   if (pl->path == IAF_PATH_TC && pl->d.path == IAF_PATH_TC) return IAF_ERR_UNSUPPORTED;
   return pl->simt_ok ? IAF_PATH_SIMT : IAF_ERR_UNSUPPORTED;

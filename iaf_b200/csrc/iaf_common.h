@@ -132,8 +132,9 @@ struct IafSimtParams {
   float* logsd_out;        // step mode: arw_logsd; layer mode: kl per element
   float* m_out;            // multiconv mode: head 0
   float* s_out;            // multiconv mode: head 1
-  float* bc_out;           // layer mode: [B,C] sum over (h,w) of kl
-  float* persample_out;    // step: logdet [B]; layer: kl_cost [B]
+  float* bc_out;           // layer mode: [B,C] sum over (h,w) of kl; logp mode: of logps
+  float* persample_out;    // step: logdet [B]; layer: kl_cost [B]; logp: logp [B]
+  float* logps_out;        // logp mode: per-element log-density (z_out / logsd_out: z' / arw_logsd, training only)
   float* hid_out[IAF_MAX_HIDDEN];  // training forward: hidden activations [B][hidden[j]][HW], nullable
   float* partial;          // [B][n_bands][C] per-band per-channel partial sums
   unsigned* counter;       // [B] band arrival counters (self-resetting)
@@ -144,12 +145,15 @@ struct IafSimtParams {
   int band_rows, n_bands;
   int flip;                // 1: data point-reflected on load/store (IafVariantFlags::reflect)
   int nl;
-  int mode;                // 0 multiconv, 1 step, 2 layer
+  int mode;                // 0 multiconv, 1 step, 2 layer, 3 logp
   float scale;             // 0.1
   int bufz_elems, bufa_elems, bufb_elems;
 };
 
-enum { IAF_MODE_MULTICONV = 0, IAF_MODE_STEP = 1, IAF_MODE_LAYER = 2 };
+// IAF_MODE_LOGP: the autoregressive (MADE) prior's log-density at z (models.py:304-309): the step's heads and affine
+// update, then logps = -0.5 log 2pi - arw_logsd - 0.5 z'^2 (rand.py:83 with mean 0.1 m, logvar 2 arw_logsd), summed per
+// (sample, channel) and per sample like the layer mode's kl.
+enum { IAF_MODE_MULTICONV = 0, IAF_MODE_STEP = 1, IAF_MODE_LAYER = 2, IAF_MODE_LOGP = 3 };
 
 // What a call at batch B would do to a set of scratch buffers sized for have_B samples (0: none yet): nothing, a first
 // allocation, or a re-allocation that frees the old buffers.  Sets combine with std::max.

@@ -48,6 +48,8 @@ __device__ __forceinline__ float iaf_apply_nl(float v, int nl) {
     }                                                                             \
   }
 
+// LOGP: the MADE prior's density (IAF_MODE_LOGP), an instantiation of its own so that the other modes' code is untouched
+template <bool LOGP>
 __global__ void __launch_bounds__(IAF_SIMT_THREADS, 2) iaf_simt_kernel(const __grid_constant__ IafSimtParams p) {
   IAF_DYN_SMEM(float, smem);
   float* bufz = smem;
@@ -208,8 +210,14 @@ __global__ void __launch_bounds__(IAF_SIMT_THREADS, 2) iaf_simt_kernel(const __g
             const float arw_logsd = p.scale * o[4 + c];
             const float zv = bufz[(ch * rows_alloc + yl) * P + x + 1];
             const float zn = (zv - arw_mean) / expf(arw_logsd);
-            p.z_out[g] = zn;
-            if (p.mode == IAF_MODE_STEP) {
+            if (!LOGP || p.z_out) p.z_out[g] = zn;
+            if (LOGP) {
+              // models.py:304-309, rand.py:83: N(0.1 m, exp(2 arw_logsd)) at z is the standard normal at z', - arw_logsd
+              const float lp = -0.9189385332046727f - arw_logsd - 0.5f * zn * zn;
+              if (p.logsd_out) p.logsd_out[g] = arw_logsd;
+              if (p.logps_out) p.logps_out[g] = lp;
+              csum[c] += lp;
+            } else if (p.mode == IAF_MODE_STEP) {
               if (p.logsd_out) p.logsd_out[g] = arw_logsd;
               csum[c] += arw_logsd;
             } else {
@@ -248,7 +256,8 @@ __global__ void __launch_bounds__(IAF_SIMT_THREADS, 2) iaf_simt_kernel(const __g
       s_chan[tid] = s;
     }
     __syncthreads();
-    const float sign = (p.mode == IAF_MODE_STEP) ? -1.f : 1.f;  // logdet = -sum(arw_logsd); kl_cost = +sum(kl)
+    // logdet = -sum(arw_logsd); kl_cost = +sum(kl); logp = +sum(logps)
+    const float sign = (p.mode == IAF_MODE_STEP) ? -1.f : 1.f;
     if (p.n_bands == 1) {
       if (p.bc_out && tid < p.head_c) p.bc_out[(size_t)n * p.head_c + tid] = s_chan[tid];
       if (p.persample_out && tid == 0) {
@@ -284,10 +293,12 @@ __global__ void __launch_bounds__(IAF_SIMT_THREADS, 2) iaf_simt_kernel(const __g
 }
 
 cudaError_t iaf_simt_set_smem() {
-  return iaf_smem_optin(iaf_simt_kernel);
+  cudaError_t e = iaf_smem_optin(iaf_simt_kernel<false>);
+  return e != cudaSuccess ? e : iaf_smem_optin(iaf_simt_kernel<true>);
 }
 
 cudaError_t iaf_launch_simt(const IafSimtParams& p, size_t smem_bytes, cudaStream_t stream) {
-  IAF_LAUNCH(iaf_simt_kernel, p.B * p.n_bands, IAF_SIMT_THREADS, smem_bytes, stream, p);
+  if (p.mode == IAF_MODE_LOGP) IAF_LAUNCH(iaf_simt_kernel<true>, p.B * p.n_bands, IAF_SIMT_THREADS, smem_bytes, stream, p);
+  else IAF_LAUNCH(iaf_simt_kernel<false>, p.B * p.n_bands, IAF_SIMT_THREADS, smem_bytes, stream, p);
   return cudaGetLastError();
 }

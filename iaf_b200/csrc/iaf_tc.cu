@@ -55,6 +55,7 @@ struct IafTcParams {
   const float* z; const float* ctx;
   const float* post_mean; const float* post_logsd; const float* prior_mean; const float* prior_logsd;
   float* z_out; float* elem; float* bc_out; float* persample_out;
+  float* logps;              // logp mode: per-element log-density (nullable)
   float* tilepart;           // [NT][MAXS][Cred]
   unsigned* counter;         // [B]
   IafTcStage st[IAF_MAX_STAGES];
@@ -258,7 +259,8 @@ __device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, ui
 // warp (other warps of the role may still be in it).  Role 0, lane 0 of MMA warp 0: 15 / 35 the (hidden) / heads MMAs'
 // operands ready, 20 / 40 their MMAs done, 21 / 41 their fragments in the accumulator tile (after waiting for the
 // epilogues to free it).  Role 1, lane 0 of epilogue warp 0: 10 z window built, 25 / 45 (hidden) / heads accumulators
-// ready, 30 (hidden) epilogue done, 50 heads epilogue done (fused), 99 kernel end.  Role 2, the producer: 60 / 61 before
+// ready, 30 (hidden) epilogue done, 50 heads epilogue done (fused), 98 the launch's mode (k = IAF_MODE_*: multiconv,
+// step, layer, logp), 99 kernel end.  Role 2, the producer: 60 / 61 before
 // / after waiting for a ring stage to be released (k = the weight chunk it will refill).
 #ifdef IAF_TC_TIMELINE
 #define TL_MAX 96
@@ -433,7 +435,8 @@ static LyKernel ly_kernel_pick(bool padw, int mode, bool elu) {
   return elu ? iaf_ly_kernel<false, MD, IAF_NL_ELU, NGW, FUSED> : iaf_ly_kernel<false, MD, -1, NGW, FUSED>;
   if (mode == IAF_MODE_MULTICONV) { LY_PICK(IAF_MODE_MULTICONV) }
   if (mode == IAF_MODE_STEP) { LY_PICK(IAF_MODE_STEP) }
-  LY_PICK(IAF_MODE_LAYER)
+  if (mode == IAF_MODE_LAYER) { LY_PICK(IAF_MODE_LAYER) }
+  LY_PICK(IAF_MODE_LOGP)
 #undef LY_PICK
 }
 // the stage kernel for a stage of N output columns: NGW = ceil(N / 32), an MMA warpgroup's span of 32 NGW columns.  NGW <= 6 (N <=
@@ -552,8 +555,8 @@ int iaf_tc_plan_create(IafTcPlan** out, const iaf_desc_t* d) {
     pl->padw[j] = pl->bias[j] + pl->N[j];
     pl->wsinv[j] = pl->bias[j] + 5 * pl->N[j];
   }
-  for (int a = 0; a < 12; ++a) {
-    const int md = (a >> 2) == 0 ? IAF_MODE_MULTICONV : ((a >> 2) == 1 ? IAF_MODE_STEP : IAF_MODE_LAYER);
+  for (int a = 0; a < 16; ++a) {
+    const int md = a >> 2;  // IAF_MODE_MULTICONV .. IAF_MODE_LOGP
     cudaError_t e = cudaSuccess;
     if (pl->fused) e = iaf_smem_optin(fz_kernel_for(a & 1, md, a & 2));
     for (int j = 0; j < pl->n_stages && e == cudaSuccess && !pl->fused; ++j) e = iaf_smem_optin(ly_kernel_for(a & 1, md, a & 2, pl->N[j]));
@@ -634,7 +637,10 @@ extern "C" void iaf_tc_timeline_dump(void) {
 #endif
 
 bool iaf_tc_mode_supported(const IafTcPlan* pl, int mode) {
-  return mode == IAF_MODE_STEP || mode == IAF_MODE_MULTICONV || (mode == IAF_MODE_LAYER && pl->layer_ok);
+  // the logp mode shares the layer mode's per-(sample, channel) partials and scratch, so it is available exactly where
+  // the layer mode is
+  return mode == IAF_MODE_STEP || mode == IAF_MODE_MULTICONV ||
+         ((mode == IAF_MODE_LAYER || mode == IAF_MODE_LOGP) && pl->layer_ok);
 }
 
 // tiles of a call at batch B (0: the slot stream overflows int)
@@ -687,6 +693,7 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
   p.z_out = a->z_out;
   p.elem = a->elem_out;
   p.bc_out = a->bc_out; p.persample_out = a->persample_out;
+  p.logps = a->logps_out;
   p.tilepart = pl->tilepart;
   p.counter = pl->counter;
   p.n_stages = 1;
@@ -1155,6 +1162,7 @@ struct IafDgStepParams {
   __nv_bfloat16* o_hi; __nv_bfloat16* o_lo;
   int B, C, cp, head_pad, H, W, Wp, SPS, HW, S_pad, S_end, fwd_flip, img_flip;
   float scale;
+  const float* g_logps; const float* g_logp_bc; const float* g_logp;  // LOGP: the MADE prior density's upstream, nullable
 };
 
 // ------------------------------------------------------------------------------------------
@@ -1162,7 +1170,10 @@ struct IafDgStepParams {
 // iaf_dg_image_kernel and the heads' iaf_bwd_bias_kernel do in three passes over [B][2 n_z][HW], in one: a block per sample
 // forms g_m, g_s (models.py:282-285 differentiated) in shared memory, writes the direct term of g_z, the sample's max and
 // scale, its bias / pad-channel column sums, and the scaled operand image of the heads' gradient.
+// LOGP: the MADE prior's density (logps = -0.5 log 2pi - arw_logsd - 0.5 z'^2) with the upstream
+// G = g_logps + g_logp_bc[b,c] + g_logp[b] in place of the step's: g_z' = -z' G, g_arw_logsd = -G.
 // ------------------------------------------------------------------------------------------
+template <bool LOGP>
 __global__ void __launch_bounds__(256) iaf_dg_step_kernel(const __grid_constant__ IafDgStepParams p) {
   extern __shared__ float sg[];  // [cp][HW]
   __shared__ float red[256];
@@ -1186,10 +1197,22 @@ __global__ void __launch_bounds__(256) iaf_dg_step_kernel(const __grid_constant_
     const int c = i / HW, gp = i - c * HW;
     const int mcol = (c >> 2) * 8 + (c & 3), scol = mcol + 4;
     const size_t e = ((size_t)n * p.C + c) * HW + gp;
-    const float ex = expf(-__ldg(p.logsd + e)), zn = __ldg(p.z_out + e), gzo = __ldg(p.g_zout + e);
-    float gs = -p.scale * zn * gzo;
-    if (p.g_logsd) gs += p.scale * __ldg(p.g_logsd + e);
-    gs -= p.scale * gld;
+    float gzo, gs, ex, zn;
+    if (LOGP) {
+      ex = expf(-__ldg(p.logsd + e));
+      zn = __ldg(p.z_out + e);
+      float G = 0.f;
+      if (p.g_logps) G += __ldg(p.g_logps + e);
+      if (p.g_logp_bc) G += __ldg(p.g_logp_bc + (size_t)n * p.C + c);
+      if (p.g_logp) G += __ldg(p.g_logp + n);
+      gzo = -zn * G;
+      gs = -p.scale * zn * gzo - p.scale * G;
+    } else {
+      ex = expf(-__ldg(p.logsd + e)); zn = __ldg(p.z_out + e); gzo = __ldg(p.g_zout + e);
+      gs = -p.scale * zn * gzo;
+      if (p.g_logsd) gs += p.scale * __ldg(p.g_logsd + e);
+      gs -= p.scale * gld;
+    }
     const float gm = -p.scale * ex * gzo;
     sg[mcol * HW + gp] = gm;
     sg[scol * HW + gp] = gs;
@@ -1260,19 +1283,16 @@ bool iaf_dg_step_supported(const IafDgPlan* pl) {
 
 // STEP entry with kept activations: g_z (direct term), per-sample scale, bias sums (-> *bias_partials, [B][5][cp]) and the
 // operand image 0 of the heads' gradient in one launch.  hb (fp32 heads gradient) is optional.
-int iaf_dg_begin_step(IafDgPlan* pl, const float* z_out, const float* logsd, const float* g_zout, const float* g_logsd,
-                      const float* g_logdet, float* g_z, float* hb, int head_pad, int B, cudaStream_t stream,
-                      const float** bias_partials) {
+static int dg_begin_step(IafDgPlan* pl, IafDgStepParams& q, bool logp, float* g_z, float* hb, int head_pad, int B,
+                         cudaStream_t stream, const float** bias_partials) {
   const iaf_desc_t& d = pl->d;
   int st = dg_ensure_scratch(pl, B, stream);
   if (st != IAF_OK) return st;
   if (!pl->step_optin) {
-    if (iaf_smem_optin(iaf_dg_step_kernel) != cudaSuccess) return IAF_ERR_CUDA;
+    if (iaf_smem_optin(iaf_dg_step_kernel<false>) != cudaSuccess) return IAF_ERR_CUDA;
+    if (iaf_smem_optin(iaf_dg_step_kernel<true>) != cudaSuccess) return IAF_ERR_CUDA;
     pl->step_optin = 1;
   }
-  IafDgStepParams q;
-  memset(&q, 0, sizeof(q));
-  q.z_out = z_out; q.logsd = logsd; q.g_zout = g_zout; q.g_logsd = g_logsd; q.g_logdet = g_logdet;
   q.g_z = g_z; q.hb = hb; q.bstep = pl->bstep; q.amax = pl->amax;
   q.o_hi = pl->img[0][0]; q.o_lo = pl->img[0][1];
   q.B = B; q.C = d.n_z; q.cp = pl->kin[pl->n_stages - 1]; q.head_pad = head_pad;
@@ -1282,7 +1302,26 @@ int iaf_dg_begin_step(IafDgPlan* pl, const float* z_out, const float* logsd, con
   q.img_flip = pl->grad_flip;
   q.fwd_flip = q.img_flip ? 0 : 1;
   q.scale = 0.1f;
-  iaf_dg_step_kernel<<<B + 1, 256, (size_t)q.cp * q.HW * 4, stream>>>(q);
+  if (logp) iaf_dg_step_kernel<true><<<B + 1, 256, (size_t)q.cp * q.HW * 4, stream>>>(q);
+  else iaf_dg_step_kernel<false><<<B + 1, 256, (size_t)q.cp * q.HW * 4, stream>>>(q);
   if (bias_partials) *bias_partials = pl->bstep;
   return cudaGetLastError() == cudaSuccess ? IAF_OK : IAF_ERR_CUDA;
+}
+
+int iaf_dg_begin_step(IafDgPlan* pl, const float* z_out, const float* logsd, const float* g_zout, const float* g_logsd,
+                      const float* g_logdet, float* g_z, float* hb, int head_pad, int B, cudaStream_t stream,
+                      const float** bias_partials) {
+  IafDgStepParams q;
+  memset(&q, 0, sizeof(q));
+  q.z_out = z_out; q.logsd = logsd; q.g_zout = g_zout; q.g_logsd = g_logsd; q.g_logdet = g_logdet;
+  return dg_begin_step(pl, q, false, g_z, hb, head_pad, B, stream, bias_partials);
+}
+
+int iaf_dg_begin_step_logp(IafDgPlan* pl, const float* z_out, const float* logsd, const float* g_logps,
+                           const float* g_logp_bc, const float* g_logp, float* g_z, float* hb, int head_pad, int B,
+                           cudaStream_t stream, const float** bias_partials) {
+  IafDgStepParams q;
+  memset(&q, 0, sizeof(q));
+  q.z_out = z_out; q.logsd = logsd; q.g_logps = g_logps; q.g_logp_bc = g_logp_bc; q.g_logp = g_logp;
+  return dg_begin_step(pl, q, true, g_z, hb, head_pad, B, stream, bias_partials);
 }

@@ -5,7 +5,7 @@
 struct IafTcPlan;
 
 struct IafTcArgs {
-  int mode;  // IAF_MODE_STEP | IAF_MODE_LAYER
+  int mode;  // IAF_MODE_MULTICONV | IAF_MODE_STEP | IAF_MODE_LAYER | IAF_MODE_LOGP
   const float* z;  // layer mode: eps
   const float* ctx;
   const float* post_mean;
@@ -16,6 +16,7 @@ struct IafTcArgs {
   float* elem_out;       // arw_logsd | kl, nullable
   float* bc_out;         // [B,C], nullable
   float* persample_out;  // [B], nullable
+  float* logps_out;      // logp mode: per-element log-density, nullable (z_out / elem_out: z' / arw_logsd, nullable)
   float* hid_out[IAF_MAX_HIDDEN];  // training forward: hidden activations [B][hidden[j]][HW], nullable
   int B;
 };
@@ -42,3 +43,8 @@ bool iaf_dg_step_supported(const IafDgPlan* p);
 int iaf_dg_begin_step(IafDgPlan* p, const float* z_out, const float* logsd, const float* g_zout, const float* g_logsd,
                       const float* g_logdet, float* g_z, float* hb, int head_pad, int B, cudaStream_t stream,
                       const float** bias_partials);
+// the same prologue for the MADE prior's density (IAF_MODE_LOGP): the upstream G = g_logps + g_logp_bc[b,c] + g_logp[b]
+// (each nullable) enters as g_z' = -z' G, g_arw_logsd = -G
+int iaf_dg_begin_step_logp(IafDgPlan* p, const float* z_out, const float* logsd, const float* g_logps,
+                           const float* g_logp_bc, const float* g_logp, float* g_z, float* hb, int head_pad, int B,
+                           cudaStream_t stream, const float** bias_partials);

@@ -349,7 +349,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     } else if (warp == LY_RED_WARP && (FUSED || q.is_heads) && (p.persample_out || p.bc_out) && MODE != IAF_MODE_MULTICONV) {
       // ===================== reducer warp: per-tile partials -> per-sample outputs, off the workers' critical path ==========
       float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
-      constexpr bool LAY = (MODE == IAF_MODE_LAYER);
+      constexpr bool LAY = (MODE == IAF_MODE_LAYER || MODE == IAF_MODE_LOGP);  // per-(sample, channel) partials
       for (int i = 0; i < n_my; ++i) {
         const int u = (int)blockIdx.x + i * (int)gridDim.x;
         const int pb = i & 1;
@@ -627,7 +627,9 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       // heads epilogue: affine update, per-element and per-sample outputs
       auto heads_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch, const SlotInfo si) {
           // ---------------- heads: affine update, per-element and per-sample outputs ----------------
-          constexpr int NRED = (MODE == IAF_MODE_LAYER) ? 8 : 1;
+          // layer and logp modes: per-(sample, channel) partials, the 8 channels of a column group apart
+          constexpr bool PERCH = (MODE == IAF_MODE_LAYER || MODE == IAF_MODE_LOGP);
+          constexpr int NRED = PERCH ? 8 : 1;
           float red[NRED];
   #pragma unroll
           for (int k_ = 0; k_ < NRED; ++k_) red[k_] = 0.f;
@@ -640,7 +642,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
           const int n_last = min(p.B - 1, fast_div(tile_s0 + q.TS - 1, p.SPS, p.mg_sps));
           const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
           const int pb = i & 1;
-          if (MODE == IAF_MODE_LAYER && (p.persample_out || p.bc_out) && i >= 2)
+          if (PERCH && (p.persample_out || p.bc_out) && i >= 2)
             mbar_wait(&bars[LB_PART_EMPTY + pb], (uint32_t)(((i >> 1) - 1) & 1));
           for (int g = cg; g < ngroups; g += CGS) {
             const int c0 = g * 16;
@@ -655,7 +657,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             uint32_t r[16];
             acc_ld16(c0, r, pitch, St.wsinv);
             const bool set_hi = ((g - cg) / CGS) & 1;
-            if (MODE == IAF_MODE_LAYER) {
+            if (PERCH) {
   #pragma unroll
               for (int k_ = 0; k_ < NRED; ++k_) red[k_] = 0.f;
             } else {
@@ -687,8 +689,14 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                   z0 = fmaf(fast_exp(pls), eps, __ldg(p.post_mean + ge));
                 }
                 const float zn = (z0 - arw_mean) * fast_exp(-arw_logsd);
-                p.z_out[ge] = zn;
-                if (MODE == IAF_MODE_STEP) {
+                if (MODE != IAF_MODE_LOGP || p.z_out) p.z_out[ge] = zn;
+                if (MODE == IAF_MODE_LOGP) {
+                  // MADE prior (models.py:304-309, rand.py:83): the standard normal at z', - arw_logsd
+                  const float lp = -0.9189385332046727f - arw_logsd - 0.5f * zn * zn;
+                  if (p.elem) p.elem[ge] = arw_logsd;
+                  if (p.logps) p.logps[ge] = lp;
+                  red[e] = lp;
+                } else if (MODE == IAF_MODE_STEP) {
                   if (p.elem) p.elem[ge] = arw_logsd;
                   red[0] += arw_logsd;
                 } else {
@@ -702,11 +710,11 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                 }
               }
             }
-            if (MODE != IAF_MODE_LAYER) {
+            if (!PERCH) {
               if (set_hi) rs1 = red[0];
               else rs0 = red[0];
             }
-            if (MODE == IAF_MODE_LAYER) {
+            if (PERCH) {
               for (int nl_ = 0; nl_ < ns; ++nl_) {
   #pragma unroll
                 for (int e = 0; e < 8; ++e) {
@@ -720,8 +728,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
           }
 
           if (p.persample_out || p.bc_out) {
-            constexpr bool LAY = (MODE == IAF_MODE_LAYER);
-            if (!LAY) {
+            if (!PERCH) {
               if (i >= 2) mbar_wait(&bars[LB_PART_EMPTY + pb], (uint32_t)(((i >> 1) - 1) & 1));
               for (int nl_ = 0; nl_ < ns; ++nl_) {
   #pragma unroll
@@ -769,6 +776,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
 
   __syncthreads();
   if (q.tl_enable) {
+    if (tid == 0) TL(1, 98, MODE);
     if (tid == 0) TL(1, 99, n_my);
     __syncwarp();
     TL_FLUSH

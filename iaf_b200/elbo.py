@@ -206,13 +206,19 @@ class CudaIAFTrain(object):
                                 prior_logsd, context)
 
 
-def stochastic_layer(step, eps, post_mean, post_logsd, prior_mean, prior_logsd, context):
-    """tf_train.py:56-75 around a step callable (z, context) -> (z', arw_logsd): returns (z', kl_bc [B,C], kl_cost [B])."""
+def posterior_sample(step, eps, post_mean, post_logsd, context):
+    """The posterior half of :func:`stochastic_layer`: sample, step, log q -> (z', logqs [B,C,H,W])."""
     c = 0.5 * math.log(2.0 * math.pi)
     z0 = post_mean + torch.exp(post_logsd) * eps                  # DiagonalGaussian.sample, distributions.py:20
     logqs = -c - post_logsd - 0.5 * eps * eps                     # logps of the sample itself: (z0-mean)/sd == eps
     z, arw_logsd = step(z0, context)
-    logqs = logqs + arw_logsd                                      # tf_train.py:72
+    return z, logqs + arw_logsd                                    # tf_train.py:72
+
+
+def stochastic_layer(step, eps, post_mean, post_logsd, prior_mean, prior_logsd, context):
+    """tf_train.py:56-75 around a step callable (z, context) -> (z', arw_logsd): returns (z', kl_bc [B,C], kl_cost [B])."""
+    c = 0.5 * math.log(2.0 * math.pi)
+    z, logqs = posterior_sample(step, eps, post_mean, post_logsd, context)
     logps = -c - prior_logsd - 0.5 * (z - prior_mean) ** 2 * torch.exp(-2.0 * prior_logsd)
     kl = logqs - logps
     return z, kl.sum(dim=(2, 3)), kl.sum(dim=(1, 2, 3))

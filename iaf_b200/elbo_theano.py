@@ -17,6 +17,14 @@ torch ops.  Parameters are a dict under the reference's Theano names (graphy/nod
 sample -> step(conv1) -> step(conv2, reversed order) -> KL with both ``arw_logsd`` in log q, assembled by
 :func:`iaf_b200.elbo.stochastic_layer` around the two calls ``iaf_layer.step(name, z, context, conv)``, conv = 1, 2.
 Any other posterior name raises ``ValueError``.
+
+``prior='made'`` (the autoregressive prior, models.py:36-38, 304-309, 328) is available with all three posteriors:
+down_conv1's prior channels are then ``[h_det n_h2 | made_context n_h2]``, the prior's own masked stack
+``{i}_{j}_prior_conv1_{k}_*`` / ``{i}_{j}_prior_conv1_out_{k}_*`` is evaluated at the posterior's final sample, and
+``kl = logqs - logps_made(z, made_context)``.  The posterior half of the down posteriors is then
+:func:`iaf_b200.elbo.posterior_sample` around ``iaf_layer.step`` (the fused diagonal-prior ``layer`` entry does not
+apply), and the prior's density is the pluggable ``iaf_layer.prior_logp(name, z, context) -> (logp_bc, logp)``.
+``prior='diag'`` is the default; any other prior name (``diag2``, ``bernoulli``, ...) raises ``ValueError``.
 """
 import math
 
@@ -26,6 +34,7 @@ import torch.nn.functional as F
 
 LOGSCALE_SCALE = 3.0  # graphy/nodes/conv.py:19 (conv.py:16-22: logscale=True, bn=False, maxweight=0)
 POSTERIORS = ("down_iaf2_nl", "up_iaf2_nl", "down_iaf2_nl2")
+PRIORS = ("diag", "made")
 
 
 def posterior_of(hps):
@@ -33,6 +42,14 @@ def posterior_of(hps):
     p = hps.get("posterior", "down_iaf2_nl")
     if p not in POSTERIORS:
         raise ValueError("posterior %r is not implemented (available: %s)" % (p, ", ".join(POSTERIORS)))
+    return p
+
+
+def prior_of(hps):
+    """The prior of ``hps`` (default diag); any other reference prior (diag2, bernoulli) is refused, not approximated."""
+    p = hps.get("prior", "diag")
+    if p not in PRIORS:
+        raise ValueError("prior %r is not implemented (available: %s)" % (p, ", ".join(PRIORS)))
     return p
 
 
@@ -118,6 +135,8 @@ def layer_down_q(w, name, h_in, up_state, eps, iaf_layer, hps, downsample):
     ds = 2 if downsample else 1
     h = conv2d(w, name + "_down_conv1", nonlinearity(h_in, nl))
     posterior = posterior_of(hps)
+    if prior_of(hps) == "made":
+        return _layer_down_q_made(w, name, h_in, h, up_state, eps, iaf_layer, hps, downsample)
     if posterior == "up_iaf2_nl":                                      # models.py:215-217, 287-290
         h_det, pz_mean, pz_logsd = torch.split(h, [nh2, nz, nz], dim=1)
         z, logqs = up_state
@@ -151,6 +170,40 @@ def layer_down_q(w, name, h_in, up_state, eps, iaf_layer, hps, downsample):
     return out, kl_bc, kl_sum
 
 
+def _layer_down_q_made(w, name, h_in, h, up_state, eps, iaf_layer, hps, downsample):
+    """down_q with prior='made' (models.py:36-38, 304-309, 328): the posterior's final sample z and its logqs, then
+    kl = logqs - logps_made(z, made_context) with the prior's own masked stack (``iaf_layer.prior_logp``)."""
+    nz, nh2, nl = hps["n_z"], hps["n_h2"], hps["nl"]
+    ds = 2 if downsample else 1
+    posterior = posterior_of(hps)
+    if posterior == "up_iaf2_nl":
+        # channel map: [h_det n_h2 | made_context n_h2]; z and logqs come from the bottom-up pass (models.py:215-217)
+        h_det, made_context = torch.split(h, [nh2, nh2], dim=1)
+        z, logqs = up_state
+    else:
+        # channel map: [h_det n_h2 | made_context n_h2 || rz_mean n_z | rz_logsd n_z | down_context n_h2]
+        h_det, made_context, rz_mean, rz_logsd, down_context = torch.split(h, [nh2, nh2, nz, nz, nh2], dim=1)
+        qz_mean, qz_logsd, up_context = up_state
+        from .elbo import posterior_sample
+        if posterior == "down_iaf2_nl2":
+            def steps(z, c):
+                z, a1 = iaf_layer.step(name, z, c, 1)
+                z, a2 = iaf_layer.step(name, z.contiguous(), c, 2)
+                return z, a1 + a2
+        else:
+            steps = lambda z, c: iaf_layer.step(name, z, c)
+        z, logqs = posterior_sample(steps, eps, (qz_mean + rz_mean).contiguous(), (qz_logsd + rz_logsd).contiguous(),
+                                    (up_context + down_context).contiguous())
+    logp_bc, logp = iaf_layer.prior_logp(name, z.contiguous(), made_context.contiguous())
+    kl_bc = logqs.sum(dim=(2, 3)) - logp_bc
+    kl_sum = logqs.sum(dim=(1, 2, 3)) - logp
+    hh = torch.cat([h_det, z], dim=1)
+    if downsample:
+        h_in = upsample_nn(h_in)
+    out = h_in + 0.1 * conv2d(w, "%s_down_conv2_%d" % (name, ds), nonlinearity(hh, nl), upsample=ds)
+    return out, kl_bc, kl_sum
+
+
 def discretized_logistic_logp(mean, logscale, binsize, sample):
     """graphy/nodes/rand.py:169-178 (.logp)."""
     scale = torch.exp(logscale)
@@ -164,6 +217,7 @@ def forward(w, x_uint8, noise, iaf_layer, hps):
     image_size.  noise[(i, j)]: the N(0,1) draw of layer (i, j).  Returns the reference's ``results`` entries plus
     bits_per_dim (= mean of ``cost``, what train.py reports)."""
     depths, nl = hps["depths"], hps["nl"]
+    prior_of(hps)
     dt = w["h_top"].dtype
     x = torch.clamp((x_uint8.to(dt) + 0.5) / 256.0, 0.0, 1.0)      # models.py:425
     B = x.shape[0]
@@ -202,6 +256,7 @@ def make_params(hps, seed=0, dtype=np.float32):
     nz, nh1, nh2, depths = hps["n_z"], hps["n_h1"], hps["n_h2"], hps["depths"]
     posterior = posterior_of(hps)
     up_post = posterior == "up_iaf2_nl"
+    made = prior_of(hps) == "made"
     w = {}
 
     def conv(name, cin, cout, k, pad_channel=True):
@@ -219,7 +274,8 @@ def make_params(hps, seed=0, dtype=np.float32):
             ds = 2 if (i > 0 and j == 0) else 1
             conv("%s_up_conv1_%d" % (n, ds), nh1, nh2 + 2 * nz + nh2, 3)
             conv(n + "_up_conv2", nh2 + nz if up_post else nh2, nh1, 3)                       # models.py:25,84
-            conv(n + "_down_conv1", nh1, (nh2 + 2 * nz) + (0 if up_post else 2 * nz + nh2), 3)  # models.py:27-28,86
+            conv(n + "_down_conv1", nh1, (2 * nh2 if made else nh2 + 2 * nz) + (0 if up_post else 2 * nz + nh2),
+                 3)                                                    # models.py:27-28,36-38,86
             conv("%s_down_conv2_%d" % (n, ds), nh2 + nz, nh1 * ds * ds, 3)
             sizes = [nz] + hps["depth_ar"] * [nh2]
             for k in range(hps["depth_ar"]):
@@ -231,6 +287,11 @@ def make_params(hps, seed=0, dtype=np.float32):
                     conv("%s_posterior_conv2_%d" % (n, k), sizes[k], sizes[k + 1], 3)
                 for k in range(2):
                     conv("%s_posterior_conv2_out_%d" % (n, k), sizes[-1], nz, 3)
+            if made:                                                   # models.py:36-38
+                for k in range(hps["depth_ar"]):
+                    conv("%s_prior_conv1_%d" % (n, k), sizes[k], sizes[k + 1], 3)
+                for k in range(2):
+                    conv("%s_prior_conv1_out_%d" % (n, k), sizes[-1], nz, 3)
     return w
 
 
@@ -241,11 +302,27 @@ class CudaIAF(object):
     def __init__(self, w, hps, path="auto"):
         from .ops import IAFOperator
         self.w, self.hps, self.path, self.IAFOperator, self.ops = w, hps, path, IAFOperator, {}
+        self.prior_ops = {}  # prior='made': layer name -> the prior's operator (prior_conv1, models.py:36-38)
 
     def _new_op(self, conv):
         nz, nh2, dar = self.hps["n_z"], self.hps["n_h2"], self.hps["depth_ar"]
         return self.IAFOperator("theano", nz, dar * [nh2], [nz, nz], nl=self.hps["nl"], path=self.path,
-                                flipmask=conv == 2)                    # models.py:92,97-98
+                                flipmask=conv == 2)                    # models.py:36-38,92,97-98 (conv 0: the prior)
+
+    def _prior_op(self, name, device):
+        op = self.prior_ops.get(name)
+        if op is None:
+            from .weights import theano_layers
+            op = self._new_op(0)
+            op.set_weights(theano_layers(self.w, "%s_prior_conv1" % name, self.hps["depth_ar"], device=device))
+            self.prior_ops[name] = op
+        return op
+
+    def prior_logp(self, name, z, context):
+        """prior='made': log-density of the autoregressive prior at the posterior's final sample z with the context
+        made_context (models.py:304-309), summed per (sample, channel) and per sample -> (logp_bc [B,C], logp [B])."""
+        _, logp_bc, logp = self._prior_op(name, z.device).ar_logp(z, context)
+        return logp_bc, logp
 
     def _op(self, name, device, conv=1):
         op = self.ops.get((name, conv))
@@ -260,6 +337,7 @@ class CudaIAF(object):
         """The inference wrapper converts ``w`` (numpy or torch) to device tensors ONCE per layer; after changing or
         replacing entries of ``w`` call this so the next evaluation re-imports and re-packs them."""
         self.ops.clear()
+        self.prior_ops.clear()
         return self
 
     def __call__(self, name, eps, post_mean, post_logsd, prior_mean, prior_logsd, context):
@@ -289,6 +367,17 @@ class CudaIAFTrain(CudaIAF):
         pre = "%s_posterior_conv%d" % (name, conv)
         names = ["%s_%d" % (pre, i) for i in range(dar)] + ["%s_out_%d" % (pre, k) for k in range(2)]
         # the live tensors of w (float32, on the device): not detached, so their .grad is filled by backward()
+        op.set_weights([(self.w[n + "_w"], self.w[n + "_s"], self.w[n + "_b"]) for n in names])
+        return op
+
+    def _prior_op(self, name, device):
+        op = self.prior_ops.get(name)
+        if op is None:
+            op = self._new_op(0)
+            self.prior_ops[name] = op
+        pre, dar = "%s_prior_conv1" % name, self.hps["depth_ar"]
+        names = ["%s_%d" % (pre, i) for i in range(dar)] + ["%s_out_%d" % (pre, k) for k in range(2)]
+        # the live tensors of w, as for the posterior convs: IAFOperator.ar_logp records one autograd node
         op.set_weights([(self.w[n + "_w"], self.w[n + "_s"], self.w[n + "_b"]) for n in names])
         return op
 

@@ -10,6 +10,8 @@ is in libiaf_b200.so (include/iaf_b200.h).  Three entry points mirror the refere
 * ``iaf_step(z, context, ...)`` -- the fused superset: the stack plus the caller's
       ``arw_mean*=.1; arw_logsd*=.1; z=(z-arw_mean)/exp(arw_logsd); logqs+=arw_logsd``
       (models.py:282-285, tf_train.py:70-72)
+* ``IAFOperator.ar_logp(z, context)`` -- the autoregressive (MADE) prior's log-density, the same stack with the
+      density epilogue of models.py:304-309 (prior='made')
 
 Both reference functions are graph builders called once; here they run eagerly per batch,
 so the masked / normalised / packed weights are cached on the operator and re-packed only
@@ -176,7 +178,7 @@ class IAFOperator(object):
     # ---- introspection --------------------------------------------------------------
     def path_used(self, H, W, device, entry=None):
         """Kernel family this operator runs on for (H, W): "tc" or "simt".  With ``entry`` ("step" | "multiconv" |
-        "layer") the answer is for THAT entry point: an ``path="auto"`` operator may serve one entry on the SIMT kernel
+        "layer" | "ar_logp") the answer is for THAT entry point: an ``path="auto"`` operator may serve one entry on the SIMT kernel
         although the plan is a tensor-core plan (e.g. ``layer`` when its scratch does not fit); ``path="tc"`` operators
         raise NotImplementedError from such a call instead of slowing down 10-40x."""
         plan = self._plan(H, W, torch.device(device))
@@ -346,12 +348,52 @@ class IAFOperator(object):
                                                _stream(eps.device)))
         return z_out, kl, kl_bc, kl_cost
 
+    def ar_logp(self, z, context, want_logps=False):
+        """Log-density of the autoregressive (MADE) prior at z, with this operator as the prior's stack
+        ``prior_conv1 = multiconv2d(name+'_prior_conv1', n_z, depth_ar*[n_h2], [n_z,n_z], ...)`` (models.py:36-38) and
+        ``context`` its made_context: ``made_mean, made_logsd = .1 * prior_conv1(z, made_context)``, ``logps =
+        gaussian_diag(made_mean, 2*made_logsd, z).logps`` (models.py:304-309, rand.py:83), in one fused entry.
+        Returns (logps [B,C,H,W] or None, logp_bc [B,C] = sum over (h,w), logp [B]).  Differentiable: when an input or a
+        parameter requires grad the call is ONE autograd node (forward iaf_ar_logp_fwd_train, backward
+        iaf_ar_logp_bwd_saved)."""
+        if self._needs_grad(z, context):
+            self.invalidate()  # training: parameters may have been stepped through .data since the last call
+            flat = [t for l in self._layers for t in l]
+            logps, logp_bc, logp = _ArLogpFn.apply(self, z, context if self.hidden else None, *flat)
+            return (logps if want_logps else None), logp_bc, logp
+        return self._ar_logp_raw(z, context, want_logps)
+
+    def _ar_logp_raw(self, z, context, want_logps=False):
+        z, context, B, H, W = self._shapes(z, context)
+        plan = self._plan(H, W, z.device)
+        logps = torch.empty_like(z) if want_logps else None
+        logp_bc = torch.empty((B, self.n_z), device=z.device, dtype=torch.float32)
+        logp = torch.empty((B,), device=z.device, dtype=torch.float32)
+        with torch.cuda.device(z.device):
+            _lib.check(self._lib.iaf_ar_logp_fwd(plan, _ptr(z), _ptr(context), _ptr(logps), _ptr(logp_bc), _ptr(logp), B,
+                                                 _stream(z.device)))
+        return logps, logp_bc, logp
+
+    def _ar_logp_train_raw(self, z, context):
+        """iaf_ar_logp_fwd_train: the density plus z', made_logsd and the hidden activations its backward needs."""
+        z, context, B, H, W = self._shapes(z, context)
+        plan = self._plan(H, W, z.device)
+        logps, z_out, logsd = torch.empty_like(z), torch.empty_like(z), torch.empty_like(z)
+        logp_bc = torch.empty((B, self.n_z), device=z.device, dtype=torch.float32)
+        logp = torch.empty((B,), device=z.device, dtype=torch.float32)
+        hidden = [torch.empty((B, h, H, W), device=z.device, dtype=torch.float32) for h in self.hidden]
+        harr = (C.c_void_p * max(1, len(hidden)))(*[h.data_ptr() for h in hidden])
+        with torch.cuda.device(z.device):
+            _lib.check(self._lib.iaf_ar_logp_fwd_train(plan, _ptr(z), _ptr(context), _ptr(logps), _ptr(logp_bc), _ptr(logp),
+                                                       _ptr(z_out), _ptr(logsd), harr, B, _stream(z.device)))
+        return logps, logp_bc, logp, z_out, logsd, hidden
+
     # ---- backward (SURVEY 8f-4) -------------------------------------------------------
     def _backward(self, kind, z, context, layers, grads_out, need_params, saved=None):
-        """Shared driver of iaf_step_bwd / iaf_step_bwd_saved / iaf_multiconv_bwd.  ``layers`` are the parameter
-        tensors the forward used; ``saved`` = (z_out, logsd, [hidden]) kept by iaf_step_fwd_train (then ``context``
-        is only a shape template for its gradient).  Returns (g_z, g_context or None, [g_w], [g_scale], [g_bias])
-        (lists None when not needed)."""
+        """Shared driver of iaf_step_bwd / iaf_step_bwd_saved / iaf_multiconv_bwd / iaf_ar_logp_bwd_saved.  ``layers``
+        are the parameter tensors the forward used; ``saved`` = (z_out, logsd, [hidden]) kept by iaf_step_fwd_train or
+        iaf_ar_logp_fwd_train (then ``context`` is only a shape template for its gradient).  Returns (g_z, g_context or
+        None, [g_w], [g_scale], [g_bias]) (lists None when not needed)."""
         z, context, B, H, W = self._shapes(z, context)
         dev = z.device
         plan = self._plan(H, W, dev, layers)
@@ -364,7 +406,15 @@ class IAFOperator(object):
             gw, gs, gb = ([torch.empty_like(l[j]) for l in layers] for j in range(3))
         pa = lambda ts: arr(ts) if ts is not None else None
         with torch.cuda.device(dev):
-            if kind == "step":
+            if kind == "ar_logp":
+                g_logps, g_logp_bc, g_logp = (None if t is None else _check_input(t, "grad") for t in grads_out)
+                z_out, logsd, hidden = saved
+                harr = (C.c_void_p * max(1, len(hidden)))(*[h.data_ptr() for h in hidden])
+                _lib.check(self._lib.iaf_ar_logp_bwd_saved(plan, _ptr(z), _ptr(z_out), _ptr(logsd), harr,
+                                                           arr([l[0] for l in layers]), arr([l[1] for l in layers]),
+                                                           _ptr(g_logps), _ptr(g_logp_bc), _ptr(g_logp), _ptr(g_z),
+                                                           _ptr(g_ctx), pa(gw), pa(gs), pa(gb), B, _stream(dev)))
+            elif kind == "step":
                 g_zout, g_logsd, g_logdet = grads_out
                 if g_zout is None:
                     g_zout = torch.zeros_like(z)
@@ -439,6 +489,36 @@ class _StepFn(torch.autograd.Function):
         need_params = any(ctx.needs_input_grad[3:])
         g_z, g_ctx, gw, gs, gb = ctx.op._backward("step", z, context, _regroup(flat), (g_zout, g_logsd, g_logdet), need_params,
                                                    saved=(z_out, logsd, hidden))
+        return (None, g_z, g_ctx) + tuple(_flat_param_grads(gw, gs, gb, len(flat) // 3))
+
+
+class _ArLogpFn(torch.autograd.Function):
+    """autograd node of the MADE prior's density: forward = iaf_ar_logp_fwd_train (z', made_logsd and the hidden
+    activations kept by the same kernels), backward = iaf_ar_logp_bwd_saved (no recompute)."""
+
+    @staticmethod
+    def forward(ctx, op, z, context, *flat):
+        with torch.no_grad():
+            logps, logp_bc, logp, z_out, logsd, hidden = op._ar_logp_train_raw(z, context)
+        ctx.op = op
+        ctx.has_ctx = context is not None
+        ctx.n_hidden = len(hidden)
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(z, *([context] if context is not None else []), z_out, logsd, *hidden, *flat)
+        return logps, logp_bc, logp
+
+    @staticmethod
+    def backward(ctx, g_logps, g_logp_bc, g_logp):
+        saved = ctx.saved_tensors
+        z = saved[0]
+        context = saved[1] if ctx.has_ctx else None
+        i = 2 if ctx.has_ctx else 1
+        z_out, logsd = saved[i], saved[i + 1]
+        hidden = list(saved[i + 2:i + 2 + ctx.n_hidden])
+        flat = saved[i + 2 + ctx.n_hidden:]
+        need_params = any(ctx.needs_input_grad[3:])
+        g_z, g_ctx, gw, gs, gb = ctx.op._backward("ar_logp", z, context, _regroup(flat), (g_logps, g_logp_bc, g_logp),
+                                                   need_params, saved=(z_out, logsd, hidden))
         return (None, g_z, g_ctx) + tuple(_flat_param_grads(gw, gs, gb, len(flat) // 3))
 
 

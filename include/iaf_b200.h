@@ -216,6 +216,34 @@ int iaf_layer_bwd(iaf_plan_t* plan, const float* eps, const float* post_mean, co
                   float* g_context, float* const* g_w, float* const* g_scale, float* const* g_bias, int B,
                   void* stream);
 
+/*
+ * The autoregressive (MADE) prior of the Theano front-end, cvae_layer(..., prior='made', ...), fused: the prior's own
+ * masked stack, of the posterior step's shape and mask order,
+ *   prior_conv1 = multiconv2d(name+'_prior_conv1', n_z, depth_ar*[n_h2], [n_z,n_z], kernel, False, nl, w)  models.py:36-38
+ * run at the posterior's final sample z with the context made_context (models.py:304-309), and its log-density
+ *   made_mean*=.1; made_logsd*=.1; logps = gaussian_diag(made_mean, 2*made_logsd, z).logps
+ *   = -0.5 log 2pi - made_logsd - 0.5 u^2,  u = (z - made_mean) exp(-made_logsd)            rand.py:83
+ * (u is the step's z').  cvae_layer's kl is logqs - logps (models.py:328).
+ * logps_out [B,n_z,H,W]; logp_bc_out [B,n_z] = sum_{h,w} logps (what the free-bits term consumes); logp_out [B] =
+ * sum_{c,h,w} logps.  Each may be NULL; the sums are fixed-order (deterministic).  Needs n_heads == 2 and
+ * head[0] == head[1] == n_z, as iaf_step_fwd.  A tensor-core plan serves it where it serves iaf_layer_fwd.
+ */
+int iaf_ar_logp_fwd(iaf_plan_t* plan, const float* z, const float* context, float* logps_out,
+                    float* logp_bc_out, float* logp_out, int B, void* stream);
+/* Training pair, as iaf_step_fwd_train / iaf_step_bwd_saved: the forward also writes z_out = u and logsd_out =
+ * made_logsd [B,n_z,H,W] and the hidden activations hidden_out[j] (all required); the backward takes them instead of
+ * recomputing the stack.  Upstream gradients g_logps [B,n_z,H,W], g_logp_bc [B,n_z], g_logp [B] (each may be NULL: a
+ * missing one contributes nothing).  Outputs and their NULL rules as iaf_step_bwd_saved: g_z [B,n_z,H,W] (the gradient
+ * through both the stack and the affine update), g_context, g_w / g_scale / g_bias. */
+int iaf_ar_logp_fwd_train(iaf_plan_t* plan, const float* z, const float* context, float* logps_out,
+                          float* logp_bc_out, float* logp_out, float* z_out, float* logsd_out,
+                          float* const* hidden_out, int B, void* stream);
+int iaf_ar_logp_bwd_saved(iaf_plan_t* plan, const float* z, const float* z_out, const float* logsd,
+                          const float* const* hidden, const float* const* w, const float* const* scale,
+                          const float* g_logps, const float* g_logp_bc, const float* g_logp, float* g_z,
+                          float* g_context, float* const* g_w, float* const* g_scale, float* const* g_bias,
+                          int B, void* stream);
+
 /* Backward of the un-fused operator iaf_multiconv_fwd: g_outs[k] [B,head[k],H,W] is the
  * gradient at head k.  Same outputs as iaf_step_bwd. */
 int iaf_multiconv_bwd(iaf_plan_t* plan, const float* z, const float* context, const float* const* w,
@@ -232,7 +260,7 @@ int iaf_plan_path(const iaf_plan_t* plan);      /* iaf_path actually selected (S
  * cannot take for this shape (e.g. the fused layer's per-(sample, channel) scratch does not fit next to the resident
  * weights) on the exact-fp32 SIMT kernel -- 10-40x slower -- and says so here; a plan created with IAF_PATH_TC never
  * downgrades: that entry returns IAF_ERR_UNSUPPORTED, and so does this function. */
-typedef enum { IAF_ENTRY_MULTICONV = 0, IAF_ENTRY_STEP = 1, IAF_ENTRY_LAYER = 2 } iaf_entry;
+typedef enum { IAF_ENTRY_MULTICONV = 0, IAF_ENTRY_STEP = 1, IAF_ENTRY_LAYER = 2, IAF_ENTRY_AR_LOGP = 3 } iaf_entry;
 int iaf_plan_path_for_entry(const iaf_plan_t* plan, int entry);
 /* Which kernels the plan's BACKWARD entries run (creates the backward plan on first use): 0 = exact-fp32 SIMT kernels,
  * 1 = data gradient on the tensor cores, 2 = data and weight gradient on the tensor cores (plans whose forward is on the
