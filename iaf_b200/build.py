@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libiaf_b200.so")
-SOURCES = ["iaf_capi.cu", "iaf_pack.cu", "iaf_simt.cu", "iaf_tc.cu", "iaf_bwd.cu"]
+SOURCES = ["iaf_capi.cu", "iaf_pack.cu", "iaf_simt.cu", "iaf_tc.cu", "iaf_bwd.cu", "iaf_inv.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 

@@ -5,6 +5,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <vector>
 
 #include "iaf_common.h"
 #include "iaf_tc.h"
@@ -35,6 +36,8 @@ long long centre_nnz(int cin, int cout, int zd, int flipmask) {
 }
 
 }  // namespace
+
+IafInvKernel iaf_inv = {nullptr, nullptr};  // (filled in by iaf_inv.cu)
 
 struct iaf_plan {
   iaf_desc_t d;
@@ -84,6 +87,15 @@ struct iaf_plan {
   // a call of this plan has been captured into a CUDA graph: the graph keeps the scratch pointers it saw, so from then on
   // no scratch may be freed or replaced (see capture_guard)
   bool captured;
+  // inverse of the step (iaf_step_inverse): the per-stage "final after z channel step k" table (built on the host at
+  // plan creation, uploaded by iaf_pack_weights) and the kernel's shared-memory layout
+  int* inv_tab_host;
+  int* inv_tab;
+  int inv_tab_n;
+  int inv_grp_off[IAF_MAX_HIDDEN];
+  int inv_ring_off[IAF_MAX_STAGES], inv_acc_off[IAF_MAX_STAGES], inv_lds_off, inv_smem_floats, inv_units;
+  size_t inv_smem;
+  bool inv_ok;
 };
 #define IAF_NSLOT 3
 
@@ -110,6 +122,60 @@ static bool simt_geometry(iaf_plan* pl, int band_rows, size_t* smem_out) {
   pl->P = P;
   pl->bufz = bufz; pl->bufa = bufa; pl->bufb = bufb; pl->tilepart = tilepart;
   pl->smem = smem;
+  return true;
+}
+
+// The inverse's tables and window (iaf_inv.cu).  z channel c is solved at step pos(c) of a pixel: c ascending, or
+// descending with flipmask.  A hidden unit becomes final at the latest step among its live centre inputs (iaf_tap_rule),
+// -1 when it has none; every live centre input of head c must be final before step pos(c), which is what makes the order
+// the mask's.  Returns false, leaving inv_ok unset, when the plan has no step (two heads of n_z) or the window does not
+// fit in shared memory: iaf_step_inverse then refuses.
+static bool inv_tables(iaf_plan* pl) {
+  const iaf_desc_t& d = pl->d;
+  if (d.n_heads != 2 || d.head[0] != d.n_z) return false;
+  const int C = d.n_z, L = d.n_hidden, fm = pl->vf.flipmask;
+  std::vector<int> prev(C), cur, tab;
+  for (int c = 0; c < C; ++c) prev[c] = fm ? C - 1 - c : c;
+  for (int j = 0; j < L; ++j) {
+    const int cin = pl->cin[j], cout = pl->cout[j];
+    cur.assign(cout, -1);
+    for (int co = 0; co < cout; ++co)
+      for (int ci = 0; ci < cin; ++ci)
+        if (iaf_tap_rule(0, ci, co, cin, cout, 0, fm).live) cur[co] = std::max(cur[co], prev[ci]);
+    // offsets of the groups of step -1 .. C-1, then the units, grouped by step (counting sort)
+    pl->inv_grp_off[j] = (int)tab.size();
+    std::vector<int> off(C + 2, 0);
+    for (int co = 0; co < cout; ++co) off[cur[co] + 2] += 1;
+    for (int g = 1; g < C + 2; ++g) off[g] += off[g - 1];
+    std::vector<int> units(cout), fill(off.begin(), off.end() - 1);
+    for (int co = 0; co < cout; ++co) units[fill[cur[co] + 1]++] = co;
+    tab.insert(tab.end(), off.begin(), off.end());
+    tab.insert(tab.end(), units.begin(), units.end());
+    prev = cur;
+  }
+  const int cin = pl->cin[L];
+  for (int co = 0; co < C; ++co)
+    for (int ci = 0; ci < cin; ++ci)
+      if (iaf_tap_rule(0, ci, co, cin, C, 1, fm).live && prev[ci] >= (fm ? C - 1 - co : co)) return false;
+  // shared memory: per stage a two-row ring of its input and its accumulators, then the per-channel sums
+  int o = 0, units = 0;
+  for (int j = 0; j < pl->n_stages; ++j) {
+    pl->inv_ring_off[j] = o; o += pl->cin[j] * 2 * (d.W + 2);
+  }
+  for (int j = 0; j < pl->n_stages; ++j) {
+    pl->inv_acc_off[j] = o; o += pl->cout_pad[j]; units += pl->cout_pad[j];
+  }
+  pl->inv_lds_off = o; o += C;
+  pl->inv_smem_floats = o;
+  pl->inv_units = units;
+  pl->inv_smem = sizeof(float) * (size_t)o;
+  if (pl->inv_smem > 225 * 1024) return false;  // the SIMT kernel's limit (iaf_plan_create)
+  if (!tab.empty()) {
+    pl->inv_tab_host = (int*)malloc(sizeof(int) * tab.size());
+    if (!pl->inv_tab_host) return false;
+    memcpy(pl->inv_tab_host, tab.data(), sizeof(int) * tab.size());
+  }
+  pl->inv_tab_n = (int)tab.size();
   return true;
 }
 
@@ -299,6 +365,16 @@ int iaf_plan_create(iaf_plan_t** out, const iaf_desc_t* desc) {
     cudaError_t e = iaf_simt_set_smem();
     if (e != cudaSuccess) { iaf_plan_destroy(pl); return cuda_fail(e, "cudaFuncSetAttribute(simt smem)"); }
   }
+  if (iaf_inv.launch && inv_tables(pl)) {
+    if (pl->inv_tab_n > 0 && cudaMalloc(&pl->inv_tab, sizeof(int) * pl->inv_tab_n) != cudaSuccess) {
+      cudaError_t e = cudaGetLastError();
+      iaf_plan_destroy(pl);
+      return cuda_fail(e, "cudaMalloc(inverse tables)");
+    }
+    cudaError_t e = iaf_inv.set_smem();
+    if (e != cudaSuccess) { iaf_plan_destroy(pl); return cuda_fail(e, "cudaFuncSetAttribute(inverse smem)"); }
+    pl->inv_ok = true;
+  }
   *out = pl;
   return IAF_OK;
 }
@@ -312,6 +388,8 @@ void iaf_plan_destroy(iaf_plan_t* pl) {
   }
   if (pl->partial) cudaFree(pl->partial);
   if (pl->counter) cudaFree(pl->counter);
+  if (pl->inv_tab) cudaFree(pl->inv_tab);
+  free(pl->inv_tab_host);
   float* st[] = {pl->st_z, pl->st_ctx, pl->st_zo, pl->st_ls, pl->st_ld};
   for (float* q : st) if (q) cudaFree(q);
   for (int i = 0; i < IAF_NSLOT; ++i) {
@@ -369,6 +447,7 @@ int iaf_pack_weights(iaf_plan_t* pl, const float* const* w, const float* const* 
     L.col0 = is_head ? 4 * (i - d.n_hidden) : 0;
     max_cout = std::max(max_cout, L.cout);
   }
+  if (pl->inv_tab) CK(cudaMemcpyAsync(pl->inv_tab, pl->inv_tab_host, sizeof(int) * pl->inv_tab_n, cudaMemcpyHostToDevice, stream));
   CK(iaf_launch_pack(pp, max_cout, stream));
   pl->launches += 1;
   if (pl->tc) {
@@ -495,6 +574,44 @@ int iaf_ar_logp_fwd_train(iaf_plan_t* pl, const float* z, const float* context, 
   if (pl->d.n_heads != 2 || pl->d.head[0] != pl->d.n_z) return IAF_ERR_BAD_SHAPE;
   return run(pl, IAF_MODE_LOGP, z, context, nullptr, nullptr, nullptr, nullptr, z_out, logsd_out, nullptr, nullptr,
              logp_bc_out, logp_out, B, (cudaStream_t)stream, hidden_out, logps_out);
+}
+
+// The inverse of iaf_step_fwd (iaf_inv.cu).  Every plan runs it on the one kernel: there is no tensor-core variant.
+int iaf_step_inverse(iaf_plan_t* pl, const float* u, const float* context, float* z_out, float* logsd_out,
+                     float* logdet_out, int B, void* stream_) {
+  if (!pl || !u || !z_out) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_hidden > 0 && !context) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_heads != 2 || pl->d.head[0] != pl->d.n_z) return IAF_ERR_BAD_SHAPE;
+  if (!pl->packed) return IAF_ERR_NOT_PACKED;
+  if (B <= 0) return IAF_ERR_BAD_ARG;
+  if (!pl->inv_ok) return IAF_ERR_UNSUPPORTED;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  { int cg = capture_guard(pl, stream, IAF_SCRATCH_FITS); if (cg != IAF_OK) return cg; }  // it has no scratch
+  { int hs = stream_handoff(pl, stream); if (hs != IAF_OK) return hs; }
+  const iaf_desc_t& d = pl->d;
+  IafInvParams p;
+  memset(&p, 0, sizeof(p));
+  p.u = u; p.ctx = context; p.z_out = z_out; p.logsd_out = logsd_out; p.logdet_out = logdet_out;
+  p.grp = pl->inv_tab;
+  for (int j = 0; j < d.n_hidden; ++j) p.grp_off[j] = pl->inv_grp_off[j];
+  for (int j = 0; j < pl->n_stages; ++j) {
+    p.stage[j].w = pl->w[j];
+    p.stage[j].bias = pl->bias[j];
+    p.stage[j].padw = pl->vf.pad_channel ? pl->padw[j] : nullptr;
+    p.stage[j].cin = pl->cin[j];
+    p.stage[j].cout = pl->cout[j];
+    p.stage[j].cout_pad = pl->cout_pad[j];
+    p.ring_off[j] = pl->inv_ring_off[j];
+    p.acc_off[j] = pl->inv_acc_off[j];
+  }
+  p.lds_off = pl->inv_lds_off; p.smem_floats = pl->inv_smem_floats;
+  p.n_stages = pl->n_stages; p.n_units = pl->inv_units;
+  p.C = d.n_z; p.H = d.H; p.W = d.W;
+  p.flip = pl->vf.reflect; p.descending = pl->vf.flipmask;
+  p.nl = d.nl; p.scale = 0.1f;
+  CK(iaf_inv.launch(p, B, pl->inv_smem, stream));
+  pl->launches += 1;
+  return IAF_OK;
 }
 
 // iaf_step_bwd on a tensor-core plan recomputes z', arw_logsd and the activations with the forward's own kernels

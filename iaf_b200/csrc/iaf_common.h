@@ -111,6 +111,18 @@ __host__ __device__ __forceinline__ size_t iaf_raw_index(int theano, int k, int 
   return theano ? ((size_t)co * (cin + 1) + ci) * 9 + k : ((size_t)k * cin + ci) * cout + co;
 }
 
+// the hidden layers' nonlinearity (iaf_nl), as the SIMT step and the inverse apply it
+__device__ __forceinline__ float iaf_apply_nl(float v, int nl) {
+  switch (nl) {
+    case IAF_NL_ELU: return v < 0.f ? expm1f(v) : v;                       // nodes/__init__.py:174
+    case IAF_NL_SOFTPLUS: return v > 0.f ? v + log1pf(expf(-v)) : log1pf(expf(v));
+    case IAF_NL_RELU: return v >= 0.f ? v : 0.f;                            // h*(h>=0)
+    case IAF_NL_TANH: return tanhf(v);
+    case IAF_NL_LEAKYRELU: return v < 0.f ? 0.01f * v : v;
+    default: return v;
+  }
+}
+
 // One conv stage as the SIMT kernel sees it (weights already masked, normalised, scaled).
 struct IafStageDev {
   const float* w;     // [5][cin][cout_pad], cout contiguous (heads: see iaf_pack.cu for the column order)
@@ -195,6 +207,37 @@ struct IafPackParams {
   IafVariantFlags vf;
 };
 
+// The inverse of the step (iaf_inv.cu): one CTA per sample walks the canonical frame in reverse raster order and, within
+// a pixel, the z channels in the mask's order.  Shared memory: per stage, a two-row ring of its input [cin][2][W+2]
+// (columns -1 and W and the row below the map stay zero), the stage's accumulators [cout_pad], and the per-channel
+// sums of arw_logsd [C].
+struct IafInvParams {
+  const float* u;          // [B,C,H,W]
+  const float* ctx;        // [B,hidden0,H,W]
+  float* z_out;
+  float* logsd_out;        // nullable
+  float* logdet_out;       // nullable
+  // per hidden stage j: grp[grp_off[j] + g], g = 0..C+1, is where the units of stage j that become final after z
+  // channel step g-1 start (step -1: before any channel), and grp[grp_off[j] + C + 2 + i] lists the units in that order
+  const int* grp;
+  int grp_off[IAF_MAX_HIDDEN];
+  IafStageDev stage[IAF_MAX_STAGES];
+  int ring_off[IAF_MAX_STAGES], acc_off[IAF_MAX_STAGES], lds_off, smem_floats;
+  int n_stages, n_units;   // n_units = sum of cout_pad
+  int C, H, W;
+  int flip;                // IafVariantFlags::reflect
+  int descending;          // the channel order: C-1 .. 0 (flipmask) or 0 .. C-1
+  int nl;
+  float scale;             // 0.1
+};
+
 cudaError_t iaf_launch_pack(const IafPackParams& p, int max_cout, cudaStream_t stream);
+// The inverse's launcher and shared-memory opt-in.  iaf_inv.cu fills them in when it is linked in; the C ABI also builds
+// without it (tests/test_emu_kernels.py's sanitizer build), and then iaf_step_inverse refuses with IAF_ERR_UNSUPPORTED.
+struct IafInvKernel {
+  cudaError_t (*launch)(const IafInvParams& p, int B, size_t smem_bytes, cudaStream_t stream);
+  cudaError_t (*set_smem)();
+};
+extern IafInvKernel iaf_inv;
 cudaError_t iaf_launch_simt(const IafSimtParams& p, size_t smem_bytes, cudaStream_t stream);
 cudaError_t iaf_simt_set_smem();

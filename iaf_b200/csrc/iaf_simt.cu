@@ -24,17 +24,6 @@
 #define IAF_CT 8   // output channels per thread tile
 #define IAF_SIMT_THREADS 256
 
-__device__ __forceinline__ float iaf_apply_nl(float v, int nl) {
-  switch (nl) {
-    case IAF_NL_ELU: return v < 0.f ? expm1f(v) : v;                       // nodes/__init__.py:174
-    case IAF_NL_SOFTPLUS: return v > 0.f ? v + log1pf(expf(-v)) : log1pf(expf(v));
-    case IAF_NL_RELU: return v >= 0.f ? v : 0.f;                            // h*(h>=0)
-    case IAF_NL_TANH: return tanhf(v);
-    case IAF_NL_LEAKYRELU: return v < 0.f ? 0.01f * v : v;
-    default: return v;
-  }
-}
-
 #define IAF_TAP(T, A, OFF)                                                        \
   {                                                                               \
     const float4 wa = __ldg(reinterpret_cast<const float4*>(wrow + (T) * tapstride));      \

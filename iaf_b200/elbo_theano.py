@@ -24,6 +24,9 @@ down_conv1's prior channels are then ``[h_det n_h2 | made_context n_h2]``, the p
 ``kl = logqs - logps_made(z, made_context)``.  The posterior half of the down posteriors is then
 :func:`iaf_b200.elbo.posterior_sample` around ``iaf_layer.step`` (the fused diagonal-prior ``layer`` entry does not
 apply), and the prior's density is the pluggable ``iaf_layer.prior_logp(name, z, context) -> (logp_bc, logp)``.
+:func:`decode` is the generative path, ``cvae1.f_decoder`` (models.py:499-521) over :func:`layer_down_p`; with
+``prior='made'`` it samples the prior through ``iaf_layer.prior_sample(name, eps, made_context) -> z``, where the
+reference uses ``z = eps`` as a placeholder (models.py:338-340).
 ``prior='diag'`` is the default; any other prior name (``diag2``, ``bernoulli``, ...) raises ``ValueError``.
 """
 import math
@@ -204,6 +207,44 @@ def _layer_down_q_made(w, name, h_in, h, up_state, eps, iaf_layer, hps, downsamp
     return out, kl_bc, kl_sum
 
 
+def layer_down_p(w, name, h_in, eps, iaf_layer, hps, downsample):
+    """cvae_layer.down_p (models.py:330-359), the generative half of the layer: the prior's sample from the noise eps,
+    then down_conv2.  prior='diag': ``z = mean_prior + eps * exp(logsd_prior)`` from down_conv1's prior channels, as the
+    reference.  prior='made': the sample of the autoregressive prior with ``made_context = h[:, n_h2:2 n_h2]``, through
+    ``iaf_layer.prior_sample(name, eps, made_context) -> z`` (the step run backwards, z = 0.1 m(z) + exp(0.1 s(z)) eps).
+    This deliberately replaces the reference's placeholder, which prints "TODO: SAMPLES FROM MADE PRIOR" and uses
+    ``z = eps`` (models.py:338-340)."""
+    nz, nh2, nl = hps["n_z"], hps["n_h2"], hps["nl"]
+    ds = 2 if downsample else 1
+    posterior_of(hps)
+    h = conv2d(w, name + "_down_conv1", nonlinearity(h_in, nl))
+    h_det = h[:, :nh2]
+    if prior_of(hps) == "made":
+        z = iaf_layer.prior_sample(name, eps.contiguous(), h[:, nh2:2 * nh2].contiguous())
+    else:
+        z = h[:, nh2:nh2 + nz] + eps * torch.exp(h[:, nh2 + nz:nh2 + 2 * nz])
+    hh = torch.cat([h_det, z], dim=1)
+    if downsample:
+        h_in = upsample_nn(h_in)
+    return h_in + 0.1 * conv2d(w, "%s_down_conv2_%d" % (name, ds), nonlinearity(hh, nl), upsample=ds)
+
+
+def decode(w, eps, iaf_layer, hps):
+    """cvae1.f_decoder (models.py:499-521) for px='logistic': noise to a uint8 image [B,3,S,S].  eps[(i, j)]: the
+    N(0,1) draw of layer (i, j), the keys ``forward``'s noise uses."""
+    depths, nl = hps["depths"], hps["nl"]
+    prior_of(hps)
+    B = eps[(0, 0)].shape[0]
+    size = hps["image_size"] // 2 ** len(depths)
+    h = w["h_top"].reshape(1, -1, 1, 1).expand(B, -1, size, size)
+    for i in reversed(range(len(depths))):
+        for j in reversed(range(depths[i])):
+            h = layer_down_p(w, "%d_%d" % (i, j), h, eps[(i, j)], iaf_layer, hps, i > 0 and j == 0)
+    out = 0.1 * conv2d(w, "x_dec", nonlinearity(h, nl), upsample=2)
+    mean_x = torch.clamp(out + 0.5, 1 / 512.0, 1 - 1 / 512.0)
+    return (256.0 * mean_x).to(torch.uint8)
+
+
 def discretized_logistic_logp(mean, logscale, binsize, sample):
     """graphy/nodes/rand.py:169-178 (.logp)."""
     scale = torch.exp(logscale)
@@ -323,6 +364,12 @@ class CudaIAF(object):
         made_context (models.py:304-309), summed per (sample, channel) and per sample -> (logp_bc [B,C], logp [B])."""
         _, logp_bc, logp = self._prior_op(name, z.device).ar_logp(z, context)
         return logp_bc, logp
+
+    def prior_sample(self, name, eps, context):
+        """prior='made': a sample of the autoregressive prior from the noise eps with the context made_context
+        (IAFOperator.ar_sample: the step inverted, in the mask's order).  Not differentiable: runs under no_grad."""
+        with torch.no_grad():
+            return self._prior_op(name, eps.device).ar_sample(eps, context)[0]
 
     def _op(self, name, device, conv=1):
         op = self.ops.get((name, conv))

@@ -12,6 +12,8 @@ is in libiaf_b200.so (include/iaf_b200.h).  Three entry points mirror the refere
       (models.py:282-285, tf_train.py:70-72)
 * ``IAFOperator.ar_logp(z, context)`` -- the autoregressive (MADE) prior's log-density, the same stack with the
       density epilogue of models.py:304-309 (prior='made')
+* ``IAFOperator.step_inverse(u, context)`` / ``ar_sample(eps, context)`` -- the step run backwards (sequential in the
+      mask's order): sampling the MADE prior
 
 Both reference functions are graph builders called once; here they run eagerly per batch,
 so the masked / normalised / packed weights are cached on the operator and re-packed only
@@ -373,6 +375,37 @@ class IAFOperator(object):
             _lib.check(self._lib.iaf_ar_logp_fwd(plan, _ptr(z), _ptr(context), _ptr(logps), _ptr(logp_bc), _ptr(logp), B,
                                                  _stream(z.device)))
         return logps, logp_bc, logp
+
+    def _refuse_grad(self, what, *tensors):
+        if self._needs_grad(*tensors):
+            raise NotImplementedError("IAFOperator.%s is not differentiable (the inverse has no backward); call it under "
+                                      "torch.no_grad()" % what)
+
+    def step_inverse(self, u, context, want_logsd=True, want_logdet=True):
+        """Inverse of :meth:`step`: (z, arw_logsd [B,C,H,W] or None, logdet [B] or None) with
+        ``(z - 0.1 m(z)) / exp(0.1 s(z)) = u``, solved in the mask's order by one sequential kernel
+        (iaf_step_inverse); arw_logsd and logdet are ``step(z)``'s own.  Not differentiable: under grad mode with an
+        input or parameter that requires grad it raises NotImplementedError."""
+        self._refuse_grad("step_inverse", u, context)
+        u, context, B, H, W = self._shapes(u, context)
+        plan = self._plan(H, W, u.device)
+        z = torch.empty_like(u)
+        logsd = torch.empty_like(u) if want_logsd else None
+        logdet = torch.empty((B,), device=u.device, dtype=torch.float32) if want_logdet else None
+        with torch.cuda.device(u.device):
+            _lib.check(self._lib.iaf_step_inverse(plan, _ptr(u), _ptr(context), _ptr(z), _ptr(logsd), _ptr(logdet), B,
+                                                  _stream(u.device)))
+        return z, logsd, logdet
+
+    def ar_sample(self, eps, context):
+        """A sample of the autoregressive (MADE) prior whose stack this operator is (see :meth:`ar_logp`):
+        ``z = 0.1 m(z) + exp(0.1 s(z)) eps``, the inverse of the step at ``eps``.  Returns (z, logp_bc [B,C], logp [B])
+        with the prior's log-density at z, ``-0.5 log 2pi - arw_logsd - 0.5 eps^2`` (rand.py:83 with u = eps) summed over
+        (h,w) and over (c,h,w).  One kernel call; not differentiable (as :meth:`step_inverse`)."""
+        self._refuse_grad("ar_sample", eps, context)
+        z, logsd, _ = self.step_inverse(eps, context, want_logsd=True, want_logdet=False)
+        logps = -0.5 * np.log(2 * np.pi) - logsd - 0.5 * eps * eps
+        return z, logps.sum(dim=(2, 3)), logps.sum(dim=(1, 2, 3))
 
     def _ar_logp_train_raw(self, z, context):
         """iaf_ar_logp_fwd_train: the density plus z', made_logsd and the hidden activations its backward needs."""

@@ -244,6 +244,18 @@ int iaf_ar_logp_bwd_saved(iaf_plan_t* plan, const float* z, const float* z_out, 
                           float* g_context, float* const* g_w, float* const* g_scale, float* const* g_bias,
                           int B, void* stream);
 
+/*
+ * Inverse of iaf_step_fwd: z with (z - 0.1 m(z)) / exp(0.1 s(z)) = u, solved in the mask's order (sequential over
+ * pixels and channels).  With u = eps ~ N(0,1) and the MADE prior's stack and made_context this samples the prior
+ * (models.py:36-38, 304-309; the reference's down_p leaves it TODO, models.py:338-340).  logsd_out = arw_logsd at z,
+ * logdet_out = -sum arw_logsd (each may be NULL), i.e. exactly iaf_step_fwd(z)'s outputs.  Needs n_heads == 2 and
+ * head[0] == head[1] == n_z.  Allocates nothing (capture-safe); deterministic.  One exact-fp32 kernel serves every plan,
+ * tensor-core plans included; IAF_ERR_UNSUPPORTED when the plan's two-row window of every stage does not fit in shared
+ * memory (4 (W + 2) (n_z + sum hidden) * 2 bytes and a little more, at most 225 KiB).
+ */
+int iaf_step_inverse(iaf_plan_t* plan, const float* u, const float* context, float* z_out,
+                     float* logsd_out, float* logdet_out, int B, void* stream);
+
 /* Backward of the un-fused operator iaf_multiconv_fwd: g_outs[k] [B,head[k],H,W] is the
  * gradient at head k.  Same outputs as iaf_step_bwd. */
 int iaf_multiconv_bwd(iaf_plan_t* plan, const float* z, const float* context, const float* const* w,
