@@ -459,9 +459,10 @@ static LyKernel fz_kernel_for(bool padw, int mode, bool elu) { return ly_kernel_
 
 static int tc_round_up(int a, int b) { return (a + b - 1) / b * b; }
 
-// per stage: an A window (first stage), the bias table, the partial scratch, the accumulator tile, an NB-deep ring
+// per stage: an A window (first stage), the bias table, the partial scratch, the accumulator tile, an NB-deep ring.
+// A stack without hidden layers (the linear IAF) is one stage, the heads, whose A window is built from fp32 z.
 static bool ly_layout(const iaf_desc_t* d, IafTcPlan* pl) {
-  if (d->n_hidden < 1 || d->n_heads != 2 || d->head[0] != d->n_z || d->head[1] != d->n_z) return false;
+  if (d->n_heads != 2 || d->head[0] != d->n_z || d->head[1] != d->n_z) return false;
   if (d->n_z % 16 != 0 || 2 * d->n_z > 32 * LY_MAX_NGW) return false;
   for (int i = 0; i < d->n_hidden; ++i)
     if (d->hidden[i] % 16 != 0 || d->hidden[i] > 32 * LY_MAX_NGW) return false;
@@ -677,6 +678,7 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
       for (int b2 = 0; b2 < 2; ++b2) {
         if (pl->img[a2][b2]) cudaFree(pl->img[a2][b2]);
         pl->img[a2][b2] = nullptr;
+        if (maxc == 0) continue;  // no hidden stage: no operand images
         if (cudaMalloc(&pl->img[a2][b2], bytes) != cudaSuccess) return IAF_ERR_CUDA;
         if (cudaMemsetAsync(pl->img[a2][b2], 0, bytes, stream) != cudaSuccess) return IAF_ERR_CUDA;
       }
@@ -760,8 +762,8 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
     q.o_lo = pl->img[j & 1][1];
     q.S_pad = pl->img_S_pad;
     q.in_mode = j ? 1 : 0;
-    q.first = j == 0;
     q.is_heads = j == pl->n_stages - 1;
+    q.first = j == 0 && !q.is_heads;  // the first HIDDEN stage adds the context: never without one (ar.py:399-403)
     q.NB = pl->ly_NB[j];
     q.sm_a = pl->ly_sm_a[j]; q.sm_b = pl->ly_sm_b[j]; q.sm_bias = pl->ly_sm_bias[j]; q.sm_part = pl->ly_sm_part[j];
     q.sm_acc = pl->ly_sm_acc[j];

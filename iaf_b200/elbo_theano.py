@@ -28,6 +28,10 @@ apply), and the prior's density is the pluggable ``iaf_layer.prior_logp(name, z,
 ``prior='made'`` it samples the prior through ``iaf_layer.prior_sample(name, eps, made_context) -> z``, where the
 reference uses ``z = eps`` as a placeholder (models.py:338-340).
 ``prior='diag'`` is the default; any other prior name (``diag2``, ``bernoulli``, ...) raises ``ValueError``.
+``posterior='down_iaf2'`` and ``'up_iaf2'`` are the linear IAF (models.py:55-56, 79-82, 152-161, 246-259): one masked
+conv ``{i}_{j}_posterior_conv1_{w,s,b}`` with ``w`` of shape [2 n_z, n_z + 1, 3, 3], whose even rows are the mean head
+and odd rows the logsd head, and no context (up_conv1 and down_conv1 have no context channels).  The operator runs it as
+a stack without hidden layers and two heads of n_z (:func:`iaf_b200.weights.deinterleave_heads`).
 """
 import math
 
@@ -35,9 +39,15 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from .weights import deinterleave_heads
+
 LOGSCALE_SCALE = 3.0  # graphy/nodes/conv.py:19 (conv.py:16-22: logscale=True, bn=False, maxweight=0)
-POSTERIORS = ("down_iaf2_nl", "up_iaf2_nl", "down_iaf2_nl2")
+POSTERIORS = ("down_iaf2_nl", "up_iaf2_nl", "down_iaf2_nl2", "down_iaf2", "up_iaf2")
 PRIORS = ("diag", "made")
+# the paper's linear IAF (models.py:55-56, 79-82): one masked conv ``ar.conv2d(name+'_posterior_conv1', n_z, 2 n_z)``,
+# no hidden layer and no context, its rows interleaving the two heads (mean = out[:, ::2], logsd = out[:, 1::2])
+LINEAR = ("down_iaf2", "up_iaf2")
+UP_POSTERIORS = ("up_iaf2_nl", "up_iaf2")  # the sample is drawn and transformed in the bottom-up pass
 
 
 def posterior_of(hps):
@@ -112,20 +122,29 @@ def gaussian_logps(mean, logvar, x):
     return -0.5 * (math.log(2 * math.pi) + logvar + (x - mean) ** 2 / torch.exp(logvar))
 
 
+def _contiguous(t):
+    return None if t is None else t.contiguous()
+
+
 def layer_up(w, name, h_in, hps, downsample, eps=None, iaf_layer=None):
     """cvae_layer.up (models.py:133-196).  down_iaf2_nl: returns (output, (qz_mean, qz_logsd, up_context)).
     up_iaf2_nl (models.py:169-178): the posterior sample is drawn and transformed HERE, with the context taken from
-    up_conv1's channels; returns (output, (z, logqs)) for the top-down pass."""
+    up_conv1's channels; returns (output, (z, logqs)) for the top-down pass.  The linear posteriors have no context:
+    up_context is None (up_iaf2: models.py:152-161)."""
     nz, nh2, nl = hps["n_z"], hps["n_h2"], hps["nl"]
     ds = 2 if downsample else 1
+    posterior = posterior_of(hps)
     h = conv2d(w, "%s_up_conv1_%d" % (name, ds), nonlinearity(h_in, nl), downsample=ds)
-    h_det, qz_mean, qz_logsd, up_context = torch.split(h, [nh2, nz, nz, nh2], dim=1)
+    if posterior in LINEAR:                                            # no up context (models.py:25, 55-56, 79-82)
+        (h_det, qz_mean, qz_logsd), up_context = torch.split(h, [nh2, nz, nz], dim=1), None
+    else:
+        h_det, qz_mean, qz_logsd, up_context = torch.split(h, [nh2, nz, nz, nh2], dim=1)
     if downsample:
         h_in = downsample_nn(h_in)
-    if posterior_of(hps) == "up_iaf2_nl":
+    if posterior in UP_POSTERIORS:
         z0 = qz_mean + torch.exp(qz_logsd) * eps                       # gaussian_diag(qz_mean, 2 qz_logsd).sample
         logqs = gaussian_logps(qz_mean, 2 * qz_logsd, z0)
-        z, arw_logsd = iaf_layer.step(name, z0.contiguous(), up_context.contiguous())
+        z, arw_logsd = iaf_layer.step(name, z0.contiguous(), _contiguous(up_context))
         logqs = logqs + arw_logsd                                      # models.py:174
         hh = torch.cat([h_det, z], dim=1)
         return h_in + 0.1 * conv2d(w, name + "_up_conv2", nonlinearity(hh, nl)), (z, logqs)
@@ -140,7 +159,7 @@ def layer_down_q(w, name, h_in, up_state, eps, iaf_layer, hps, downsample):
     posterior = posterior_of(hps)
     if prior_of(hps) == "made":
         return _layer_down_q_made(w, name, h_in, h, up_state, eps, iaf_layer, hps, downsample)
-    if posterior == "up_iaf2_nl":                                      # models.py:215-217, 287-290
+    if posterior in UP_POSTERIORS:                                     # models.py:215-217, 287-290
         h_det, pz_mean, pz_logsd = torch.split(h, [nh2, nz, nz], dim=1)
         z, logqs = up_state
         kl = logqs - gaussian_logps(pz_mean, 2 * pz_logsd, z)
@@ -149,12 +168,18 @@ def layer_down_q(w, name, h_in, up_state, eps, iaf_layer, hps, downsample):
             h_in = upsample_nn(h_in)
         out = h_in + 0.1 * conv2d(w, "%s_down_conv2_%d" % (name, ds), nonlinearity(hh, nl), upsample=ds)
         return out, kl.sum(dim=(2, 3)), kl.sum(dim=(1, 2, 3))
-    # channel map: [h_det n_h2 | pz_mean n_z | pz_logsd n_z || rz_mean n_z | rz_logsd n_z | down_context n_h2]
-    h_det, pz_mean, pz_logsd, rz_mean, rz_logsd, down_context = torch.split(h, [nh2, nz, nz, nz, nz, nh2], dim=1)
     qz_mean, qz_logsd, up_context = up_state
+    if posterior in LINEAR:
+        # channel map: [h_det n_h2 | pz_mean n_z | pz_logsd n_z || rz_mean n_z | rz_logsd n_z]  (models.py:79-82, 246-259)
+        h_det, pz_mean, pz_logsd, rz_mean, rz_logsd = torch.split(h, [nh2, nz, nz, nz, nz], dim=1)
+        context = None
+    else:
+        # channel map: [h_det n_h2 | pz_mean n_z | pz_logsd n_z || rz_mean n_z | rz_logsd n_z | down_context n_h2]
+        h_det, pz_mean, pz_logsd, rz_mean, rz_logsd, down_context = torch.split(h, [nh2, nz, nz, nz, nz, nh2], dim=1)
+        context = (up_context + down_context).contiguous()
     # posterior N(qz.mean + rz_mean, qz.logvar + 2 rz_logsd) with qz.logvar = 2 qz_logsd (models.py:139,275)
     stats = ((qz_mean + rz_mean).contiguous(), (qz_logsd + rz_logsd).contiguous(), pz_mean.contiguous(),
-             pz_logsd.contiguous(), (up_context + down_context).contiguous())
+             pz_logsd.contiguous(), context)
     if posterior == "down_iaf2_nl2":
         # models.py:281-291: step(conv1), then step(conv2) in the reversed order; both arw_logsd go into logqs
         from .elbo import stochastic_layer
@@ -179,14 +204,20 @@ def _layer_down_q_made(w, name, h_in, h, up_state, eps, iaf_layer, hps, downsamp
     nz, nh2, nl = hps["n_z"], hps["n_h2"], hps["nl"]
     ds = 2 if downsample else 1
     posterior = posterior_of(hps)
-    if posterior == "up_iaf2_nl":
+    if posterior in UP_POSTERIORS:
         # channel map: [h_det n_h2 | made_context n_h2]; z and logqs come from the bottom-up pass (models.py:215-217)
         h_det, made_context = torch.split(h, [nh2, nh2], dim=1)
         z, logqs = up_state
     else:
-        # channel map: [h_det n_h2 | made_context n_h2 || rz_mean n_z | rz_logsd n_z | down_context n_h2]
-        h_det, made_context, rz_mean, rz_logsd, down_context = torch.split(h, [nh2, nh2, nz, nz, nh2], dim=1)
         qz_mean, qz_logsd, up_context = up_state
+        if posterior in LINEAR:
+            # channel map: [h_det n_h2 | made_context n_h2 || rz_mean n_z | rz_logsd n_z]
+            h_det, made_context, rz_mean, rz_logsd = torch.split(h, [nh2, nh2, nz, nz], dim=1)
+            context = None
+        else:
+            # channel map: [h_det n_h2 | made_context n_h2 || rz_mean n_z | rz_logsd n_z | down_context n_h2]
+            h_det, made_context, rz_mean, rz_logsd, down_context = torch.split(h, [nh2, nh2, nz, nz, nh2], dim=1)
+            context = (up_context + down_context).contiguous()
         from .elbo import posterior_sample
         if posterior == "down_iaf2_nl2":
             def steps(z, c):
@@ -196,7 +227,7 @@ def _layer_down_q_made(w, name, h_in, h, up_state, eps, iaf_layer, hps, downsamp
         else:
             steps = lambda z, c: iaf_layer.step(name, z, c)
         z, logqs = posterior_sample(steps, eps, (qz_mean + rz_mean).contiguous(), (qz_logsd + rz_logsd).contiguous(),
-                                    (up_context + down_context).contiguous())
+                                    context)
     logp_bc, logp = iaf_layer.prior_logp(name, z.contiguous(), made_context.contiguous())
     kl_bc = logqs.sum(dim=(2, 3)) - logp_bc
     kl_sum = logqs.sum(dim=(1, 2, 3)) - logp
@@ -296,8 +327,9 @@ def make_params(hps, seed=0, dtype=np.float32):
     rng = np.random.RandomState(seed)
     nz, nh1, nh2, depths = hps["n_z"], hps["n_h1"], hps["n_h2"], hps["depths"]
     posterior = posterior_of(hps)
-    up_post = posterior == "up_iaf2_nl"
+    up_post, linear = posterior in UP_POSTERIORS, posterior in LINEAR
     made = prior_of(hps) == "made"
+    n_ctx = 0 if linear else nh2                       # the context channels of up_conv1 / down_conv1
     w = {}
 
     def conv(name, cin, cout, k, pad_channel=True):
@@ -313,16 +345,19 @@ def make_params(hps, seed=0, dtype=np.float32):
         for j in range(depths[i]):
             n = "%d_%d" % (i, j)
             ds = 2 if (i > 0 and j == 0) else 1
-            conv("%s_up_conv1_%d" % (n, ds), nh1, nh2 + 2 * nz + nh2, 3)
-            conv(n + "_up_conv2", nh2 + nz if up_post else nh2, nh1, 3)                       # models.py:25,84
-            conv(n + "_down_conv1", nh1, (2 * nh2 if made else nh2 + 2 * nz) + (0 if up_post else 2 * nz + nh2),
-                 3)                                                    # models.py:27-28,36-38,86
+            conv("%s_up_conv1_%d" % (n, ds), nh1, nh2 + 2 * nz + n_ctx, 3)
+            conv(n + "_up_conv2", nh2 + nz if up_post else nh2, nh1, 3)                       # models.py:25,55-84
+            conv(n + "_down_conv1", nh1, (2 * nh2 if made else nh2 + 2 * nz) + (0 if up_post else 2 * nz + n_ctx),
+                 3)                                                    # models.py:27-28,36-38,79-86
             conv("%s_down_conv2_%d" % (n, ds), nh2 + nz, nh1 * ds * ds, 3)
             sizes = [nz] + hps["depth_ar"] * [nh2]
-            for k in range(hps["depth_ar"]):
-                conv("%s_posterior_conv1_%d" % (n, k), sizes[k], sizes[k + 1], 3)
-            for k in range(2):
-                conv("%s_posterior_conv1_out_%d" % (n, k), sizes[-1], nz, 3)
+            if linear:                                                 # ar.conv2d(n_z, 2 n_z): rows interleave the heads
+                conv("%s_posterior_conv1" % n, nz, 2 * nz, 3)
+            else:
+                for k in range(hps["depth_ar"]):
+                    conv("%s_posterior_conv1_%d" % (n, k), sizes[k], sizes[k + 1], 3)
+                for k in range(2):
+                    conv("%s_posterior_conv1_out_%d" % (n, k), sizes[-1], nz, 3)
             if posterior == "down_iaf2_nl2":                           # models.py:98
                 for k in range(hps["depth_ar"]):
                     conv("%s_posterior_conv2_%d" % (n, k), sizes[k], sizes[k + 1], 3)
@@ -345,10 +380,24 @@ class CudaIAF(object):
         self.w, self.hps, self.path, self.IAFOperator, self.ops = w, hps, path, IAFOperator, {}
         self.prior_ops = {}  # prior='made': layer name -> the prior's operator (prior_conv1, models.py:36-38)
 
+    def _linear(self, conv):
+        return conv != 0 and posterior_of(self.hps) in LINEAR
+
     def _new_op(self, conv):
         nz, nh2, dar = self.hps["n_z"], self.hps["n_h2"], self.hps["depth_ar"]
-        return self.IAFOperator("theano", nz, dar * [nh2], [nz, nz], nl=self.hps["nl"], path=self.path,
+        hidden = [] if self._linear(conv) else dar * [nh2]             # the linear IAF: no hidden layer, no context
+        return self.IAFOperator("theano", nz, hidden, [nz, nz], nl=self.hps["nl"], path=self.path,
                                 flipmask=conv == 2)                    # models.py:36-38,92,97-98 (conv 0: the prior)
+
+    def _posterior_layers(self, name, conv, convert):
+        """The (w, s, b) triples of posterior conv ``conv``, each tensor passed through ``convert``: the stack's, or the
+        linear IAF's one conv with its interleaved rows split into the two heads."""
+        pre = "%s_posterior_conv%d" % (name, conv)
+        if self._linear(conv):
+            return deinterleave_heads(*(convert(self.w[pre + "_" + k]) for k in "wsb"))
+        dar = self.hps["depth_ar"]
+        names = ["%s_%d" % (pre, i) for i in range(dar)] + ["%s_out_%d" % (pre, k) for k in range(2)]
+        return [tuple(convert(self.w[n + "_" + k]) for k in "wsb") for n in names]
 
     def _prior_op(self, name, device):
         op = self.prior_ops.get(name)
@@ -374,9 +423,9 @@ class CudaIAF(object):
     def _op(self, name, device, conv=1):
         op = self.ops.get((name, conv))
         if op is None:
-            from .weights import theano_layers
+            from .weights import _as_f32
             op = self._new_op(conv)
-            op.set_weights(theano_layers(self.w, "%s_posterior_conv%d" % (name, conv), self.hps["depth_ar"], device=device))
+            op.set_weights(self._posterior_layers(name, conv, lambda a: _as_f32(a, device)))
             self.ops[(name, conv)] = op
         return op
 
@@ -407,14 +456,12 @@ class CudaIAFTrain(CudaIAF):
 
     def _op(self, name, device, conv=1):
         op = self.ops.get((name, conv))
-        dar = self.hps["depth_ar"]
         if op is None:
             op = self._new_op(conv)
             self.ops[(name, conv)] = op
-        pre = "%s_posterior_conv%d" % (name, conv)
-        names = ["%s_%d" % (pre, i) for i in range(dar)] + ["%s_out_%d" % (pre, k) for k in range(2)]
-        # the live tensors of w (float32, on the device): not detached, so their .grad is filled by backward()
-        op.set_weights([(self.w[n + "_w"], self.w[n + "_s"], self.w[n + "_b"]) for n in names])
+        # the live tensors of w (float32, on the device): not detached, so their .grad is filled by backward().  The linear
+        # IAF's rows are split on every call, inside autograd, so its gradient lands interleaved in w[...]
+        op.set_weights(self._posterior_layers(name, conv, lambda t: t))
         return op
 
     def _prior_op(self, name, device):

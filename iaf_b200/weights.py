@@ -49,6 +49,15 @@ def theano_layers(w, name, n_hidden, n_heads=2, device="cuda"):
     return [(t(w[n + "_w"]), t(w[n + "_s"]), t(w[n + "_b"])) for n in names]
 
 
+def deinterleave_heads(w, s, b):
+    """The two heads of a linear IAF conv ``ar.conv2d(name, n_z, 2 n_z)`` (models.py:55-56, 79-82): its output rows
+    interleave them, ``mean = out[:, ::2]``, ``logsd = out[:, 1::2]`` (models.py:152-161, 246-259).  Returns the
+    (w, s, b) triples of the mean and the logsd head, views of the given tensors (so autograd scatters their gradients
+    back into the interleaved rows).  Row 2i and row 2i + 1 have the mask of row i of ``ar.conv2d(n_z, n_z)`` with
+    zerodiagonal (ar.py:250-256), and weight normalisation is per row, so each head is an ordinary heads conv."""
+    return [(w[k::2], s[k::2], b[k::2]) for k in range(2)]
+
+
 def tf_layers(variables, scope, n_hidden=2, n_heads=2, device="cuda"):
     """(V, g, b) triples for ``ar_multiconv2d`` under ``scope`` (e.g. ``model/IAF_0_3/ar_multiconv2d``)."""
     names = ["layer_%d" % i for i in range(n_hidden)] + ["layer_out_%d" % k for k in range(n_heads)]
