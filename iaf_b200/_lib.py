@@ -60,6 +60,7 @@ SYMBOLS = {
     "iaf_ar_logp_bwd_saved": (C.c_int, [_P, _P, _P, _P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), _P, _P, _P, _P, _P,
                                         C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.c_int, _P]),
     "iaf_step_inverse": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, _P]),
+    "iaf_step_inverse_adjoint": (C.c_int, [_P, _P, _P, C.POINTER(_P), _P, _P, _P, _P, C.c_int, _P]),
     "iaf_strerror": (C.c_char_p, [C.c_int]),
     "iaf_last_cuda_error": (C.c_char_p, []),
     "iaf_version": (C.c_int, []),

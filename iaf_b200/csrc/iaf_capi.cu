@@ -37,7 +37,7 @@ long long centre_nnz(int cin, int cout, int zd, int flipmask) {
 
 }  // namespace
 
-IafInvKernel iaf_inv = {nullptr, nullptr};  // (filled in by iaf_inv.cu)
+IafInvKernel iaf_inv = {nullptr, nullptr, nullptr};  // (filled in by iaf_inv.cu)
 
 struct iaf_plan {
   iaf_desc_t d;
@@ -96,6 +96,12 @@ struct iaf_plan {
   int inv_ring_off[IAF_MAX_STAGES], inv_acc_off[IAF_MAX_STAGES], inv_lds_off, inv_smem_floats, inv_units;
   size_t inv_smem;
   bool inv_ok;
+  // its adjoint (iaf_step_inverse_adjoint): the "gradient final after z channel step k" table (in inv_tab, after the
+  // inverse's) and the kernel's shared-memory layout
+  int adj_grp_off[IAF_MAX_HIDDEN];
+  int adj_ring_off[IAF_MAX_STAGES], adj_acc_off[IAF_MAX_STAGES], adj_smem_floats, adj_units;
+  size_t adj_smem;
+  bool adj_ok;
 };
 #define IAF_NSLOT 3
 
@@ -170,6 +176,40 @@ static bool inv_tables(iaf_plan* pl) {
   pl->inv_units = units;
   pl->inv_smem = sizeof(float) * (size_t)o;
   if (pl->inv_smem > 225 * 1024) return false;  // the SIMT kernel's limit (iaf_plan_create)
+  // The adjoint's table (iaf_inv_adj_kernel): its chain runs the steps backwards, so a unit's gradient is final at the
+  // EARLIEST step among its live centre consumers in the stage above (the heads: channel c at step pos(c)), C (before
+  // the chain) when it has none.  Groups of step 0 .. C, appended to the same table.
+  std::vector<int> nxt(C);
+  for (int c = 0; c < C; ++c) nxt[c] = fm ? C - 1 - c : c;
+  for (int j = L - 1; j >= 0; --j) {
+    const int cin = pl->cin[j + 1], heads = j + 1 == L, ncons = heads ? C : pl->cout[j + 1];
+    cur.assign(cin, C);
+    for (int co = 0; co < ncons; ++co)
+      for (int ci = 0; ci < cin; ++ci)
+        if (iaf_tap_rule(0, ci, co, cin, ncons, heads, fm).live) cur[ci] = std::min(cur[ci], nxt[co]);
+    pl->adj_grp_off[j] = (int)tab.size();
+    std::vector<int> off(C + 2, 0);
+    for (int u = 0; u < cin; ++u) off[cur[u] + 1] += 1;
+    for (int g = 1; g < C + 2; ++g) off[g] += off[g - 1];
+    std::vector<int> members(cin), fill(off.begin(), off.end() - 1);
+    for (int u = 0; u < cin; ++u) members[fill[cur[u]]++] = u;
+    tab.insert(tab.end(), off.begin(), off.end());
+    tab.insert(tab.end(), members.begin(), members.end());
+    nxt = cur;
+  }
+  // its shared memory: per stage a two-row ring of its output gradients (the heads': 2 n_z), then per stage the
+  // gradient accumulators of its input.  Refused on its own, keeping the inverse, when it does not fit.
+  o = 0; units = 0;
+  for (int j = 0; j < pl->n_stages; ++j) {
+    pl->adj_ring_off[j] = o; o += pl->cout[j] * 2 * (d.W + 2);
+  }
+  for (int j = 0; j < pl->n_stages; ++j) {
+    pl->adj_acc_off[j] = o; o += pl->cin[j]; units += pl->cin[j];
+  }
+  pl->adj_smem_floats = o;
+  pl->adj_units = units;
+  pl->adj_smem = sizeof(float) * (size_t)o;
+  pl->adj_ok = pl->adj_smem <= 225 * 1024;
   if (!tab.empty()) {
     pl->inv_tab_host = (int*)malloc(sizeof(int) * tab.size());
     if (!pl->inv_tab_host) return false;
@@ -610,6 +650,49 @@ int iaf_step_inverse(iaf_plan_t* pl, const float* u, const float* context, float
   p.flip = pl->vf.reflect; p.descending = pl->vf.flipmask;
   p.nl = d.nl; p.scale = 0.1f;
   CK(iaf_inv.launch(p, B, pl->inv_smem, stream));
+  pl->launches += 1;
+  return IAF_OK;
+}
+
+// The adjoint of iaf_step_inverse (iaf_inv.cu): one sequential kernel, on every plan.  B == 0 only checks the plan.
+int iaf_step_inverse_adjoint(iaf_plan_t* pl, const float* u, const float* logsd, const float* const* hidden,
+                             const float* g_z, const float* g_logsd, const float* g_logdet, float* g_u, int B,
+                             void* stream_) {
+  if (!pl || B < 0) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_heads != 2 || pl->d.head[0] != pl->d.n_z) return IAF_ERR_BAD_SHAPE;
+  if (!pl->packed) return IAF_ERR_NOT_PACKED;
+  if (!pl->inv_ok || !pl->adj_ok || !iaf_inv.launch_adj) return IAF_ERR_UNSUPPORTED;
+  if (B == 0) return IAF_OK;
+  if (!u || !logsd || !g_z || !g_u) return IAF_ERR_BAD_ARG;
+  if (pl->d.n_hidden > 0 && !hidden) return IAF_ERR_BAD_ARG;
+  for (int j = 0; j < pl->d.n_hidden; ++j)
+    if (!hidden[j]) return IAF_ERR_BAD_ARG;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  { int cg = capture_guard(pl, stream, IAF_SCRATCH_FITS); if (cg != IAF_OK) return cg; }  // it has no scratch
+  { int hs = stream_handoff(pl, stream); if (hs != IAF_OK) return hs; }
+  const iaf_desc_t& d = pl->d;
+  IafInvAdjParams p;
+  memset(&p, 0, sizeof(p));
+  p.u = u; p.logsd = logsd; p.g_z = g_z; p.g_logsd = g_logsd; p.g_logdet = g_logdet; p.g_u = g_u;
+  for (int j = 0; j < d.n_hidden; ++j) p.hid[j] = hidden[j];
+  p.grp = pl->inv_tab;
+  for (int j = 0; j < d.n_hidden; ++j) p.grp_off[j] = pl->adj_grp_off[j];
+  for (int j = 0; j < pl->n_stages; ++j) {
+    p.stage[j].w = pl->w[j];
+    p.stage[j].bias = pl->bias[j];
+    p.stage[j].padw = nullptr;  // the pad channel is a constant input: no gradient
+    p.stage[j].cin = pl->cin[j];
+    p.stage[j].cout = pl->cout[j];
+    p.stage[j].cout_pad = pl->cout_pad[j];
+    p.ring_off[j] = pl->adj_ring_off[j];
+    p.acc_off[j] = pl->adj_acc_off[j];
+  }
+  p.smem_floats = pl->adj_smem_floats;
+  p.n_stages = pl->n_stages; p.n_units = pl->adj_units;
+  p.C = d.n_z; p.H = d.H; p.W = d.W;
+  p.flip = pl->vf.reflect; p.descending = pl->vf.flipmask;
+  p.nl = d.nl; p.scale = 0.1f;
+  CK(iaf_inv.launch_adj(p, B, pl->adj_smem, stream));
   pl->launches += 1;
   return IAF_OK;
 }

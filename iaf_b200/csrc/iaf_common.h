@@ -231,12 +231,41 @@ struct IafInvParams {
   float scale;             // 0.1
 };
 
+// The adjoint of the inverse (iaf_inv_adj_kernel, iaf_inv.cu): g_u = J^-T (g_z + A_z^T (g_logsd - g_logdet)) at
+// z = inverse(u), J = d step / d z, A_z = d arw_logsd / d z.  One CTA per sample walks the canonical frame in raster
+// order and, within a pixel, the z channels in the reverse of the mask's order.  Shared memory: per stage, a two-row
+// ring of its output gradients [cout][2][W+2] (the heads' as [2 n_z], m and s of channel c at 2c and 2c+1; columns -1
+// and W and the row above the map stay zero), then per stage the gradient accumulators of its input [cin].
+struct IafInvAdjParams {
+  const float* u;          // [B,C,H,W]
+  const float* logsd;      // [B,C,H,W]: arw_logsd at z (the inverse's own)
+  const float* hid[IAF_MAX_HIDDEN];  // hidden activations at z [B][hidden[j]][H][W] (iaf_step_fwd_train)
+  const float* g_z;        // [B,C,H,W]
+  const float* g_logsd;    // nullable
+  const float* g_logdet;   // nullable, [B]
+  float* g_u;
+  // per hidden stage j: grp[grp_off[j] + k], k = 0..C+1, is where the units of stage j whose gradient is final after
+  // z channel step k start (step C: before the chain), and grp[grp_off[j] + C + 2 + i] lists the units in that order
+  const int* grp;
+  int grp_off[IAF_MAX_HIDDEN];
+  IafStageDev stage[IAF_MAX_STAGES];
+  int ring_off[IAF_MAX_STAGES], acc_off[IAF_MAX_STAGES], smem_floats;
+  int n_stages, n_units;   // n_units = sum of cin
+  int C, H, W;
+  int flip;                // IafVariantFlags::reflect
+  int descending;          // the mask's channel order: C-1 .. 0 (flipmask) or 0 .. C-1 (the chain walks it backwards)
+  int nl;
+  float scale;             // 0.1
+};
+
 cudaError_t iaf_launch_pack(const IafPackParams& p, int max_cout, cudaStream_t stream);
-// The inverse's launcher and shared-memory opt-in.  iaf_inv.cu fills them in when it is linked in; the C ABI also builds
-// without it (tests/test_emu_kernels.py's sanitizer build), and then iaf_step_inverse refuses with IAF_ERR_UNSUPPORTED.
+// The inverse's and its adjoint's launchers and shared-memory opt-in.  iaf_inv.cu fills them in when it is linked in;
+// the C ABI also builds without it (tests/test_emu_kernels.py's sanitizer build), and then iaf_step_inverse and
+// iaf_step_inverse_adjoint refuse with IAF_ERR_UNSUPPORTED.
 struct IafInvKernel {
   cudaError_t (*launch)(const IafInvParams& p, int B, size_t smem_bytes, cudaStream_t stream);
   cudaError_t (*set_smem)();
+  cudaError_t (*launch_adj)(const IafInvAdjParams& p, int B, size_t smem_bytes, cudaStream_t stream);
 };
 extern IafInvKernel iaf_inv;
 cudaError_t iaf_launch_simt(const IafSimtParams& p, size_t smem_bytes, cudaStream_t stream);

@@ -133,15 +133,153 @@ __global__ void __launch_bounds__(IAF_INV_THREADS) iaf_inv_kernel(const __grid_c
   }
 }
 
-static cudaError_t iaf_inv_set_smem() { return iaf_smem_optin(iaf_inv_kernel); }
+// nl'(pre-activation) from the activation h = nl(pre-activation) (the table of iaf_bwd.cu's bw_nl_grad)
+__device__ __forceinline__ float iaf_inv_nl_grad(float h, int nl) {
+  switch (nl) {
+    case IAF_NL_ELU: return h > 0.f ? 1.f : h + 1.f;
+    case IAF_NL_SOFTPLUS: return 1.f - expf(-h);
+    case IAF_NL_RELU: return h > 0.f ? 1.f : 0.f;
+    case IAF_NL_TANH: return 1.f - h * h;
+    case IAF_NL_LEAKYRELU: return h < 0.f ? 0.01f : 1.f;
+    default: return 1.f;
+  }
+}
+
+// The adjoint of the inverse, exact fp32: g_u = v with J^T v = g_z + A_z^T G_a at z = inverse(u), where J = d step / d z
+// (triangular in the mask's order, diagonal exp(-a)), A_z = d a / d z, a = arw_logsd, G_a = g_logsd - g_logdet.  Per
+// position this is the recurrence
+//   v_c = exp(a_c) (g_z_c + [VJP of the stack at z with (gm, gs)]_c),  gm_i = 0.1 exp(-a_i) v_i,  gs_i = 0.1 (G_a_i + u_i v_i)
+// in which only positions after c in the mask's order contribute, so it runs the inverse's order backwards: pixels in
+// raster order of the canonical frame and, inside a pixel, the z channels in the reverse of the mask's order.  The
+// transpose of iaf_inv_kernel:
+//   1. every stage's non-centre taps, seen from the input side, read output gradients at (y,x-1) and (y-1,x-1..x+1),
+//      already final: one pass over all (stage, input) pairs puts them (and g_z for stage 0) into the stage's
+//      input-gradient accumulator;
+//   2. for each z channel c in reverse order: the accumulator of z_c is complete (every unit that reads z_c at the
+//      centre has been finalised), so v_c = exp(a_c) acc; (gm_c, gs_c) enter the heads' centre taps; then, stage by
+//      stage downwards, the hidden units whose last live centre consumer was just finalised get their gradient
+//      delta = acc nl'(h) and their centre taps enter the stage below.
+// Which units become final at which step comes from the host (iaf_capi.cu, inv_tables): the earliest step, in the
+// mask's order, among a unit's live centre consumers; C (before the chain) when it has none.  The two-row rings hold
+// output gradients (rows y-1 and y); the weights are the SIMT pack read through the read-only cache.  Shared memory and
+// __syncthreads only, as iaf_inv_kernel: the host emulation runs it, and one sample's result is bit-identical whatever
+// the batch.
+__global__ void __launch_bounds__(IAF_INV_THREADS) iaf_inv_adj_kernel(const __grid_constant__ IafInvAdjParams p) {
+  IAF_DYN_SMEM(float, smem);
+  const int tid = threadIdx.x;
+  const int n = blockIdx.x;
+  const int H = p.H, W = p.W, HW = H * W, C = p.C, L = p.n_stages - 1;
+  const int RP = W + 2;  // ring row pitch: columns -1 .. W
+  const float g_ld = p.g_logdet ? __ldg(p.g_logdet + n) : 0.f;
+
+  for (int i = tid; i < p.smem_floats; i += IAF_INV_THREADS) smem[i] = 0.f;
+  __syncthreads();
+
+  for (int y = 0; y < H; ++y) {
+    const int s0 = y & 1, s1 = s0 ^ 1;  // ring slots of rows y and y-1
+    for (int x = 0; x < W; ++x) {
+      const int pix = y * W + x;
+      const int gp = p.flip ? HW - 1 - pix : pix;
+
+      // ---- 1. the non-centre taps of every stage, from the input side ----
+      {
+        int j = 0, base = 0;
+        for (int e = tid; e < p.n_units; e += IAF_INV_THREADS) {
+          while (e >= base + p.stage[j].cin) base += p.stage[j++].cin;
+          const IafStageDev& S = p.stage[j];
+          const int ci = e - base;
+          float v = j == 0 ? __ldg(p.g_z + ((size_t)n * C + ci) * HW + gp) : 0.f;
+          const float* ring = smem + p.ring_off[j];
+          const float* wr = S.w + (size_t)ci * S.cout_pad;
+          const size_t ts = (size_t)S.cin * S.cout_pad;
+          for (int co = 0; co < S.cout; ++co) {
+            // heads: ring entry 2c + h is packed column (c/4)*8 + c%4 + 4h (iaf_pack.cu)
+            const int col = j < L ? co : ((co >> 3) * 8 + ((co >> 1) & 3) + 4 * (co & 1));
+            const float* r0 = ring + (co * 2 + s0) * RP + x + 1;
+            const float* r1 = ring + (co * 2 + s1) * RP + x + 1;
+            v = fmaf(r0[-1], __ldg(wr + ts + col), v);      // ( 0,+1) of output (y,   x-1)
+            v = fmaf(r1[1], __ldg(wr + 2 * ts + col), v);   // (+1,-1) of output (y-1, x+1)
+            v = fmaf(r1[0], __ldg(wr + 3 * ts + col), v);   // (+1, 0) of output (y-1, x)
+            v = fmaf(r1[-1], __ldg(wr + 4 * ts + col), v);  // (+1,+1) of output (y-1, x-1)
+          }
+          smem[p.acc_off[j] + ci] = v;
+        }
+      }
+      __syncthreads();
+
+      // ---- 2. the chain over the z channels, backwards (step C: the units no z channel's head depends on) ----
+      for (int k = C; k >= 0; --k) {
+        if (k < C) {
+          const int c = p.descending ? C - 1 - k : k;
+          const int cm = (c >> 2) * 8 + (c & 3);
+          const size_t g = ((size_t)n * C + c) * HW + gp;
+          const float acc0 = smem[p.acc_off[0] + c];  // g_z_c plus the stack's VJP at z_c: complete
+          const float v = expf(__ldg(p.logsd + g)) * acc0;
+          const float gm = p.scale * acc0;  // 0.1 exp(-a_c) v_c
+          const float gs = p.scale * fmaf(__ldg(p.u + g), v, (p.g_logsd ? __ldg(p.g_logsd + g) : 0.f) - g_ld);
+          if (L == 0) __syncthreads();  // the heads read z directly: acc0 is read before the centre taps below add to it
+          if (tid == 0) {
+            float* ring = smem + p.ring_off[L];
+            ring[(c * 4 + s0) * RP + x + 1] = gm;      // ring entry 2c
+            ring[(c * 4 + 2 + s0) * RP + x + 1] = gs;  // ring entry 2c + 1
+            p.g_u[g] = v;
+          }
+          const IafStageDev& S = p.stage[L];
+          float* acc = smem + p.acc_off[L];
+          for (int ci = tid; ci < S.cin; ci += IAF_INV_THREADS) {
+            const float* wc = S.w + (size_t)ci * S.cout_pad + cm;  // centre tap, heads m_c and s_c
+            acc[ci] = fmaf(__ldg(wc + 4), gs, fmaf(__ldg(wc), gm, acc[ci]));
+          }
+          __syncthreads();
+        }
+        for (int j = L - 1; j >= 0; --j) {
+          const int* off = p.grp + p.grp_off[j];
+          const int b0 = __ldg(off + k), b1 = __ldg(off + k + 1);
+          if (b0 == b1) continue;
+          const int* units = off + C + 2;
+          const float* gacc = smem + p.acc_off[j + 1];  // gradients of stage j's outputs (stage j+1's inputs)
+          const float* h = p.hid[j] + (size_t)n * p.stage[j].cout * HW + gp;
+          float* ring = smem + p.ring_off[j];
+          for (int i = b0 + tid; i < b1; i += IAF_INV_THREADS) {
+            const int u = __ldg(units + i);
+            ring[(u * 2 + s0) * RP + x + 1] = gacc[u] * iaf_inv_nl_grad(__ldg(h + (size_t)u * HW), p.nl);
+          }
+          __syncthreads();
+          const IafStageDev& S = p.stage[j];
+          float* acc = smem + p.acc_off[j];
+          for (int ci = tid; ci < S.cin; ci += IAF_INV_THREADS) {
+            float v = acc[ci];
+            const float* wc = S.w + (size_t)ci * S.cout_pad;  // centre tap, input channel ci
+            for (int i = b0; i < b1; ++i) {
+              const int u = __ldg(units + i);
+              v = fmaf(__ldg(wc + u), ring[(u * 2 + s0) * RP + x + 1], v);
+            }
+            acc[ci] = v;
+          }
+          __syncthreads();
+        }
+      }
+    }
+  }
+}
+
+static cudaError_t iaf_inv_set_smem() {
+  cudaError_t e = iaf_smem_optin(iaf_inv_kernel);
+  return e != cudaSuccess ? e : iaf_smem_optin(iaf_inv_adj_kernel);
+}
 
 static cudaError_t iaf_launch_inv(const IafInvParams& p, int B, size_t smem_bytes, cudaStream_t stream) {
   IAF_LAUNCH(iaf_inv_kernel, B, IAF_INV_THREADS, smem_bytes, stream, p);
   return cudaGetLastError();
 }
 
+static cudaError_t iaf_launch_inv_adj(const IafInvAdjParams& p, int B, size_t smem_bytes, cudaStream_t stream) {
+  IAF_LAUNCH(iaf_inv_adj_kernel, B, IAF_INV_THREADS, smem_bytes, stream, p);
+  return cudaGetLastError();
+}
+
 namespace {
 struct IafInvRegister {
-  IafInvRegister() { iaf_inv = IafInvKernel{iaf_launch_inv, iaf_inv_set_smem}; }
+  IafInvRegister() { iaf_inv = IafInvKernel{iaf_launch_inv, iaf_inv_set_smem, iaf_launch_inv_adj}; }
 } iaf_inv_register;
 }  // namespace

@@ -13,7 +13,8 @@ is in libiaf_b200.so (include/iaf_b200.h).  Three entry points mirror the refere
 * ``IAFOperator.ar_logp(z, context)`` -- the autoregressive (MADE) prior's log-density, the same stack with the
       density epilogue of models.py:304-309 (prior='made')
 * ``IAFOperator.step_inverse(u, context)`` / ``ar_sample(eps, context)`` -- the step run backwards (sequential in the
-      mask's order): sampling the MADE prior
+      mask's order): sampling the MADE prior; ``step_inverse(..., differentiable=True)`` / ``ar_rsample(eps, context)``
+      are the same with a backward (the adjoint, a second sequential kernel): reparameterised samples
 
 Both reference functions are graph builders called once; here they run eagerly per batch,
 so the masked / normalised / packed weights are cached on the operator and re-packed only
@@ -280,10 +281,10 @@ class IAFOperator(object):
             _lib.check(self._lib.iaf_multiconv_fwd_train(plan, _ptr(z), _ptr(context), oarr, harr, B, _stream(z.device)))
         return outs, hidden
 
-    def _step_train_raw(self, z, context):
+    def _step_train_raw(self, z, context, layers=None):
         """iaf_step_fwd_train: the step plus the hidden activations the backward needs (kept by the same kernels)."""
         z, context, B, H, W = self._shapes(z, context)
-        plan = self._plan(H, W, z.device)
+        plan = self._plan(H, W, z.device, layers)
         z_out, logsd = torch.empty_like(z), torch.empty_like(z)
         logdet = torch.empty((B,), device=z.device, dtype=torch.float32)
         hidden = [torch.empty((B, h, H, W), device=z.device, dtype=torch.float32) for h in self.hidden]
@@ -378,15 +379,31 @@ class IAFOperator(object):
 
     def _refuse_grad(self, what, *tensors):
         if self._needs_grad(*tensors):
-            raise NotImplementedError("IAFOperator.%s is not differentiable (the inverse has no backward); call it under "
-                                      "torch.no_grad()" % what)
+            raise NotImplementedError("IAFOperator.%s is not differentiable; call it under torch.no_grad(), or use "
+                                      "step_inverse(..., differentiable=True) / ar_rsample for a reparameterised "
+                                      "sample" % what)
 
-    def step_inverse(self, u, context, want_logsd=True, want_logdet=True):
+    def step_inverse(self, u, context, want_logsd=True, want_logdet=True, differentiable=False):
         """Inverse of :meth:`step`: (z, arw_logsd [B,C,H,W] or None, logdet [B] or None) with
         ``(z - 0.1 m(z)) / exp(0.1 s(z)) = u``, solved in the mask's order by one sequential kernel
-        (iaf_step_inverse); arw_logsd and logdet are ``step(z)``'s own.  Not differentiable: under grad mode with an
-        input or parameter that requires grad it raises NotImplementedError."""
+        (iaf_step_inverse); arw_logsd and logdet are ``step(z)``'s own.  Under grad mode with an input or parameter
+        that requires grad it raises NotImplementedError, unless ``differentiable=True``: then the call is ONE autograd
+        node whose backward solves the adjoint (iaf_step_inverse_adjoint) for the gradient at u and runs the step's own
+        backward at z for the context and parameter gradients.  A map whose adjoint does not fit raises
+        NotImplementedError before anything is launched."""
+        if differentiable and self._needs_grad(u, context):
+            uc, _, B, H, W = self._shapes(u, context)
+            with torch.cuda.device(uc.device):  # B = 0: the plan's check only
+                _lib.check(self._lib.iaf_step_inverse_adjoint(self._plan(H, W, uc.device), None, None, None, None, None,
+                                                              None, None, 0, _stream(uc.device)))
+            self.invalidate()  # training: parameters may have been stepped through .data since the last call
+            flat = [t for l in self._layers for t in l]
+            z, logsd, logdet = _StepInverseFn.apply(self, u, context if self.hidden else None, *flat)
+            return z, (logsd if want_logsd else None), (logdet if want_logdet else None)
         self._refuse_grad("step_inverse", u, context)
+        return self._step_inverse_raw(u, context, want_logsd, want_logdet)
+
+    def _step_inverse_raw(self, u, context, want_logsd=True, want_logdet=True):
         u, context, B, H, W = self._shapes(u, context)
         plan = self._plan(H, W, u.device)
         z = torch.empty_like(u)
@@ -406,6 +423,30 @@ class IAFOperator(object):
         z, logsd, _ = self.step_inverse(eps, context, want_logsd=True, want_logdet=False)
         logps = -0.5 * np.log(2 * np.pi) - logsd - 0.5 * eps * eps
         return z, logps.sum(dim=(2, 3)), logps.sum(dim=(1, 2, 3))
+
+    def ar_rsample(self, eps, context):
+        """:meth:`ar_sample` reparameterised: the same (z, logp_bc, logp), differentiable with respect to ``eps``,
+        ``context`` and the prior's parameters (``step_inverse(..., differentiable=True)``)."""
+        z, logsd, _ = self.step_inverse(eps, context, want_logsd=True, want_logdet=False, differentiable=True)
+        logps = -0.5 * np.log(2 * np.pi) - logsd - 0.5 * eps * eps
+        return z, logps.sum(dim=(2, 3)), logps.sum(dim=(1, 2, 3))
+
+    def _step_inverse_adjoint_raw(self, u, logsd, hidden, g_z, g_logsd=None, g_logdet=None, layers=None):
+        """iaf_step_inverse_adjoint: g_u from the inverse's u and arw_logsd, the hidden activations at z and the upstream
+        gradients (g_logsd, g_logdet may be None)."""
+        u = _check_input(u, "u")
+        B, _, H, W = u.shape
+        plan = self._plan(H, W, u.device, layers)
+        logsd, g_z = _check_input(logsd, "logsd", u.shape), _check_input(g_z, "g_z", u.shape)
+        g_logsd = None if g_logsd is None else _check_input(g_logsd, "g_logsd", u.shape)
+        g_logdet = None if g_logdet is None else _check_input(g_logdet, "g_logdet", (B,))
+        hidden = [_check_input(h, "hidden", (B, n, H, W)) for h, n in zip(hidden, self.hidden)]
+        harr = (C.c_void_p * max(1, len(hidden)))(*[h.data_ptr() for h in hidden])
+        g_u = torch.empty_like(u)
+        with torch.cuda.device(u.device):
+            _lib.check(self._lib.iaf_step_inverse_adjoint(plan, _ptr(u), _ptr(logsd), harr, _ptr(g_z), _ptr(g_logsd),
+                                                          _ptr(g_logdet), _ptr(g_u), B, _stream(u.device)))
+        return g_u
 
     def _ar_logp_train_raw(self, z, context):
         """iaf_ar_logp_fwd_train: the density plus z', made_logsd and the hidden activations its backward needs."""
@@ -523,6 +564,44 @@ class _StepFn(torch.autograd.Function):
         g_z, g_ctx, gw, gs, gb = ctx.op._backward("step", z, context, _regroup(flat), (g_zout, g_logsd, g_logdet), need_params,
                                                    saved=(z_out, logsd, hidden))
         return (None, g_z, g_ctx) + tuple(_flat_param_grads(gw, gs, gb, len(flat) // 3))
+
+
+class _StepInverseFn(torch.autograd.Function):
+    """autograd node of the step's inverse: forward = iaf_step_inverse; backward = the hidden activations at z
+    (iaf_step_fwd_train), the adjoint solve g_u = J^-T (g_z + A^T G_a) (iaf_step_inverse_adjoint), then the step's own
+    backward at z with upstream (-g_u, g_logsd, g_logdet) and kept (u, arw_logsd) for the context and parameter
+    gradients (iaf_step_bwd_saved; its g_z, which is -g_z, is not needed)."""
+
+    @staticmethod
+    def forward(ctx, op, u, context, *flat):
+        with torch.no_grad():
+            z, logsd, logdet = op._step_inverse_raw(u, context)
+        ctx.op = op
+        ctx.has_ctx = context is not None
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(u, *([context] if context is not None else []), z, logsd, *flat)
+        return z, logsd, logdet
+
+    @staticmethod
+    def backward(ctx, g_z, g_logsd, g_logdet):
+        saved = ctx.saved_tensors
+        u = saved[0]
+        context = saved[1] if ctx.has_ctx else None
+        i = 2 if ctx.has_ctx else 1
+        z, logsd = saved[i], saved[i + 1]
+        flat = saved[i + 2:]
+        layers = _regroup(flat)
+        op = ctx.op
+        if g_z is None:
+            g_z = torch.zeros_like(u)
+        hidden = op._step_train_raw(z, context, layers)[3]
+        g_u = op._step_inverse_adjoint_raw(u, logsd, hidden, g_z, g_logsd, g_logdet, layers)
+        need_params = any(ctx.needs_input_grad[3:])
+        g_ctx, gw, gs, gb = None, None, None, None
+        if need_params or (ctx.has_ctx and ctx.needs_input_grad[2]):
+            _, g_ctx, gw, gs, gb = op._backward("step", z, context, layers, (-g_u, g_logsd, g_logdet), need_params,
+                                                saved=(u, logsd, hidden))
+        return (None, g_u, g_ctx) + tuple(_flat_param_grads(gw, gs, gb, len(flat) // 3))
 
 
 class _ArLogpFn(torch.autograd.Function):

@@ -256,6 +256,22 @@ int iaf_ar_logp_bwd_saved(iaf_plan_t* plan, const float* z, const float* z_out, 
 int iaf_step_inverse(iaf_plan_t* plan, const float* u, const float* context, float* z_out,
                      float* logsd_out, float* logdet_out, int B, void* stream);
 
+/*
+ * Adjoint of iaf_step_inverse, for its backward: with z = inverse(u), arw_logsd a(z) and logdet = -sum a, and upstream
+ * gradients g_z [B,n_z,H,W], g_logsd [B,n_z,H,W] and g_logdet [B] (g_logsd and g_logdet may be NULL: a missing one
+ * contributes nothing), writes g_u [B,n_z,H,W] = J^-T (g_z + A^T (g_logsd - g_logdet)), J = d step / d z and A = d a / d z
+ * at z: one triangular solve in the reverse of the mask's order.  Inputs: u, logsd = a(z) (iaf_step_inverse's
+ * logsd_out) and hidden[j] [B,hidden[j],H,W], the hidden activations at z (iaf_step_fwd_train; NULL without hidden
+ * layers).  The context and parameter gradients are the step's own backward at z with upstream -g_u, g_logsd, g_logdet
+ * (iaf_step_bwd_saved with z_out = u), whose g_z is then -g_z.  Allocates nothing (capture-safe); deterministic; one
+ * exact-fp32 kernel on every plan.  IAF_ERR_UNSUPPORTED when the plan has no inverse, or when the two-row window of
+ * every stage's output gradients does not fit in shared memory (4 (2 (W + 2) (2 n_z + sum hidden) + n_z + sum hidden)
+ * bytes, at most 225 KiB).  B == 0 launches nothing and reads no pointer: IAF_OK when the plan has the adjoint.
+ */
+int iaf_step_inverse_adjoint(iaf_plan_t* plan, const float* u, const float* logsd, const float* const* hidden,
+                             const float* g_z, const float* g_logsd, const float* g_logdet, float* g_u, int B,
+                             void* stream);
+
 /* Backward of the un-fused operator iaf_multiconv_fwd: g_outs[k] [B,head[k],H,W] is the
  * gradient at head k.  Same outputs as iaf_step_bwd. */
 int iaf_multiconv_bwd(iaf_plan_t* plan, const float* z, const float* context, const float* const* w,

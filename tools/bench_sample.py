@@ -5,7 +5,9 @@ fixed-point baseline it replaces: z <- 0.1 m(z) + exp(0.1 s(z)) eps, one iaf_ste
 The fixed point is exact after at most n_z*H*W iterations (the length of the dependency chain); the script times K of
 its iterations and reports the per-iteration time, the number of iterations after which the fp32 iterate reaches the
 kernel's own round-trip error on this data (measured, capped), and the products of the per-iteration time with both
-counts, labelled as extrapolated.  Also reports the round-trip error max|step(ar_sample(eps)).z' - eps| on the timed data.
+counts, labelled as extrapolated.  Also reports the round-trip error max|step(ar_sample(eps)).z' - eps| on the timed data,
+and the reparameterised sample's training pair: ar_rsample's forward and the backward of its logp (each call timed on
+its own with CUDA events), and the adjoint kernel (iaf_step_inverse_adjoint) alone.
 Shapes: the prior of c2a (n_z 32, hidden [64]) and c2b (hidden [160, 160]), Theano variant, 16x16, B = 256.  CUDA
 events after a warm-up, the calls alternating over several rounds.  Prints one JSON line with the card's name and power
 limit.
@@ -82,6 +84,42 @@ def main():
                     e1.record()
                     torch.cuda.synchronize()
                     ms[name].append(e0.elapsed_time(e1) / calls)
+        # the reparameterised sample's training pair: ar_rsample with eps, context and the parameters requiring grad,
+        # then the backward of its logp (hidden activations at z, the adjoint, the step's saved backward); and the
+        # adjoint kernel alone on the same data
+        train = [tuple(t.detach().clone().requires_grad_(True) for t in l) for l in dev]
+        top = IAFOperator("theano", n_z, hidden, [n_z, n_z], nl="elu").set_weights(train)
+        eg, cg = e.clone().requires_grad_(True), c.clone().requires_grad_(True)
+        with torch.no_grad():
+            zi, lsi, _ = top.step_inverse(e, c)
+            hid_act = top._step_train_raw(zi, c)[3]
+            g_z, g_ls = torch.randn_like(e), torch.randn_like(e)
+
+        def adjoint():
+            return top._step_inverse_adjoint_raw(e, lsi, hid_act, g_z, g_ls)
+
+        pair = {"ar_rsample_fwd": [], "ar_rsample_bwd": [], "adjoint_kernel": []}
+        for r in range(rounds + 1):  # round 0: warm-up
+            for _ in range(calls):
+                ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+                ev[0].record()
+                lp = top.ar_rsample(eg, cg)[2]
+                ev[1].record()
+                lp.sum().backward()
+                ev[2].record()
+                torch.cuda.synchronize()
+                if r:
+                    pair["ar_rsample_fwd"].append(ev[0].elapsed_time(ev[1]))
+                    pair["ar_rsample_bwd"].append(ev[1].elapsed_time(ev[2]))
+            with torch.no_grad():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(calls):
+                    adjoint()
+                e1.record()
+                torch.cuda.synchronize()
+                if r:
+                    pair["adjoint_kernel"].append(e0.elapsed_time(e1) / calls)
         med = {name: statistics.median(v) for name, v in ms.items()}
         it_ms = med["fixed_point_iteration"]
         out[shape] = {
@@ -90,7 +128,10 @@ def main():
             "fixed_point_iterations_to_kernel_roundtrip": iters if iters is not None else "more than %d" % cap,
             "extrapolated_fixed_point_ms_at_chain_length": it_ms * n_z * H * W,
             "extrapolated_fixed_point_ms_at_measured_iterations": (it_ms * iters) if iters is not None else None,
-            "roundtrip_max_abs_err": rt}
+            "roundtrip_max_abs_err": rt,
+            "ar_rsample_fwd_ms": statistics.median(pair["ar_rsample_fwd"]),
+            "ar_rsample_bwd_ms": statistics.median(pair["ar_rsample_bwd"]),
+            "adjoint_kernel_ms": statistics.median(pair["adjoint_kernel"])}
     print(json.dumps(out))
 
 
