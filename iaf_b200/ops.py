@@ -390,12 +390,15 @@ class IAFOperator(object):
         that requires grad it raises NotImplementedError, unless ``differentiable=True``: then the call is ONE autograd
         node whose backward solves the adjoint (iaf_step_inverse_adjoint) for the gradient at u and runs the step's own
         backward at z for the context and parameter gradients.  A map whose adjoint does not fit raises
-        NotImplementedError before anything is launched."""
+        NotImplementedError before anything is launched, and so does a map the step's backward does not take when the
+        context or a parameter requires grad (only the gradient at u needs no step backward)."""
         if differentiable and self._needs_grad(u, context):
-            uc, _, B, H, W = self._shapes(u, context)
+            uc, cc, B, H, W = self._shapes(u, context)
             with torch.cuda.device(uc.device):  # B = 0: the plan's check only
                 _lib.check(self._lib.iaf_step_inverse_adjoint(self._plan(H, W, uc.device), None, None, None, None, None,
                                                               None, None, 0, _stream(uc.device)))
+            if (cc is not None and cc.requires_grad) or any(t.requires_grad for l in self._layers for t in l):
+                self.backward_path(H, W, uc.device)  # creates the step's backward plan, or raises
             self.invalidate()  # training: parameters may have been stepped through .data since the last call
             flat = [t for l in self._layers for t in l]
             z, logsd, logdet = _StepInverseFn.apply(self, u, context if self.hidden else None, *flat)
