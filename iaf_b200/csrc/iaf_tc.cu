@@ -41,8 +41,8 @@
 #define TC_ZITEMS 4  // z-window (slot, chunk) items per epilogue thread of the stage kernel
 
 struct IafTcStage {
-  const __nv_bfloat16* whi;  // global packed [K/8][N][8]
-  const __nv_bfloat16* wlo;
+  const __nv_bfloat16* whi;  // global packed [K/8][N][8], or for SPLIT stages [K/8][2 NS][8] lo and hi (LY_SPLIT_NGW)
+  const __nv_bfloat16* wlo;  // the lo image [K/8][N][8]; unused by SPLIT stages
   const float* bias;         // [N] packed column order
   const float* padw;         // [4][N] or nullptr
   const float* wsinv;        // [N] packed column order: the inverse of the power of two each weight column carries
@@ -309,12 +309,14 @@ __device__ __forceinline__ SlotInfo decode_slot(const IafTcParams& p, int s, int
 
 // ------------------------------------------------------------------------------------------
 // weight preparation for this path: same math as iaf_pack.cu, fp16 hi/lo split, written as
-// the wgmma B-operand image [K/8][N][8] (K index [ci / 16][tap][ci % 16], K-major, no swizzle).
+// the wgmma B-operand images [K/8][N][8] (K index [ci / 16][tap][ci % 16], K-major, no swizzle), or for a SPLIT stage
+// the one image [K/8][2 NS][8] (see LY_SPLIT_NGW).
 // ------------------------------------------------------------------------------------------
 struct TcPackLayer {
   const float* w; const float* scale; const float* bias;
   __nv_bfloat16* whi; __nv_bfloat16* wlo; float* bias_out; float* padw_out; float* wsinv_out;
   int cin, cout, N, zerodiag, head, is_head;
+  int NS;  // SPLIT stage: the span NS, lo and hi in whi; 0: separate images
 };
 struct TcPackParams {
   TcPackLayer layer[IAF_MAX_HIDDEN + IAF_MAX_HEADS];
@@ -381,9 +383,14 @@ __global__ void __launch_bounds__(128) iaf_tc_pack_kernel(const __grid_constant_
       const __half lh = __float2half_rn(vc - __half2float(hh));
       const __nv_bfloat16 h = __ushort_as_bfloat16(__half_as_ushort(hh));  // raw 16-bit patterns travel in the bf16-typed images
       const __nv_bfloat16 l = __ushort_as_bfloat16(__half_as_ushort(lh));
-      const size_t o = ((size_t)(k >> 3) * L.N + col) * 8 + (k & 7);  // hi / lo images [K/8][N][8]
-      L.whi[o] = h;
-      L.wlo[o] = l;
+      const size_t o = ((size_t)(k >> 3) * (L.NS ? 2 * L.NS : L.N) + col) * 8 + (k & 7);
+      if (L.NS) {
+        L.whi[o] = l;
+        L.whi[o + (size_t)L.NS * 8] = h;
+      } else {
+        L.whi[o] = h;
+        L.wlo[o] = l;
+      }
     } else {
       const int t = t_pad0 + e - n_real;
       if (t > 0) L.padw_out[(size_t)(t - 1) * L.N + col] = tc_masked_weight(L, p.vf, t, L.cin, co) * factor;
@@ -403,8 +410,9 @@ struct IafTcPlan {
   IafVariantFlags vf;
   int n_stages;
   int cin[IAF_MAX_STAGES], N[IAF_MAX_STAGES], K[IAF_MAX_STAGES];
+  int NS[IAF_MAX_STAGES];    // ly_split_span of the kernel that runs the stage
   __nv_bfloat16* whi[IAF_MAX_STAGES];
-  __nv_bfloat16* wlo[IAF_MAX_STAGES];
+  __nv_bfloat16* wlo[IAF_MAX_STAGES];  // null for SPLIT stages
   float* bias[IAF_MAX_STAGES];
   float* padw[IAF_MAX_STAGES];
   float* wsinv[IAF_MAX_STAGES];  // [N]: inverse weight scale of each packed column
@@ -457,6 +465,18 @@ static LyKernel ly_kernel_for(bool padw, int mode, bool elu, int N) {
 #define FZ_NGW 2
 static LyKernel fz_kernel_for(bool padw, int mode, bool elu) { return ly_kernel_pick<FZ_NGW, true>(padw, mode, elu); }
 
+// The weight images of a stage of N columns, as the kernel that runs it (per-stage, or one-launch: fused) reads them:
+// NS = 32 NGW, the span of a SPLIT stage, whose hi and lo columns share one image (LY_SPLIT_NGW); 0 for a wider stage,
+// which has a hi and a lo image
+static int ly_split_span(int N, bool fused) {
+  const int ngw = fused ? FZ_NGW : (N + 31) / 32;
+  return ngw <= LY_SPLIT_NGW ? 32 * ngw : 0;
+}
+// bytes of one weight chunk (LY_KC K-steps of 16), hi and lo
+static int ly_chunk_bytes(int N, int NS) { return LY_KC * 2 * 2 * (NS ? NS : N) * 16; }
+// bytes of the hi image, or of a SPLIT stage's one image
+static size_t ly_image_bytes(int K, int N, int NS) { return (size_t)K * (NS ? 2 * NS : N) * 2; }
+
 static int tc_round_up(int a, int b) { return (a + b - 1) / b * b; }
 
 // per stage: an A window (first stage), the bias table, the partial scratch, the accumulator tile, an NB-deep ring.
@@ -495,7 +515,8 @@ static bool ly_layout(const iaf_desc_t* d, IafTcPlan* pl) {
     q->ly_sm_acc[j] = off; off += TC_TILE * ly_acc_pitch(q->N[j]) * 4;
     off = tc_round_up(off, 128);
     q->ly_sm_b[j] = off;
-    const int slot = 2 * LY_KC * 2 * q->N[j] * 16 + (j ? 4 * q->WIN * 16 : 0);  // weight chunk hi+lo (+ A chunk pair hi+lo)
+    // weight chunk hi+lo (+ A chunk pair hi+lo)
+    const int slot = ly_chunk_bytes(q->N[j], ly_split_span(q->N[j], false)) + (j ? 4 * q->WIN * 16 : 0);
     q->ly_stage[j] = slot;
     int nb = (TC_SMEM_LIMIT - LY_B_SLACK - off) / slot;
     if (nb < 2) return false;
@@ -522,7 +543,7 @@ static bool fz_layout(const iaf_desc_t* d, IafTcPlan* q) {
   off = tc_round_up(off, 16);
   q->fz_sm_acc = off; off += TC_TILE * ly_acc_pitch(std::max(q->N[0], q->N[1])) * 4;
   off = tc_round_up(off, 128);
-  for (int j = 0; j < 2; ++j) { q->fz_sm_b[j] = off; off += 2 * q->K[j] * q->N[j] * 2; }
+  for (int j = 0; j < 2; ++j) { q->fz_sm_b[j] = off; off += (int)ly_image_bytes(q->K[j], q->N[j], ly_split_span(q->N[j], true)); }
   off += LY_B_SLACK;
   q->fz_smem = (size_t)off;
   return off <= TC_SMEM_LIMIT;
@@ -546,9 +567,10 @@ int iaf_tc_plan_create(IafTcPlan** out, const iaf_desc_t* d) {
   if (prop.major != 9) { delete pl; return IAF_ERR_UNSUPPORTED; }  // wgmma: sm_90a
   pl->num_sms = iaf_plan_num_sms(prop.multiProcessorCount);
   for (int j = 0; j < pl->n_stages; ++j) {
-    const size_t wb = (size_t)pl->K[j] * pl->N[j] * 2;
+    pl->NS[j] = ly_split_span(pl->N[j], pl->fused);
+    const size_t wb = ly_image_bytes(pl->K[j], pl->N[j], pl->NS[j]);
     // bias [N] and pad-channel weights [4][N] are ONE table [5][N]; the inverse weight scales [N] follow it
-    if (cudaMalloc(&pl->whi[j], wb) != cudaSuccess || cudaMalloc(&pl->wlo[j], wb) != cudaSuccess ||
+    if (cudaMalloc(&pl->whi[j], wb) != cudaSuccess || (!pl->NS[j] && cudaMalloc(&pl->wlo[j], wb) != cudaSuccess) ||
         cudaMalloc(&pl->bias[j], sizeof(float) * 6 * pl->N[j]) != cudaSuccess) {
       iaf_tc_plan_destroy(pl);
       return IAF_ERR_CUDA;
@@ -593,9 +615,9 @@ int iaf_tc_pack(IafTcPlan* pl, const float* const* w, const float* const* scale,
   pp.vf = pl->vf;
   int max_cout = 0;
   for (int j = 0; j < pl->n_stages; ++j) {
-    const size_t wb = (size_t)pl->K[j] * pl->N[j] * 2;
+    const size_t wb = ly_image_bytes(pl->K[j], pl->N[j], pl->NS[j]);
     if (cudaMemsetAsync(pl->whi[j], 0, wb, stream) != cudaSuccess) return IAF_ERR_CUDA;
-    if (cudaMemsetAsync(pl->wlo[j], 0, wb, stream) != cudaSuccess) return IAF_ERR_CUDA;
+    if (pl->wlo[j] && cudaMemsetAsync(pl->wlo[j], 0, wb, stream) != cudaSuccess) return IAF_ERR_CUDA;
     if (cudaMemsetAsync(pl->padw[j], 0, sizeof(float) * 4 * pl->N[j], stream) != cudaSuccess) return IAF_ERR_CUDA;
   }
   for (int i = 0; i < pp.n_layers; ++i) {
@@ -608,6 +630,7 @@ int iaf_tc_pack(IafTcPlan* pl, const float* const* w, const float* const* scale,
     L.cin = pl->cin[j];
     L.cout = is_head ? d.head[i - d.n_hidden] : d.hidden[i];
     L.N = pl->N[j];
+    L.NS = pl->NS[j];
     L.zerodiag = is_head ? 1 : 0;
     L.is_head = is_head ? 1 : 0;
     L.head = is_head ? i - d.n_hidden : 0;
@@ -736,9 +759,9 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
     q.NB = LY_MAX_NB;
     q.sm_a = pl->fz_sm_a; q.sm_h = pl->fz_sm_h; q.sm_bias = pl->fz_sm_bias[0]; q.sm_bias1 = pl->fz_sm_bias[1];
     q.sm_part = pl->fz_sm_part; q.sm_acc = pl->fz_sm_acc; q.sm_b = pl->fz_sm_b[0]; q.sm_b1 = pl->fz_sm_b[1];
-    q.b_chunk_bytes = LY_KC * 2 * pl->N[0] * 16; q.n_bchunks = (pl->K[0] / 16) / LY_KC;
-    q.b_chunk_bytes1 = LY_KC * 2 * pl->N[1] * 16; q.n_bchunks1 = (pl->K[1] / 16) / LY_KC;
-    q.stage_bytes = 2 * q.b_chunk_bytes;
+    q.b_chunk_bytes = ly_chunk_bytes(pl->N[0], pl->NS[0]); q.n_bchunks = (pl->K[0] / 16) / LY_KC;
+    q.b_chunk_bytes1 = ly_chunk_bytes(pl->N[1], pl->NS[1]); q.n_bchunks1 = (pl->K[1] / 16) / LY_KC;
+    q.stage_bytes = q.b_chunk_bytes;
     q.TS = TS; q.TO = TS;
     q.tl_enable = 1;
     if (!launch(fz_kernel_for(padw, a->mode, elu), q, pl->fz_smem)) return IAF_ERR_CUDA;
@@ -767,7 +790,7 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
     q.NB = pl->ly_NB[j];
     q.sm_a = pl->ly_sm_a[j]; q.sm_b = pl->ly_sm_b[j]; q.sm_bias = pl->ly_sm_bias[j]; q.sm_part = pl->ly_sm_part[j];
     q.sm_acc = pl->ly_sm_acc[j];
-    q.b_chunk_bytes = LY_KC * 2 * pl->N[j] * 16;
+    q.b_chunk_bytes = ly_chunk_bytes(pl->N[j], pl->NS[j]);
     q.stage_bytes = pl->ly_stage[j];
     q.n_bchunks = (pl->K[j] / 16) / LY_KC;
     { const char* tls = getenv("IAF_TL_STAGE"); q.tl_enable = tls ? (atoi(tls) == j) : (j == pl->n_stages - 1); }
@@ -793,8 +816,9 @@ struct IafDgPlan {
   int grad_flip;  // the gradient stream: the point reflection of the forward's (1 - IafVariantFlags::reflect)
   int n_stages;
   int kin[IAF_MAX_STAGES], nout[IAF_MAX_STAGES];  // dgrad of layer j: input planes (= packed columns of layer j), output channels (= cin of layer j)
+  int ns[IAF_MAX_STAGES];    // ly_split_span of the stage
   __nv_bfloat16* whi[IAF_MAX_STAGES];
-  __nv_bfloat16* wlo[IAF_MAX_STAGES];
+  __nv_bfloat16* wlo[IAF_MAX_STAGES];  // null for SPLIT stages
   float* zeros;  // bias table of the stages (the kernel adds it; the gradient has none): [5][maxn]
   int maxn;
   int sm_bias[IAF_MAX_STAGES], sm_part[IAF_MAX_STAGES], sm_acc[IAF_MAX_STAGES], sm_b[IAF_MAX_STAGES], stage[IAF_MAX_STAGES],
@@ -833,23 +857,27 @@ __global__ void __launch_bounds__(1024) iaf_dg_wscale_kernel(const float4* __res
 }
 
 __global__ void __launch_bounds__(256) iaf_dg_pack_kernel(const float* __restrict__ w, const float* __restrict__ wscale,
-                                                          __nv_bfloat16* whi, __nv_bfloat16* wlo, int cin, int ncol) {
+                                                          __nv_bfloat16* whi, __nv_bfloat16* wlo, int cin, int ncol,
+                                                          int ns) {
   // w: effective (masked, normalised) forward weights [tap][cin][ncol] fp32, times the stage's weight scale.  B operand of
   // the data gradient: K index [column / 16][tap][column % 16] (the layered kernel's K order), N index = ci; images
-  // [K/8][N][8], fp16 hi / lo.
-  const int total = IAF_NTAPS * cin * ncol;
+  // [K/8][N][8], fp16 hi / lo, or for a SPLIT stage (ns = its span) one image [K/8][2 ns][8] whose columns ci >= cin of
+  // both halves are written as zeros here.
+  const int nc = ns ? ns : cin;
+  const int total = IAF_NTAPS * nc * ncol;
   const float sw = __ldg(wscale);
   for (int i = blockIdx.x * 256 + threadIdx.x; i < total; i += gridDim.x * 256) {
     const int kc = i % ncol;
-    const int ci = (i / ncol) % cin;
-    const int t = i / (ncol * cin);
-    const float vc = fminf(fmaxf(w[i] * sw, -65000.f), 65000.f);
+    const int ci = (i / ncol) % nc;
+    const int t = i / (ncol * nc);
+    const float vc = ci < cin ? fminf(fmaxf(w[((size_t)t * cin + ci) * ncol + kc] * sw, -65000.f), 65000.f) : 0.f;
     const __half hh = __float2half_rn(vc);
     const __half lh = __float2half_rn(vc - __half2float(hh));
     const int k = ((kc >> 4) * IAF_NTAPS + t) * 16 + (kc & 15);
-    const size_t o = ((size_t)(k >> 3) * cin + ci) * 8 + (k & 7);
-    whi[o] = __ushort_as_bfloat16(__half_as_ushort(hh));
-    wlo[o] = __ushort_as_bfloat16(__half_as_ushort(lh));
+    const size_t o = ((size_t)(k >> 3) * (ns ? 2 * ns : cin) + ci) * 8 + (k & 7);
+    __nv_bfloat16* lo = ns ? whi : wlo;
+    whi[o + (size_t)ns * 8] = __ushort_as_bfloat16(__half_as_ushort(hh));
+    lo[o] = __ushort_as_bfloat16(__half_as_ushort(lh));
   }
 }
 
@@ -974,14 +1002,15 @@ int iaf_dg_plan_create(IafDgPlan** out, const iaf_desc_t* d, const int* cin, con
     pl->sm_acc[j] = off; off += TC_TILE * ly_acc_pitch(N) * 4;
     off = tc_round_up(off, 128);
     pl->sm_b[j] = off;
-    const int slot = 2 * LY_KC * 2 * N * 16 + 4 * pl->WIN * 16;  // weight chunk hi+lo + A chunk pair hi+lo
+    pl->ns[j] = ly_split_span(N, false);
+    const int slot = ly_chunk_bytes(N, pl->ns[j]) + 4 * pl->WIN * 16;  // weight chunk hi+lo + A chunk pair hi+lo
     pl->stage[j] = slot;
     const int nb = (TC_SMEM_LIMIT - LY_B_SLACK - off) / slot;
     if (nb < 2) { iaf_dg_plan_destroy(pl); return IAF_ERR_UNSUPPORTED; }
     pl->NB[j] = std::min(nb, LY_MAX_NB);
     pl->smem[j] = (size_t)off + (size_t)pl->NB[j] * slot + LY_B_SLACK;
-    const size_t wb = (size_t)IAF_NTAPS * kin * N * 2;
-    if (cudaMalloc(&pl->whi[j], wb) != cudaSuccess || cudaMalloc(&pl->wlo[j], wb) != cudaSuccess) {
+    const size_t wb = ly_image_bytes(IAF_NTAPS * kin, N, pl->ns[j]);
+    if (cudaMalloc(&pl->whi[j], wb) != cudaSuccess || (!pl->ns[j] && cudaMalloc(&pl->wlo[j], wb) != cudaSuccess)) {
       iaf_dg_plan_destroy(pl);
       return IAF_ERR_CUDA;
     }
@@ -1066,8 +1095,9 @@ int iaf_dg_stage(IafDgPlan* pl, int j, const float* w_packed, int in_buf, const 
   {
     const int total = IAF_NTAPS * N * kin;
     iaf_dg_wscale_kernel<<<1, 1024, 0, stream>>>(reinterpret_cast<const float4*>(w_packed), total / 4, pl->wscale + j);
-    iaf_dg_pack_kernel<<<std::min(592, (total + 255) / 256), 256, 0, stream>>>(w_packed, pl->wscale + j, pl->whi[j],
-                                                                              pl->wlo[j], N, kin);
+    const int total_img = IAF_NTAPS * (pl->ns[j] ? pl->ns[j] : N) * kin;
+    iaf_dg_pack_kernel<<<std::min(592, (total_img + 255) / 256), 256, 0, stream>>>(w_packed, pl->wscale + j, pl->whi[j],
+                                                                                  pl->wlo[j], N, kin, pl->ns[j]);
     if (cudaGetLastError() != cudaSuccess) return IAF_ERR_CUDA;
   }
   const int SPS = (d.H + 1) * (d.W + 1);
@@ -1099,7 +1129,7 @@ int iaf_dg_stage(IafDgPlan* pl, int j, const float* w_packed, int in_buf, const 
   q.first = hprev ? 1 : 0;
   q.NB = pl->NB[j];
   q.sm_a = 0; q.sm_b = pl->sm_b[j]; q.sm_bias = pl->sm_bias[j]; q.sm_part = pl->sm_part[j]; q.sm_acc = pl->sm_acc[j];
-  q.b_chunk_bytes = LY_KC * 2 * N * 16;
+  q.b_chunk_bytes = ly_chunk_bytes(N, pl->ns[j]);
   q.stage_bytes = pl->stage[j];
   q.n_bchunks = kin / 16;
   q.bwd = hprev ? 1 : 2;

@@ -9,8 +9,9 @@
 //     K-steps through an NB-deep shared-memory ring (cp.async.bulk + expect_tx on an mbarrier); both MMA warpgroups
 //     release a ring stage once their wgmma reads of it have completed;
 //   * five warpgroups with their own jobs: warpgroups 0 and 1 issue the MMAs, warpgroup r for rows [64 r, +64) of the
-//     tile and ALL of the stage's columns (one wgmma m64nNk16 per K-step, tap and product; two of half the width for
-//     stages of 129-160 columns; two passes over K for 161-192), accumulating in registers; warpgroups 2 and 3 build the first stage's z window and
+//     tile and ALL of the stage's columns (one wgmma m64nNk16 per K-step, tap and product; two per K-step and tap, the
+//     second of twice the width, for spans of at most 64 columns; two of half the width for stages of 129-160 columns;
+//     two passes over K for 161-192), accumulating in registers; warpgroups 2 and 3 build the first stage's z window and
 //     run the epilogues; in warpgroup 4, warp 16 is the producer and warp 17 the reducer.  setmaxnreg moves registers
 //     from warpgroup 4 to the MMA warpgroups;
 //   * the accumulators go through a shared-memory tile [128][N + 4] so that the epilogue keeps one thread per slot
@@ -41,10 +42,15 @@
 #define LY_PART_SETS 16
 #define LY_KC 5        // K-steps (of 16) per weight chunk
 #define LY_MAX_NB 6
-// Bytes every layout of the stage kernel reserves past its last weight image: the column span of an MMA warpgroup (see
-// ly_mma_tile), 32 NGW columns, of the last K plane reads up to 16 * (32 * NGW - N) bytes past the plane's end -- 256 for
-// the per-stage instantiations (NGW = ceil(N / 32)), 768 for the fused one (NGW = 2, N down to 16: hidden [16]) -- and
-// that read must stay inside the CTA's allocation.  (The previous layout's second column half ended at the same byte.)
+// Stages whose MMA warpgroup spans at most 32 LY_SPLIT_NGW columns (SPLIT, see ly_mma_tile) sum the correction products
+// apart and keep their weights as one image [K/8][2 NS][8], NS = 32 NGW the span: each K plane holds the lo columns
+// [0, NS), then the hi columns [NS, 2 NS), both halves zero from N on.  Wider stages keep a hi and a lo image [K/8][N][8].
+#define LY_SPLIT_NGW 2
+// Bytes every layout of the stage kernel reserves past its last weight image.  A SPLIT stage's spans end inside their K
+// plane.  A wider stage's span, 32 NGW columns with NGW = ceil(N / 32), of the last K plane reads up to
+// 16 * (32 * NGW - N) = 256 bytes past the plane's end, and that read must stay inside the CTA's allocation.  The
+// reserve is kept at 1024 bytes, as when the one-launch kernel's spans could read 768 bytes past N = 16, so that every
+// layout's size, and with it which stacks run in one launch, is unchanged.
 #define LY_B_SLACK 1024
 
 enum { LB_BFULL = 0, LB_BEMPTY = LY_MAX_NB, LB_PART = 2 * LY_MAX_NB,
@@ -67,8 +73,8 @@ struct IafLyParams {
   int first;                   // 1: first stage (adds the context)
   int NB;                      // weight ring depth
   int sm_a, sm_b, sm_bias, sm_part, sm_acc;
-  int stage_bytes;             // bytes of one ring stage: 2 * b_chunk_bytes (+ 4 * WIN * 16 when the A pair rides along)
-  int b_chunk_bytes;           // bytes of one ring slot half (hi or lo): LY_KC * 2 * N * 16
+  int stage_bytes;             // bytes of one ring stage: b_chunk_bytes (+ 4 * WIN * 16 when the A pair rides along)
+  int b_chunk_bytes;           // bytes of one weight chunk, hi and lo: LY_KC * 2 planes of 2 NS (SPLIT) or 2 N columns
   int n_bchunks;               // weight chunks per tile
   int tl_enable;               // timeline builds only: this launch flushes its events
   // one-launch step for stacks with one hidden layer (the FUSED instantiation): t.st[0] is the hidden layer, t.st[1] the
@@ -109,14 +115,20 @@ __device__ __forceinline__ float dg_scale_from_amax(float amax) {
 
 // The MMAs of one stage (or one pass over it) for one tile, run by the two MMA warpgroups.  Warpgroup r computes rows
 // [64 r, +64) and the 16 SPG columns from col0: D[64 x 16 SPG] += A_t[64 x 16] B_t[16 x 16 SPG] over K-steps, taps and
-// the three split products, accumulating in registers (acc; returned with the correction sum added).  Each product is
-// one wgmma over the span (NI = 1), or for 160 columns two of half the span (NI = 2): an m64n160 instruction needs more
-// registers than the launch's 96 by itself, although all 80 accumulators fit after setmaxnreg.  The halves' fragments sit
-// side by side in acc exactly as one instruction's would.  In the B image [K/8][N][8] a span of contiguous columns is one
-// K-major descriptor (8-column groups 128 B apart, the two K halves one plane apart).  NGW is a compile-time count: a span
-// past the stage's columns computes on whatever follows in shared memory -- the next K plane, the next image, or the
-// LY_B_SLACK bytes every layout reserves past its last one -- and is not stored, so every wgmma is issued
-// unconditionally and ptxas keeps them asynchronous.
+// the three split products, accumulating in registers (returned in acc[0, 8 SPG) with the correction sum added).  A
+// span of contiguous columns of a B image is one K-major descriptor (8-column groups 128 B apart, the two K halves one
+// plane apart).  SPLIT stages (NGW <= LY_SPLIT_NGW) hold [W_lo | W_hi] in each K plane, so A_hi is fetched once for both
+// of its products: per K-step and tap, the correction sum acc[0, 8 SPG) += A_lo W_hi over the span, then one
+// instruction of twice the span computes A_hi [W_lo | W_hi] into all of acc, the main sum in acc[8 SPG, 16 SPG).  Each
+// sum adds the same products in the same order as three instructions of the span would.  The correction sum comes
+// first because ptxas keeps a wgmma whose accumulators are a prefix of the next one's asynchronous, and serializes
+// every wgmma of the kernel when they are a suffix.  Wider stages issue each product as one wgmma over the span (NI = 1),
+// or for 160 columns two of half the span (NI = 2): an m64n160 instruction needs more registers than the launch's 96 by
+// itself, although all 80 accumulators fit after setmaxnreg.  The halves' fragments sit side by side in acc exactly as
+// one instruction's would.  NGW is a compile-time count: a span past the stage's columns computes on zeros (SPLIT) or
+// on whatever follows in shared memory -- the next K plane, the next image, or the LY_B_SLACK bytes every layout
+// reserves past its last one -- and is not stored, so every wgmma is issued unconditionally and ptxas keeps them
+// asynchronous.
 //   ring: the tile's weight chunks are the CTA's gchunk, gchunk + 1, ... (every tile streams all n_chunks); chunk g sits
 //   in ring stage g % NB (parity from g / NB), released after its MMAs complete;
 //   otherwise resident: chunk c sits in stage c behind barrier bar0 + c (parity 0).
@@ -129,14 +141,16 @@ __device__ __forceinline__ void mma_bar_sync() { asm volatile("bar.sync 1, %0;" 
 template <int SPG, bool SPLIT>
 __device__ __forceinline__ void ly_mma_tile(float* acc, uint64_t* bars, int N, int col0, int n_chunks, bool ring, int NB,
                                             int gchunk, int bar0, uint32_t b_addr0, uint32_t stage_bytes,
-                                            uint32_t b_chunk_bytes, bool a_in_stage, uint32_t a_addr, uint32_t a_plane,
+                                            uint32_t b_lo_off, bool a_in_stage, uint32_t a_addr, uint32_t a_plane,
                                             uint32_t a_lo_off, int Wp, int a_release) {
   constexpr int NA = 8 * SPG;          // accumulators per thread: 64 x 16 SPG over the 128 threads of the warpgroup
   constexpr int NI = SPG > 8 ? 2 : 1;  // wgmma instructions per product
   constexpr int GI = SPG / NI;         // 16-column groups per instruction
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rh = warp >> 2, wl = warp & 3;
-  const uint32_t b_plane = (uint32_t)N * 16u;
+  // bytes per K plane of the B image: SPLIT, the span's lo and hi columns; otherwise the N columns of the hi (lo) image,
+  // whose chunk sits b_lo_off bytes after the hi one's in a ring stage
+  const uint32_t b_plane = SPLIT ? 2u * 16u * SPG * 16u : (uint32_t)N * 16u;
   const uint32_t sh[IAF_NTAPS] = {0u, 1u, (uint32_t)(Wp - 1), (uint32_t)Wp, (uint32_t)(Wp + 1)};  // 16-byte units
   const uint32_t a_kstep = (2u * a_plane) >> 4, b_tstep = (2u * b_plane) >> 4;
   const uint32_t a_row = (uint32_t)(rh * 64);  // 64 slots = 64 descriptor units
@@ -144,14 +158,9 @@ __device__ __forceinline__ void ly_mma_tile(float* acc, uint64_t* bars, int N, i
   // added one by one to the main sum, each is rounded at the main sum's magnitude by the tensor cores' accumulation, and
   // over K = 160 those roundings reach ~2e-7 of a unit pre-activation -- enough to put a ReLU's derivative on the wrong
   // side of a pre-activation that small.  Summed apart and added once at the end, they cost one rounding.  Stages of at
-  // most 64 columns do so.
-  float acl[SPLIT ? NA : 1];
+  // most 64 columns do so, in acc[0, NA), the main sum in acc[NA, 2 NA).
 #pragma unroll
-  for (int e = 0; e < NA; ++e) {
-    acc[e] = 0.f;
-    if (SPLIT) acl[SPLIT ? e : 0] = 0.f;
-  }
-  float* corr = SPLIT ? acl : acc;
+  for (int e = 0; e < (SPLIT ? 2 : 1) * NA; ++e) acc[e] = 0.f;
   int prev_stg = -1;
   for (int c = 0; c < n_chunks; ++c) {
     const int stg = ring ? (int)((uint32_t)gchunk % (uint32_t)NB) : c;
@@ -169,18 +178,23 @@ __device__ __forceinline__ void ly_mma_tile(float* acc, uint64_t* bars, int N, i
     }
     ah0 += a_row; al0 += a_row;
     const uint32_t bh0 = wg_desc_lo(bbase, b_plane) + (uint32_t)col0;  // 16 B per column
-    const uint32_t bl0 = wg_desc_lo(bbase + b_chunk_bytes, b_plane) + (uint32_t)col0;
+    const uint32_t bl0 = SPLIT ? 0u : wg_desc_lo(bbase + b_lo_off, b_plane) + (uint32_t)col0;
     wgmma_fence();
 #pragma unroll 1
     for (int t = 0; t < IAF_NTAPS; ++t) {
       const uint64_t ah = mk_desc(ah0 + sh[t]), al = mk_desc(al0 + sh[t]);
       const uint32_t bt = (uint32_t)t * b_tstep;
+      if constexpr (SPLIT) {
+        wgmma_m64nNk16<SPG>(acc, al, mk_desc(bh0 + bt + 16u * SPG));  // W_hi: NS columns into the plane
+        wgmma_m64nNk16<2 * SPG>(acc, ah, mk_desc(bh0 + bt));
+      } else {
 #pragma unroll
-      for (int h = 0; h < NI; ++h) {  // instruction h: columns [16 GI h, +16 GI), 16 B per column in the descriptor
-        const uint32_t bc = bt + (uint32_t)(16 * GI * h);
-        wgmma_m64nNk16<GI>(corr + 8 * GI * h, al, mk_desc(bh0 + bc));
-        wgmma_m64nNk16<GI>(corr + 8 * GI * h, ah, mk_desc(bl0 + bc));
-        wgmma_m64nNk16<GI>(acc + 8 * GI * h, ah, mk_desc(bh0 + bc));
+        for (int h = 0; h < NI; ++h) {  // instruction h: columns [16 GI h, +16 GI), 16 B per column in the descriptor
+          const uint32_t bc = bt + (uint32_t)(16 * GI * h);
+          wgmma_m64nNk16<GI>(acc + 8 * GI * h, al, mk_desc(bh0 + bc));
+          wgmma_m64nNk16<GI>(acc + 8 * GI * h, ah, mk_desc(bl0 + bc));
+          wgmma_m64nNk16<GI>(acc + 8 * GI * h, ah, mk_desc(bh0 + bc));
+        }
       }
     }
     wgmma_commit();
@@ -197,7 +211,7 @@ __device__ __forceinline__ void ly_mma_tile(float* acc, uint64_t* bars, int N, i
   }
   if (SPLIT) {
 #pragma unroll
-    for (int e = 0; e < NA; ++e) acc[e] += acl[SPLIT ? e : 0];
+    for (int e = 0; e < NA; ++e) acc[e] = acc[NA + e] + acc[e];
   }
 }
 
@@ -249,7 +263,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   // the tile's chunks once per pass)
   constexpr int NP = NGW > 5 ? 2 : 1;
   constexpr int SPG = 2 * NGW / NP;
-  constexpr bool SPLIT = NGW <= 2;
+  constexpr bool SPLIT = NGW <= LY_SPLIT_NGW;
 
   // programmatic dependent launch: everything up to the barrier init overlaps the previous grid
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -295,16 +309,15 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       // ===================== producer: A windows (operand-image input) and the weight ring =====================
       if (lane == 0 && FUSED) {
         // both stages' weights, resident: hidden chunk c behind barrier c, heads chunk c behind barrier n_bchunks + c
+        static_assert(!FUSED || SPLIT, "the one-launch kernel's images are [W_lo | W_hi] planes");
         for (int s = 0; s < 2; ++s) {
           const IafTcStage& S = p.st[s];
           const int nb = s ? q.n_bchunks1 : q.n_bchunks, bcb = s ? q.b_chunk_bytes1 : q.b_chunk_bytes;
           uint8_t* base = smem + (s ? q.sm_b1 : q.sm_b);
           for (int c = 0; c < nb; ++c) {
             uint64_t* bar = &bars[LB_BFULL + (s ? q.n_bchunks : 0) + c];
-            const size_t bo = (size_t)c * bcb;
-            mbar_expect_tx(bar, (uint32_t)(2 * bcb));
-            bulk_g2s(base + 2 * c * bcb, reinterpret_cast<const uint8_t*>(S.whi) + bo, (uint32_t)bcb, bar);
-            bulk_g2s(base + 2 * c * bcb + bcb, reinterpret_cast<const uint8_t*>(S.wlo) + bo, (uint32_t)bcb, bar);
+            mbar_expect_tx(bar, (uint32_t)bcb);
+            bulk_g2s(base + c * bcb, reinterpret_cast<const uint8_t*>(S.whi) + (size_t)c * bcb, (uint32_t)bcb, bar);
           }
         }
       } else if (lane == 0) {
@@ -324,10 +337,9 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
               TL(2, 61, gchunk);
             }
             uint8_t* dst = smem + q.sm_b + stg * q.stage_bytes;
-            const size_t bo = (size_t)c * q.b_chunk_bytes;
             if (q.in_mode) {
-              // one ring stage = A chunk pair (hi c0, hi c1, lo c0, lo c1) + the weight chunk (hi, lo) of K-step c
-              mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)(4 * a_plane + 2 * q.b_chunk_bytes));
+              // one ring stage = A chunk pair (hi c0, hi c1, lo c0, lo c1) + the weight chunk of K-step c
+              mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)(4 * a_plane + q.b_chunk_bytes));
   #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 const size_t go = ((size_t)(2 * c + h) * q.S_pad + (size_t)u * TC_TILE) * 8;
@@ -336,11 +348,17 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
               }
               dst += 4 * a_plane;
             } else {
-              mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)(2 * q.b_chunk_bytes));
+              mbar_expect_tx(&bars[LB_BFULL + stg], (uint32_t)q.b_chunk_bytes);
             }
-            bulk_g2s(dst, reinterpret_cast<const uint8_t*>(St0.whi) + bo, (uint32_t)q.b_chunk_bytes, &bars[LB_BFULL + stg]);
-            bulk_g2s(dst + q.b_chunk_bytes, reinterpret_cast<const uint8_t*>(St0.wlo) + bo, (uint32_t)q.b_chunk_bytes,
-                     &bars[LB_BFULL + stg]);
+            if (SPLIT) {  // the chunk's planes of the one image
+              bulk_g2s(dst, reinterpret_cast<const uint8_t*>(St0.whi) + (size_t)c * q.b_chunk_bytes,
+                       (uint32_t)q.b_chunk_bytes, &bars[LB_BFULL + stg]);
+            } else {      // the hi half, then the lo half
+              const int half = q.b_chunk_bytes / 2;
+              const size_t bo = (size_t)c * half;
+              bulk_g2s(dst, reinterpret_cast<const uint8_t*>(St0.whi) + bo, (uint32_t)half, &bars[LB_BFULL + stg]);
+              bulk_g2s(dst + half, reinterpret_cast<const uint8_t*>(St0.wlo) + bo, (uint32_t)half, &bars[LB_BFULL + stg]);
+            }
             ++gchunk;
           }
         }
@@ -403,7 +421,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   } else if (warp < LY_MMA_WARPS) {
     // ===================== MMA warpgroups: a tile's MMAs run while the epilogue warps finish the previous one =======
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(LY_REGS_MMA));
-    float acc[8 * SPG];
+    float acc[(SPLIT ? 2 : 1) * 8 * SPG];  // SPLIT: room for the correction sum (ly_mma_tile)
     const bool tl0 = warp == 0 && lane == 0;
     for (int i = 0; i < n_my; ++i) {
       if (!q.in_mode) mbar_wait(&bars[LB_WIN_FULL], (uint32_t)(i & 1));
@@ -413,8 +431,8 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       for (int ps = 0; ps < NP; ++ps) {
         if (ps) mma_bar_sync();
         ly_mma_tile<SPG, SPLIT>(acc, bars, St0.N, 16 * SPG * ps, q.n_bchunks, ring, q.NB, (i * NP + ps) * q.n_bchunks,
-                                LB_BFULL, smem_u32(smem + q.sm_b), (uint32_t)(FUSED ? 2 * q.b_chunk_bytes : q.stage_bytes),
-                                (uint32_t)q.b_chunk_bytes, q.in_mode != 0, smem_u32(smem + q.sm_a), (uint32_t)a_plane,
+                                LB_BFULL, smem_u32(smem + q.sm_b), (uint32_t)(FUSED ? q.b_chunk_bytes : q.stage_bytes),
+                                (uint32_t)(q.b_chunk_bytes / 2), q.in_mode != 0, smem_u32(smem + q.sm_a), (uint32_t)a_plane,
                                 (uint32_t)a_lo_off, p.Wp, (q.in_mode || ps + 1 < NP) ? -1 : (int)LB_WIN_EMPTY);
         if (tl0 && ps + 1 == NP) TL(0, 20, i);
         ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St0.N, 16 * SPG * ps, FUSED ? 2 * i : i,
@@ -428,7 +446,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
         mma_bar_sync();
         if (tl0) TL(0, 35, i);
         ly_mma_tile<SPG, SPLIT>(acc, bars, St1.N, 0, q.n_bchunks1, false, 1, 0, LB_BFULL + q.n_bchunks,
-                                smem_u32(smem + q.sm_b1), (uint32_t)(2 * q.b_chunk_bytes1), (uint32_t)q.b_chunk_bytes1,
+                                smem_u32(smem + q.sm_b1), (uint32_t)q.b_chunk_bytes1, (uint32_t)(q.b_chunk_bytes1 / 2),
                                 false, smem_u32(smem + q.sm_h), (uint32_t)h_plane, (uint32_t)((St1.cin >> 3) * h_plane),
                                 p.Wp, LB_H_EMPTY);
         if (tl0) TL(0, 40, i);
