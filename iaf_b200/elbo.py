@@ -62,21 +62,27 @@ def discretized_logistic(mean, logscale, sample, binsize=1 / 256.0):
     return logp.sum(dim=(1, 2, 3))
 
 
-def forward(params, x_uint8, noise, iaf_layer, hps):
-    """bits/dim and the per-sample pieces for one batch.
+def _layers(hps):
+    return [(i, j) for i in range(hps["depth"]) for j in range(hps["num_blocks"])]
 
-    hps: dict(z_size, h_size, depth, num_blocks, kl_min, image_size).  noise[(i, j)]: the N(0,1) draw of
-    layer (i, j)'s posterior (tf_train.py:57).  iaf_layer(scope, eps, post_mean, post_logsd, prior_mean,
-    prior_logsd, context) -> (z, kl_bc [B,C], kl_cost [B])."""
-    zs, hs = hps["z_size"], hps["h_size"]
+
+def _image(params, x_uint8):
     x = x_uint8.to(params["h_top"].dtype)
-    x = torch.clamp((x + 0.5) / 256.0, 0.0, 1.0) - 0.5          # tf_train.py:164-165
-    orig_x = x
-    B = x.shape[0]
+    return torch.clamp((x + 0.5) / 256.0, 0.0, 1.0) - 0.5       # tf_train.py:164-165
+
+
+def expand_samples(t, n):
+    """[B, ...] -> [B n, ...]: every image's row repeated n times, image-major (distributions.py:41-52, ``repeat``)."""
+    return t if t is None or n == 1 else t.repeat_interleave(n, dim=0)
+
+
+def _up_pass(params, x, hps):
+    """IAFLayer.up over all layers (tf_train.py:29-44): {(i, j): (qz_mean, qz_logsd, up_context)}.  It does not depend
+    on the posterior's noise."""
+    zs, hs = hps["z_size"], hps["h_size"]
     h = conv2d(params, "x_enc", x, stride=2)
-    layers = [(i, j) for i in range(hps["depth"]) for j in range(hps["num_blocks"])]
     up = {}
-    for (i, j) in layers:                                         # IAFLayer.up, tf_train.py:29-44
+    for (i, j) in _layers(hps):
         sc = "IAF_%d_%d" % (i, j)
         down = (i > 0) and (j == 0)
         t = conv2d(params, sc + "/up_conv1", F.elu(h), stride=2 if down else 1)
@@ -86,19 +92,28 @@ def forward(params, x_uint8, noise, iaf_layer, hps):
         if down:
             h = resize_nearest_neighbor(h, 0.5)
         h = h + 0.1 * hh
+    return up
+
+
+def _down_pass(params, up, noise, iaf_layer, hps, n, free_bits=True):
+    """IAFLayer.down over all layers (tf_train.py:46-95) and the decoder mean, for ``n`` posterior samples per image:
+    the rows of ``noise`` are image-major, and ``up`` (one row per image) is expanded to them layer by layer.
+    Returns (kl_obj, kl_cost, xd); kl_obj is kl_cost when ``free_bits`` is False."""
+    zs, hs = hps["z_size"], hps["h_size"]
+    B = next(iter(noise.values())).shape[0]
     size = hps["image_size"] // 2 ** hps["depth"]
     h = params["h_top"].reshape(1, -1, 1, 1).expand(B, hs, size, size)
     kl_obj = torch.zeros(B, dtype=h.dtype, device=h.device)
     kl_cost = torch.zeros(B, dtype=h.dtype, device=h.device)
-    for (i, j) in reversed(layers):                               # IAFLayer.down, tf_train.py:46-95
+    for (i, j) in reversed(_layers(hps)):
         sc = "IAF_%d_%d" % (i, j)
         down = (i > 0) and (j == 0)
         t = conv2d(params, sc + "/down_conv1", F.elu(h))
         pz_mean, pz_logsd, rz_mean, rz_logsd, down_context, h_det = torch.split(t, [zs] * 4 + [hs] * 2, dim=1)
-        qz_mean, qz_logsd, up_context = up[(i, j)]
+        qz_mean, qz_logsd, up_context = (expand_samples(u, n) for u in up[(i, j)])
         z, kl_bc, cost = iaf_layer(sc, noise[(i, j)], (rz_mean + qz_mean).contiguous(), (rz_logsd + qz_logsd).contiguous(),
                                    pz_mean.contiguous(), pz_logsd.contiguous(), (up_context + down_context).contiguous())
-        if hps["kl_min"] > 0:                                     # tf_train.py:77-83: free bits, batch mean is local
+        if free_bits and hps["kl_min"] > 0:                       # tf_train.py:77-83: free bits, batch mean is local
             obj = torch.clamp(kl_bc.mean(dim=0, keepdim=True), min=hps["kl_min"]).expand(B, -1).sum(dim=1)
         else:
             obj = cost
@@ -112,12 +127,129 @@ def forward(params, x_uint8, noise, iaf_layer, hps):
             hh = conv2d(params, sc + "/down_conv2", hh)
         h = h + 0.1 * hh
     xd = deconv2d(params, "x_dec", F.elu(h))
-    xd = torch.clamp(xd, -0.5 + 1 / 512.0, 0.5 - 1 / 512.0)
+    return kl_obj, kl_cost, torch.clamp(xd, -0.5 + 1 / 512.0, 0.5 - 1 / 512.0)
+
+
+def forward(params, x_uint8, noise, iaf_layer, hps):
+    """bits/dim and the per-sample pieces for one batch.
+
+    hps: dict(z_size, h_size, depth, num_blocks, kl_min, image_size).  noise[(i, j)]: the N(0,1) draw of
+    layer (i, j)'s posterior (tf_train.py:57).  iaf_layer(scope, eps, post_mean, post_logsd, prior_mean,
+    prior_logsd, context) -> (z, kl_bc [B,C], kl_cost [B])."""
+    orig_x = _image(params, x_uint8)
+    B = orig_x.shape[0]
+    kl_obj, kl_cost, xd = _down_pass(params, _up_pass(params, orig_x, hps), noise, iaf_layer, hps, 1)
     log_pxz = discretized_logistic(xd, params["dec_log_stdv"], orig_x)
     loss = (kl_cost - log_pxz).sum()                              # compute_lowerbound, k = 1 (distributions.py:55-57)
     num_pixels = 3 * hps["image_size"] ** 2
     return dict(bits_per_dim=loss / (math.log(2.0) * num_pixels * B), obj=(kl_obj - log_pxz).sum(), kl_cost=kl_cost,
                 kl_obj=kl_obj, log_pxz=log_pxz)
+
+
+class LogMeanExp(object):
+    """Streaming per-image ``log (1/k) sum_j exp(w_j)`` in fp64: a running max and a sum scaled by it, so chunks of
+    log-weights near -1e4 with a spread of 1e3 neither overflow nor underflow.  Also keeps the plain sum of the
+    log-weights (their mean is the ELBO of the same samples)."""
+
+    def __init__(self, n_images, device):
+        self.max = torch.full((n_images,), -math.inf, dtype=torch.float64, device=device)
+        self.scaled = torch.zeros(n_images, dtype=torch.float64, device=device)
+        self.total = torch.zeros(n_images, dtype=torch.float64, device=device)
+        self.count = 0
+
+    def add(self, w):
+        """w: [n_images, c] log-weights of c more samples of every image."""
+        w = w.to(torch.float64)
+        m = torch.maximum(self.max, w.max(dim=1).values)
+        self.scaled = self.scaled * torch.exp(self.max - m) + torch.exp(w - m[:, None]).sum(dim=1)
+        self.max = m
+        self.total = self.total + w.sum(dim=1)
+        self.count += w.shape[1]
+
+    def result(self):
+        """(log mean exp [n_images], mean [n_images]) over every sample added."""
+        return self.max + torch.log(self.scaled) - math.log(self.count), self.total / self.count
+
+
+# every tensor of one estimator call stays below 2^31 elements: the kernels index memory in 64 bits, but their sample and
+# tensor-core slot indices are 32-bit ints, and the slot stream refuses a call past 2^31 slots (iaf_tc.cu, tc_num_tiles)
+MAX_ELEMS = 2 ** 31 - 1
+# and at most this many samples per call: every layer's operator keeps its own kernel scratch, sized for the largest
+# call it has seen (about 0.1 MB per sample and layer at h_size 160), so memory grows with the samples per call times
+# the layers.  4096 samples fill the H100 many times over; the README's TF eval model (20 layers) at 100 images and
+# 119 samples each (the index bound) ran out of 80 GB.
+MAX_SAMPLES = 4096
+
+
+def default_chunk(n_images, k, elems_per_sample):
+    """Samples per image of one call: the largest that keeps every tensor below 2^31 elements and the call at most
+    MAX_SAMPLES samples, at most k, at least 1."""
+    return max(1, min(k, MAX_ELEMS // (n_images * elems_per_sample), MAX_SAMPLES // n_images))
+
+
+def _elems_per_sample(hps):
+    """An upper bound on the elements of one posterior sample's largest tensor (down_conv1's output, the padded input
+    of the encoder and the decoder's full transposed-conv output are the candidates)."""
+    zs, hs, S = hps["z_size"], hps["h_size"], hps["image_size"]
+    return max((4 * zs + 2 * hs + 1) * (S // 2 + 4) ** 2, 4 * (S + 4) ** 2)
+
+
+def default_noise(shapes, device, dtype, seed=0):
+    """noise(start, count): torch.randn from ONE seeded generator on ``device``, drawn chunk by chunk, so the draws (and
+    the estimate) depend on the chunk size.  shapes: {(i, j): (B, C, H, W)}."""
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+
+    def noise(start, count):
+        return {key: torch.randn((B * count,) + tuple(s), generator=gen, device=device, dtype=dtype)
+                for key, (B, *s) in sorted(shapes.items())}
+    return noise
+
+
+def _noise_shapes(hps, B):
+    zs, S = hps["z_size"], hps["image_size"]
+    return {(i, j): (B, zs, S // 2 ** (i + 1), S // 2 ** (i + 1)) for (i, j) in _layers(hps)}
+
+
+def _check_k_chunk(k, chunk):
+    if int(k) < 1 or (chunk is not None and int(chunk) < 1):
+        raise ValueError("k and chunk must be positive")
+
+
+def log_likelihood(params, x_uint8, iaf_layer, hps, k, chunk=None, noise=None, seed=0):
+    """Importance-sampled log-likelihood with k posterior samples per image (tf_train.py:167-170, 218 at ``hps.k = k``;
+    ``compute_lowerbound``, distributions.py:55-62): ``log_px[b] = -log k + logsumexp_j (log_pxz - kl_cost)[b, j]``, with
+    the true KL sum ``kl_cost`` (never the free-bits objective).
+
+    The up pass does not depend on the noise: it runs once per image, and its posterior statistics and context are
+    expanded over the samples.  Samples are processed ``chunk`` per image at a time (image-major, as ``repeat`` lays them
+    out) and reduced into a running fp64 log-sum-exp, so memory is bounded by B * chunk samples whatever k is.  Default
+    chunk: the largest that keeps every tensor of one call below 2^31 elements and the call at most MAX_SAMPLES samples
+    (:func:`default_chunk`).  noise(start, count) ->
+    {(i, j): [B count, z_size, s, s]}: samples [start, start + count) of every image; default: torch.randn from one
+    generator seeded with ``seed`` on the parameters' device.  An evaluation: runs under no_grad and records no graph
+    (use the inference wrapper, CudaIAF).
+
+    Returns dict(log_px [B] fp64 nats, bits_per_dim (tf_train.py:142), elbo [B] fp64: the mean log-weight)."""
+    _check_k_chunk(k, chunk)
+    k = int(k)
+    B = x_uint8.shape[0]
+    dev, dt = params["h_top"].device, params["h_top"].dtype
+    chunk = default_chunk(B, k, _elems_per_sample(hps)) if chunk is None else min(int(chunk), k)
+    if noise is None:
+        noise = default_noise(_noise_shapes(hps, B), dev, dt, seed)
+    with torch.no_grad():
+        x = _image(params, x_uint8)
+        up = _up_pass(params, x, hps)
+        acc = LogMeanExp(B, dev)
+        for start in range(0, k, chunk):
+            n = min(chunk, k - start)
+            _, kl_cost, xd = _down_pass(params, up, noise(start, n), iaf_layer, hps, n, free_bits=False)
+            log_pxz = discretized_logistic(xd, params["dec_log_stdv"], expand_samples(x, n))
+            acc.add((log_pxz.double() - kl_cost.double()).reshape(B, n))
+        log_px, mean_w = acc.result()
+    num_pixels = 3 * hps["image_size"] ** 2
+    return dict(log_px=log_px, bits_per_dim=(-log_px).sum() / (math.log(2.0) * num_pixels * B), elbo=mean_w)
 
 
 def make_params(hps, seed=0, dtype=np.float32):
@@ -238,3 +370,26 @@ def sharded_bits_per_dim(params, x_uint8, noise, iaf_layer, hps, group=None):
     loss_local = out["bits_per_dim"] * (math.log(2.0) * num_pixels * (hi - lo))
     (loss,) = allreduce_scalars([loss_local], group)
     return loss / (math.log(2.0) * num_pixels * x_uint8.shape[0])
+
+
+def sharded_log_likelihood(params, x_uint8, iaf_layer, hps, k, chunk=None, noise=None, seed=0, group=None,
+                           estimator=None):
+    """Image-sharded importance-sampled bits/dim: every rank runs all k samples of its contiguous slice of the images
+    (``shard_range``), and ONE sum all-reduce of the summed -log_px gives the global bits/dim.  ``estimator``: this
+    module's :func:`log_likelihood` (default) or ``elbo_theano.log_likelihood``.  A given ``noise(start, count)`` covers
+    the global batch; each rank takes its images' rows.  The default noise is seeded with ``seed`` on every rank."""
+    import torch.distributed as dist
+    from .parallel import allreduce_scalars, shard_range
+    estimator = log_likelihood if estimator is None else estimator
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    B = x_uint8.shape[0]
+    lo, hi = shard_range(B, rank, world)
+    local = None if noise is None else (
+        lambda start, count: {key: v[lo * count:hi * count] for key, v in noise(start, count).items()})
+    if hi > lo:
+        nll = (-estimator(params, x_uint8[lo:hi], iaf_layer, hps, k, chunk, local, seed)["log_px"]).sum()
+    else:
+        nll = torch.zeros((), dtype=torch.float64, device=x_uint8.device)
+    (nll,) = allreduce_scalars([nll], group)
+    return nll / (math.log(2.0) * 3 * hps["image_size"] ** 2 * B)

@@ -284,35 +284,57 @@ def discretized_logistic_logp(mean, logscale, binsize, sample):
     return logps.flatten(1).sum(dim=1)
 
 
-def forward(w, x_uint8, noise, iaf_layer, hps):
-    """cvae1.f_encode_decode (models.py:435-497).  hps: n_z, n_h1, n_h2, depths (list), depth_ar, nl, kl_min,
-    image_size.  noise[(i, j)]: the N(0,1) draw of layer (i, j).  Returns the reference's ``results`` entries plus
-    bits_per_dim (= mean of ``cost``, what train.py reports)."""
-    depths, nl = hps["depths"], hps["nl"]
-    prior_of(hps)
-    dt = w["h_top"].dtype
-    x = torch.clamp((x_uint8.to(dt) + 0.5) / 256.0, 0.0, 1.0)      # models.py:425
-    B = x.shape[0]
+def _image(w, x_uint8):
+    return torch.clamp((x_uint8.to(w["h_top"].dtype) + 0.5) / 256.0, 0.0, 1.0)     # models.py:425
+
+
+def _up_pass(w, x, noise, iaf_layer, hps):
+    """cvae_layer.up over all layers: {(i, j): up_state}.  noise is only read by the up posteriors."""
+    depths = hps["depths"]
     h = conv2d(w, "x_enc", x - 0.5, downsample=2)
     ups = {}
     for i in range(len(depths)):
         for j in range(depths[i]):
-            h, ups[(i, j)] = layer_up(w, "%d_%d" % (i, j), h, hps, i > 0 and j == 0, noise[(i, j)], iaf_layer)
+            eps = None if noise is None else noise[(i, j)]
+            h, ups[(i, j)] = layer_up(w, "%d_%d" % (i, j), h, hps, i > 0 and j == 0, eps, iaf_layer)
+    return ups
+
+
+def _down_pass(w, ups, noise, iaf_layer, hps, n):
+    """cvae_layer.down_q over all layers and the decoder mean, for ``n`` samples per row of ``ups`` (the rows of
+    ``noise`` are image-major; each up state is expanded to them layer by layer).  Returns
+    ([(cost key, kl_bc, kl_sum)] top layer first, mean_x)."""
+    from .elbo import expand_samples
+    depths, nl = hps["depths"], hps["nl"]
+    B = noise[(0, 0)].shape[0]
     size = hps["image_size"] // 2 ** len(depths)
     h = w["h_top"].reshape(1, -1, 1, 1).expand(B, -1, size, size)
-    results = {}
-    obj_kl = torch.zeros((), dtype=dt, device=x.device)
+    kls = []
     for i in reversed(range(len(depths))):
         for j in reversed(range(depths[i])):
-            h, kl_bc, kl_sum = layer_down_q(w, "%d_%d" % (i, j), h, ups[(i, j)], noise[(i, j)], iaf_layer, hps,
+            up_state = tuple(expand_samples(u, n) for u in ups[(i, j)])
+            h, kl_bc, kl_sum = layer_down_q(w, "%d_%d" % (i, j), h, up_state, noise[(i, j)], iaf_layer, hps,
                                             i > 0 and j == 0)
-            results["cost_z%03d_%03d" % (i, j)] = kl_sum
-            if hps["kl_min"] > 0:    # models.py:458-461: free bits per feature map, averaged over the minibatch
-                obj_kl = obj_kl + torch.clamp(kl_bc.mean(dim=0), min=hps["kl_min"]).sum()
-            else:
-                obj_kl = obj_kl + kl_sum
+            kls.append(("cost_z%03d_%03d" % (i, j), kl_bc, kl_sum))
     out = 0.1 * conv2d(w, "x_dec", nonlinearity(h, nl), upsample=2)
-    mean_x = torch.clamp(out + 0.5, 1 / 512.0, 1 - 1 / 512.0)
+    return kls, torch.clamp(out + 0.5, 1 / 512.0, 1 - 1 / 512.0)
+
+
+def forward(w, x_uint8, noise, iaf_layer, hps):
+    """cvae1.f_encode_decode (models.py:435-497).  hps: n_z, n_h1, n_h2, depths (list), depth_ar, nl, kl_min,
+    image_size.  noise[(i, j)]: the N(0,1) draw of layer (i, j).  Returns the reference's ``results`` entries plus
+    bits_per_dim (= mean of ``cost``, what train.py reports)."""
+    prior_of(hps)
+    x = _image(w, x_uint8)
+    results = {}
+    obj_kl = torch.zeros((), dtype=x.dtype, device=x.device)
+    kls, mean_x = _down_pass(w, _up_pass(w, x, noise, iaf_layer, hps), noise, iaf_layer, hps, 1)
+    for key, kl_bc, kl_sum in kls:
+        results[key] = kl_sum
+        if hps["kl_min"] > 0:        # models.py:458-461: free bits per feature map, averaged over the minibatch
+            obj_kl = obj_kl + torch.clamp(kl_bc.mean(dim=0), min=hps["kl_min"]).sum()
+        else:
+            obj_kl = obj_kl + kl_sum
     logpx = discretized_logistic_logp(mean_x, w["logsd_x"], 1 / 256.0, x)
     num = 3 * hps["image_size"] ** 2
     obj = (logpx - obj_kl) / (num * math.log(2.0))
@@ -320,6 +342,59 @@ def forward(w, x_uint8, noise, iaf_layer, hps):
     results["cost"] = -obj
     results["bits_per_dim"] = (-obj).mean()
     return results
+
+
+def _elems_per_sample(hps):
+    """An upper bound on the elements of one posterior sample's largest tensor: a level-0 conv output or its
+    pad-channel input, or an image-sized one."""
+    nz, nh1, nh2, S = hps["n_z"], hps["n_h1"], hps["n_h2"], hps["image_size"]
+    return max((max(nh1, 2 * nh2 + 4 * nz) + 1) * (S // 2 + 2) ** 2, 4 * (S + 4) ** 2)
+
+
+def log_likelihood(w, x_uint8, iaf_layer, hps, k, chunk=None, noise=None, seed=0):
+    """Importance-sampled log-likelihood with k posterior samples per image, what ``est_marglik = k`` estimates
+    (train.py:187-205): ``log_px[b] = log mean_j exp(logpx - sum_layers kl_sum)[b, j]`` in nats, and
+    ``bits_per_dim = -mean(log_px) / (prod(shape_x) log 2)`` (train.py:203).
+
+    The log-weight uses the true KL sums, whatever ``kl_min`` is.  This departs from the reference, whose
+    ``est_marglik`` reuses the training ``cost``: with kl_min > 0 that contains the free-bits floor (models.py:458-466),
+    so its estimate is then not an estimate of log p(x).  With kl_min = 0 the two agree.
+
+    For the down posteriors the up pass does not depend on the noise: it runs once per image and its state is expanded
+    over the samples.  For up_iaf2_nl / up_iaf2 the sample is drawn in the up pass (models.py:145-176), so the up pass
+    runs per sample.  Chunking, noise(start, count) and the default noise are those of ``iaf_b200.elbo.log_likelihood``;
+    noise[(i, j)] is the draw ``forward`` takes.  Runs under no_grad: use the inference wrapper, CudaIAF.
+    Returns dict(log_px [B] fp64 nats, bits_per_dim, elbo [B] fp64: the mean log-weight)."""
+    from .elbo import LogMeanExp, _check_k_chunk, default_chunk, default_noise, expand_samples
+    posterior, depths = posterior_of(hps), hps["depths"]
+    prior_of(hps)
+    _check_k_chunk(k, chunk)
+    k = int(k)
+    B, S = x_uint8.shape[0], hps["image_size"]
+    dev, dt = w["h_top"].device, w["h_top"].dtype
+    chunk = default_chunk(B, k, _elems_per_sample(hps)) if chunk is None else min(int(chunk), k)
+    if noise is None:
+        shapes = {(i, j): (B, hps["n_z"], S // 2 ** (i + 1), S // 2 ** (i + 1))
+                  for i in range(len(depths)) for j in range(depths[i])}
+        noise = default_noise(shapes, dev, dt, seed)
+    with torch.no_grad():
+        x = _image(w, x_uint8)
+        shared = None if posterior in UP_POSTERIORS else _up_pass(w, x, None, iaf_layer, hps)
+        acc = LogMeanExp(B, dev)
+        for start in range(0, k, chunk):
+            n = min(chunk, k - start)
+            eps = noise(start, n)
+            xs = expand_samples(x, n)
+            if shared is None:
+                kls, mean_x = _down_pass(w, _up_pass(w, xs, eps, iaf_layer, hps), eps, iaf_layer, hps, 1)
+            else:
+                kls, mean_x = _down_pass(w, shared, eps, iaf_layer, hps, n)
+            logw = discretized_logistic_logp(mean_x, w["logsd_x"], 1 / 256.0, xs).double()
+            for _, _, kl_sum in kls:
+                logw = logw - kl_sum.double()
+            acc.add(logw.reshape(B, n))
+        log_px, mean_w = acc.result()
+    return dict(log_px=log_px, bits_per_dim=-log_px.mean() / (3 * S * S * math.log(2.0)), elbo=mean_w)
 
 
 def make_params(hps, seed=0, dtype=np.float32):
