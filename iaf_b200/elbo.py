@@ -9,12 +9,15 @@ conv / deconv, elu, discretized logistic) expressed with stock torch ops on what
 dtype the parameters live on.  Parameters are a dict under the reference's TF variable names:
 ``x_enc/{V,g,b}``, ``IAF_{i}_{j}/{up_conv1,up_conv3,down_conv1,down_conv2|down_deconv2}/{V,g,b}``,
 ``IAF_{i}_{j}/ar_multiconv2d/layer_{k}|layer_out_{k}/{V,g,b}``, ``h_top``, ``dec_log_stdv``, ``x_dec/{V,g,b}``.
+:func:`data_init` is the reference's data-dependent initialisation of all of them (mode "init").
 """
 import math
 
 import numpy as np
 import torch
 import torch.nn.functional as F
+
+from .masks import tf_conv_ar_mask
 
 
 def _same_pad(n, k, s):
@@ -23,28 +26,46 @@ def _same_pad(n, k, s):
     return total // 2, total - total // 2
 
 
+def _conv_same(x, w, stride):
+    """tf.nn.conv2d, SAME padding, NCHW input, filter [kh,kw,Cin,Cout]."""
+    pt, pb = _same_pad(x.shape[2], w.shape[0], stride)
+    pl, pr = _same_pad(x.shape[3], w.shape[1], stride)
+    return F.conv2d(F.pad(x, (pl, pr, pt, pb)), w.permute(3, 2, 0, 1), stride=stride)
+
+
+def _deconv_same(x, w, stride):
+    """my_deconv2d (layers.py:67-76): conv2d_transpose, SAME padding, filter [kh,kw,Cout,Cin]."""
+    H, W = x.shape[2] * stride, x.shape[3] * stride
+    y = F.conv_transpose2d(x, w.permute(3, 2, 0, 1), stride=stride)  # full output (H-1)*s + k
+    pt, _ = _same_pad(H, w.shape[0], stride)
+    pl, _ = _same_pad(W, w.shape[1], stride)
+    return y[:, :, pt:pt + H, pl:pl + W]
+
+
+def _l2_normalize(v):
+    """tf.nn.l2_normalize(v, [0, 1, 2]) = v * rsqrt(max(sum(v^2), 1e-12))."""
+    return v * torch.rsqrt(torch.clamp((v * v).sum(dim=(0, 1, 2), keepdim=True), min=1e-12))
+
+
 def conv2d(params, name, x, stride=1):
-    """tf_utils/layers.py:31-64 (run-time branch, mask=None): w = exp(g) * l2_normalize(V,[0,1,2]); SAME padding."""
+    """tf_utils/layers.py:31-64 (run-time branch, mask=None): w = exp(g) * l2_normalize(V,[0,1,2]); SAME padding.
+    During :func:`data_init` the init branch (layers.py:38-51) instead."""
+    if isinstance(params, InitPass):
+        return params.init(name, _conv_same(x, _l2_normalize(params[name + "/V"]), stride), 0.1)
     V, g, b = params[name + "/V"], params[name + "/g"], params[name + "/b"]
     w = torch.exp(g).reshape(1, 1, 1, -1) * V * torch.rsqrt(torch.clamp((V * V).sum(dim=(0, 1, 2), keepdim=True), min=1e-12))
-    kh, kw = V.shape[0], V.shape[1]
-    pt, pb = _same_pad(x.shape[2], kh, stride)
-    pl, pr = _same_pad(x.shape[3], kw, stride)
-    x = F.pad(x, (pl, pr, pt, pb))
-    return F.conv2d(x, w.permute(3, 2, 0, 1), stride=stride) + b.reshape(1, -1, 1, 1)
+    return _conv_same(x, w, stride) + b.reshape(1, -1, 1, 1)
 
 
 def deconv2d(params, name, x, stride=2):
-    """tf_utils/layers.py:67-112: conv2d_transpose, SAME, filter [kh,kw,Cout,Cin], weight norm over [0,1,2] -> per Cin."""
+    """tf_utils/layers.py:67-112: conv2d_transpose, SAME, filter [kh,kw,Cout,Cin], weight norm over [0,1,2] -> per Cin.
+    During :func:`data_init` the init branch (layers.py:86-100) instead."""
+    if isinstance(params, InitPass):
+        return params.init(name, _deconv_same(x, _l2_normalize(params[name + "/V"]), stride), 0.1)
     V, g, b = params[name + "/V"], params[name + "/g"], params[name + "/b"]
     # layers.py:108: w = reshape(exp(g), [1,1,num_filters,1]) * l2_normalize(v, [0,1,2])
     w = torch.exp(g).reshape(1, 1, -1, 1) * V * torch.rsqrt(torch.clamp((V * V).sum(dim=(0, 1, 2), keepdim=True), min=1e-12))
-    kh, kw = V.shape[0], V.shape[1]
-    H, W = x.shape[2] * stride, x.shape[3] * stride
-    y = F.conv_transpose2d(x, w.permute(3, 2, 0, 1), stride=stride)  # full output (H-1)*s + k
-    pt, _ = _same_pad(H, kh, stride)
-    pl, _ = _same_pad(W, kw, stride)
-    return y[:, :, pt:pt + H, pl:pl + W] + b.reshape(1, -1, 1, 1)
+    return _deconv_same(x, w, stride) + b.reshape(1, -1, 1, 1)
 
 
 def resize_nearest_neighbor(x, scale):
@@ -283,6 +304,88 @@ def make_params(hps, seed=0, dtype=np.float32):
     p["h_top"] = (0.1 * rng.randn(hs)).astype(dtype)
     p["dec_log_stdv"] = np.asarray(-1.0, dtype=dtype)
     return p
+
+
+class InitPass(dict):
+    """The parameters while a data-dependent init pass runs (``tf_train.py:175`` with mode "init"; ``'__init' in w`` in
+    the Theano model).  The weight-normed convs of :mod:`iaf_b200.elbo` and :mod:`iaf_b200.elbo_theano` recognise it and
+    take their init branch: they write the gain and bias they derive from the batch here and return the standardised
+    pre-activation, which the next layers are initialised on."""
+
+    def init(self, name, x_init, init_scale):
+        """TF, layers.py:47-51 (conv2d) and 95-99 (deconv2d): ``x_init`` is the convolution with the l2-normalised V.
+        Population moments over (0, 2, 3), ``scale = init_scale / sqrt(var + 1e-10)``, ``g = log(scale) / 3`` and
+        ``b = -m scale``; returns ``scale (x_init - m)``.  The run-time branch applies exp(g), not exp(3 g), so an
+        initialised layer runs at gain scale^(1/3), exactly as the reference's does."""
+        m = x_init.mean(dim=(0, 2, 3))
+        var = x_init.var(dim=(0, 2, 3), unbiased=False)
+        scale = init_scale / torch.sqrt(var + 1e-10)
+        self[name + "/g"] = torch.log(scale) / 3.0
+        self[name + "/b"] = -m * scale
+        return scale.reshape(1, -1, 1, 1) * (x_init - m.reshape(1, -1, 1, 1))
+
+
+def _init_ar_conv2d(params, name, x, zerodiagonal):
+    """ar_conv2d (layers.py:144-154) in init mode: the masked, l2-normalised V, init_scale 1 (layers.py:145)."""
+    V = params[name + "/V"]
+    mask = torch.from_numpy(tf_conv_ar_mask(V.shape[2], V.shape[3], zerodiagonal)).to(V)
+    return params.init(name, _conv_same(x, _l2_normalize(mask * V), 1), 1.0)
+
+
+class _InitLayer(object):
+    """iaf_layer of the init pass (IAFLayer.down in mode "init", tf_train.py:56-85): z is the PRIOR's sample
+    (tf_train.py:60-61), log q the posterior's density at it, and the masked stack (tf_train.py:69) runs conv by conv
+    in init mode, with ``+ context`` after the first hidden conv.  Records each stack's input in ``stacks``."""
+
+    def __init__(self, params):
+        self.params, self.stacks = params, {}
+
+    def __call__(self, scope, eps, post_mean, post_logsd, prior_mean, prior_logsd, context):
+        c = 0.5 * math.log(2.0 * math.pi)
+        z = prior_mean + torch.exp(prior_logsd) * eps
+        logqs = -c - post_logsd - 0.5 * (z - post_mean) ** 2 * torch.exp(-2.0 * post_logsd)
+        pre = scope + "/ar_multiconv2d/"
+        self.stacks[pre[:-1]] = (z, context)
+        h = z
+        for k in range(2):
+            h = _init_ar_conv2d(self.params, pre + "layer_%d" % k, h, False)
+            if k == 0:
+                h = h + context
+            h = F.elu(h)
+        arw_mean, arw_logsd = (0.1 * _init_ar_conv2d(self.params, pre + "layer_out_%d" % k, h, True) for k in range(2))
+        z = (z - arw_mean) / torch.exp(arw_logsd)
+        logqs = logqs + arw_logsd
+        logps = -c - prior_logsd - 0.5 * (z - prior_mean) ** 2 * torch.exp(-2.0 * prior_logsd)
+        kl = logqs - logps
+        return z, kl.sum(dim=(2, 3)), kl.sum(dim=(1, 2, 3))
+
+
+def data_init_pass(params, x_uint8, hps, noise=None, seed=0):
+    """:func:`data_init` with what the pass saw: (params, out, stacks).  ``out`` is :func:`forward`'s dict for the init
+    pass (the terms ``CVAE1(hps, "init", x)`` computes); ``stacks[scope + "/ar_multiconv2d"] = (z, context)`` is the
+    input each masked stack was initialised on."""
+    if noise is None:
+        noise = default_noise(_noise_shapes(hps, x_uint8.shape[0]), params["h_top"].device, params["h_top"].dtype,
+                              seed)(0, 1)
+    p = InitPass(params)
+    layer = _InitLayer(p)
+    with torch.no_grad():
+        out = forward(p, x_uint8, noise, layer, hps)
+    return dict(p), out, layer.stacks
+
+
+def data_init(params, x_uint8, hps, noise=None, seed=0):
+    """The reference's data-dependent initialisation (tf_train.py:222-228: ``CVAE1(hps, "init", x[:batch_size])``) on
+    the batch ``x_uint8``: returns a new dict with the ``g`` and ``b`` of every conv, deconv and masked conv set from
+    the batch's statistics (tf_utils/layers.py:38-51, 86-100, and 144-166 with init_scale 1).  Every other entry is
+    passed through: ``V`` (the reference draws it from N(0, 0.05) as :func:`make_params` does), ``h_top`` (zero in the
+    reference, tf_train.py:190) and ``dec_log_stdv``.  The pass runs in stock torch ops on the parameters' device and
+    dtype, in :func:`forward`'s order, with z drawn from each layer's prior.  noise[(i, j)]: that draw's N(0, 1) noise
+    (the shapes :func:`forward` takes); default: torch.randn from one generator seeded with ``seed``.
+
+    As in the reference, ``g = log(scale) / 3`` while the run-time branch applies ``exp(g)``: an initialised layer
+    runs at scale^(1/3) of the standardising scale, not at it."""
+    return data_init_pass(params, x_uint8, hps, noise, seed)[0]
 
 
 class CudaIAF(object):

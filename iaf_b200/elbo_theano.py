@@ -32,16 +32,21 @@ reference uses ``z = eps`` as a placeholder (models.py:338-340).
 conv ``{i}_{j}_posterior_conv1_{w,s,b}`` with ``w`` of shape [2 n_z, n_z + 1, 3, 3], whose even rows are the mean head
 and odd rows the logsd head, and no context (up_conv1 and down_conv1 have no context channels).  The operator runs it as
 a stack without hidden layers and two heads of n_z (:func:`iaf_b200.weights.deinterleave_heads`).
+:func:`data_init` is cvae1's data-dependent initialisation (``w['__init']``) for every posterior and prior above.
 """
 import math
+import warnings
 
 import numpy as np
 import torch
 import torch.nn.functional as F
 
+from .elbo import InitPass
+from .masks import theano_conv_ar_mask
 from .weights import deinterleave_heads
 
 LOGSCALE_SCALE = 3.0  # graphy/nodes/conv.py:19 (conv.py:16-22: logscale=True, bn=False, maxweight=0)
+INIT_STDEV = 0.1      # graphy/nodes/conv.py:22: the std a datainit conv's output is initialised to
 POSTERIORS = ("down_iaf2_nl", "up_iaf2_nl", "down_iaf2_nl2", "down_iaf2", "up_iaf2")
 PRIORS = ("diag", "made")
 # the paper's linear IAF (models.py:55-56, 79-82): one masked conv ``ar.conv2d(name+'_posterior_conv1', n_z, 2 n_z)``,
@@ -79,13 +84,16 @@ def pad2dwithchannel(x, k):
 
 def conv2d(w, name, x, downsample=1, upsample=1):
     """graphy/nodes/conv.py:122-274, run-time branch: kernel / ||kernel|| * exp(3 s) per output map (no epsilon),
-    pad channel for k > 1, TRUE convolution 'valid' with stride ``downsample``, bias, then depth-to-space."""
+    pad channel for k > 1, TRUE convolution 'valid' with stride ``downsample``, bias, then depth-to-space.  During
+    :func:`data_init` the datainit branch (conv.py:225-250) runs on the output before depth-to-space."""
     W, b, s = w[name + "_w"], w[name + "_b"], w[name + "_s"]
     k = W.shape[2]
     kern = W / torch.sqrt((W * W).sum(dim=(1, 2, 3), keepdim=True)) * torch.exp(LOGSCALE_SCALE * s).reshape(-1, 1, 1, 1)
     if k > 1:
         x = pad2dwithchannel(x, k)
     y = F.conv2d(x, kern.flip(2, 3), stride=downsample) + b.reshape(1, -1, 1, 1)   # dnn_conv default conv_mode='conv'
+    if isinstance(w, InitPass):
+        y = _data_init(w, name, y, 1.0 / INIT_STDEV, 1e-7)                          # conv.py:225-250 (datainit)
     if upsample > 1:
         y = F.pixel_shuffle(y, upsample)     # depool2d_split, conv.py:26-33: channel c*f*f + fy*f + fx -> (y*f+fy, x*f+fx)
     return y
@@ -444,6 +452,113 @@ def make_params(hps, seed=0, dtype=np.float32):
                 for k in range(2):
                     conv("%s_prior_conv1_out_%d" % (n, k), sizes[-1], nz, 3)
     return w
+
+
+def _data_init(w, name, h, inv_stdev, eps):
+    """The data-dependent branch of a conv on its output h (bias included): conv.py:225-250 with ``inv_stdev`` 1 /
+    init_stdev and ``eps`` 1e-7, ar.py:331-353 with 1 and 0.  ``std = data_std inv_stdev + eps`` from the population
+    std over (0, 2, 3), ``_s = -log(std) / 3``, h / std, ``_b = -mean`` of that; returns the standardised h.  When a
+    channel's std is exactly 0 the conv keeps its parameters and returns h, with the reference's warning."""
+    data_std = h.std(dim=(0, 2, 3), unbiased=False)
+    num_zeros = int((data_std == 0).sum())
+    if num_zeros > 0:
+        warnings.warn("Stdev=0 for %d features in %s. Skipping data-dependent init." % (num_zeros, name))
+        return h
+    std = data_std * inv_stdev + eps
+    w[name + "_s"] = -torch.log(std) / LOGSCALE_SCALE
+    h = h / std.reshape(1, -1, 1, 1)
+    mean = h.mean(dim=(0, 2, 3))
+    w[name + "_b"] = -mean
+    return h - mean.reshape(1, -1, 1, 1)
+
+
+def _init_ar_conv2d(w, name, h, zerodiagonal, flipmask):
+    """ar.conv2d (graphy/nodes/ar.py:241-353) in the init pass: the mask (masks.py), l2normalize with its zeroed centre
+    rows and 1e-8 (ar.py:267-281), exp(3 s), the pad channel, TRUE convolution, bias, then the data-dependent branch."""
+    W, s, b = w[name + "_w"], w[name + "_s"], w[name + "_b"]
+    n_out, n_in = W.shape[0], W.shape[1] - 1
+    kerns = torch.from_numpy(theano_conv_ar_mask(n_in, n_out, zerodiagonal=zerodiagonal, flipmask=flipmask)).to(W) * W
+    if zerodiagonal:
+        keep = torch.ones_like(kerns)
+        keep[:n_out // n_in if n_out >= n_in else 1, :, 1, 1] = 0
+        kerns = kerns * keep
+    kerns = kerns * (1.0 / (torch.sqrt((kerns ** 2).sum(dim=(1, 2, 3), keepdim=True)) + 1e-8))
+    kerns = kerns * torch.exp(LOGSCALE_SCALE * s).reshape(-1, 1, 1, 1)
+    y = F.conv2d(pad2dwithchannel(h, 3), kerns.flip(2, 3)) + b.reshape(1, -1, 1, 1)
+    return _data_init(w, name, y, 1.0, 0.0)
+
+
+class _InitLayer(object):
+    """iaf_layer of the init pass: the masked convs of every posterior and prior stack run in init mode, in the order
+    ``f_encode_decode`` runs them, with the operator's formulas around them (models.py:168-176, 272-291, 304-309).
+    Records each stack's input in ``stacks``."""
+
+    def __init__(self, w, hps):
+        self.w, self.hps, self.stacks = w, hps, {}
+
+    def _stack(self, pre, z, context, flipmask=False):
+        """multiconv2d (ar.py:396-416) -> [mean, logsd]; the linear IAF's one conv with its rows interleaving them."""
+        self.stacks[pre] = (z, context)
+        if pre.endswith("_posterior_conv1") and posterior_of(self.hps) in LINEAR:
+            out = _init_ar_conv2d(self.w, pre, z, True, False)
+            return out[:, ::2], out[:, 1::2]
+        h = z
+        for k in range(self.hps["depth_ar"]):
+            h = _init_ar_conv2d(self.w, "%s_%d" % (pre, k), h, False, flipmask)
+            if k == 0:
+                h = h + context
+            h = nonlinearity(h, self.hps["nl"])
+        return [_init_ar_conv2d(self.w, "%s_out_%d" % (pre, k), h, True, flipmask) for k in range(2)]
+
+    def step(self, name, z, context, conv=1):
+        mean, logsd = self._stack("%s_posterior_conv%d" % (name, conv), z, context, flipmask=conv == 2)
+        arw_logsd = 0.1 * logsd
+        return (z - 0.1 * mean) / torch.exp(arw_logsd), arw_logsd
+
+    def __call__(self, name, eps, post_mean, post_logsd, prior_mean, prior_logsd, context):
+        from .elbo import stochastic_layer
+        return stochastic_layer(lambda z, c: self.step(name, z, c), eps, post_mean, post_logsd, prior_mean, prior_logsd,
+                                context)
+
+    def prior_logp(self, name, z, context):
+        mean, logsd = self._stack("%s_prior_conv1" % name, z, context)
+        logps = gaussian_logps(0.1 * mean, 2 * (0.1 * logsd), z)
+        return logps.sum(dim=(2, 3)), logps.sum(dim=(1, 2, 3))
+
+
+def data_init_pass(w, x_uint8, hps, noise=None, seed=0):
+    """:func:`data_init` with what the pass saw: (w, results, stacks).  ``results`` is :func:`forward`'s dict for the
+    init pass; ``stacks[name] = (z, context)`` is the input the masked stack ``name`` (``{i}_{j}_posterior_conv{1,2}``,
+    ``{i}_{j}_prior_conv1``) was initialised on."""
+    posterior_of(hps)
+    prior_of(hps)
+    if noise is None:
+        from .elbo import default_noise
+        B, S, depths = x_uint8.shape[0], hps["image_size"], hps["depths"]
+        shapes = {(i, j): (B, hps["n_z"], S // 2 ** (i + 1), S // 2 ** (i + 1))
+                  for i in range(len(depths)) for j in range(depths[i])}
+        noise = default_noise(shapes, w["h_top"].device, w["h_top"].dtype, seed)(0, 1)
+    p = InitPass(w)
+    layer = _InitLayer(p, hps)
+    with torch.no_grad():
+        results = forward(p, x_uint8, noise, layer, hps)
+    return dict(p), results, layer.stacks
+
+
+def data_init(w, x_uint8, hps, noise=None, seed=0):
+    """The reference's data-dependent initialisation, ``cvae1(..., data_init={'x': x})`` (models.py:540-544: one
+    ``f_encode_decode`` with ``w['__init']`` set) on the batch ``x_uint8``: returns a new dict with the ``_s`` and
+    ``_b`` of every conv set from the batch's statistics.  The plain convs (x_enc, x_dec, up_conv1/2, down_conv1/2) take
+    conv.py:225-250: ``std = data_std / 0.1 + 1e-7``; every masked conv (the posterior stacks, the flipped second stack
+    of down_iaf2_nl2, the linear IAF's conv with its interleaved rows, the MADE prior's ``prior_conv1``), heads
+    included, takes ar.py:331-353: ``std = data_std``.  Then ``_s = -log(std) / 3`` and ``_b = -mean`` of the rescaled
+    output.  A conv with a channel of std exactly 0 skips its init, warning as the reference prints.  Every ``_w``,
+    ``h_top`` and ``logsd_x`` is passed through.
+
+    The pass is :func:`forward` in stock torch ops on the device and dtype of ``w`` (tensors), the posterior sampled from
+    the noise as in training.  noise[(i, j)]: the N(0, 1) draw of layer (i, j) (the shapes :func:`forward` takes);
+    default: torch.randn from one generator seeded with ``seed``."""
+    return data_init_pass(w, x_uint8, hps, noise, seed)[0]
 
 
 class CudaIAF(object):

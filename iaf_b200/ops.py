@@ -745,7 +745,9 @@ def _nl_name(nl):
 
 def ar_multiconv2d(name, x, context, n_h, n_out, nl="elu", params=None, path="auto", **_):
     """Drop-in for tf_utils/layers.py:ar_multiconv2d -> list of tensors (one per n_out entry).
-    ``params`` stands in for the TF variable scope: a dict holding V/g/b under the TF names."""
+    ``params`` stands in for the TF variable scope: a dict holding V/g/b under the TF names.  ``init=True`` (the
+    reference's data-dependent branch, layers.py:38-51) is ignored: this always runs the run-time branch; initialise
+    the parameters with ``iaf_b200.elbo.data_init``."""
     if params is None:
         raise ValueError("params (the variable store) is required in eager mode")
     nl = _nl_name(nl)
@@ -778,7 +780,9 @@ def multiconv2d(name, n_in, n_h, n_out, size_kernel=(3, 3), flipmask=False, nl="
                 path="auto"):
     """Drop-in for graphy/nodes/ar.py:multiconv2d.  Creates the parameters the reference creates
     (``{name}_{i}_w/_b/_s`` and ``{name}_out_{k}_w/_b/_s``, ar.py:288-296) in ``w`` if absent and
-    returns an object with ``__call__(h, context, w, return_hiddens=False)``, ``w`` and ``postup``."""
+    returns an object with ``__call__(h, context, w, return_hiddens=False)``, ``w`` and ``postup``.  ``'__init' in w``
+    (the data-dependent branch, ar.py:331-353) is ignored: the call always runs the run-time branch; initialise the
+    parameters with ``iaf_b200.elbo_theano.data_init``."""
     if w is None:
         w = {}
     if not isinstance(n_out, list) and isinstance(n_out, int):
