@@ -32,6 +32,14 @@ class IafDesc(C.Structure):
                 ("H", C.c_int), ("W", C.c_int), ("nl", C.c_int), ("path", C.c_int)]
 
 
+ADAMAX_RULES = {"tf": 0, "theano": 1}
+ADAMAX_MAX_TENSORS = 800
+
+
+class AdamaxTensor(C.Structure):
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("numel", C.c_int64), ("offset", C.c_int64)]
+
+
 # every symbol include/iaf_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -61,6 +69,9 @@ SYMBOLS = {
                                         C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.c_int, _P]),
     "iaf_step_inverse": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, _P]),
     "iaf_step_inverse_adjoint": (C.c_int, [_P, _P, _P, C.POINTER(_P), _P, _P, _P, _P, C.c_int, _P]),
+    "iaf_adamax_step": (C.c_int, [C.c_int, C.POINTER(AdamaxTensor), C.c_int, _P, _P, _P, C.c_double, C.c_double,
+                                  C.c_double, C.c_double, C.c_float, _P]),
+    "iaf_adamax_launch_count": (C.c_uint64, []),
     "iaf_strerror": (C.c_char_p, [C.c_int]),
     "iaf_last_cuda_error": (C.c_char_p, []),
     "iaf_version": (C.c_int, []),

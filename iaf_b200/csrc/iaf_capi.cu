@@ -1,6 +1,8 @@
 // C ABI of libiaf_b200.so (declared in include/iaf_b200.h): plan management, weight
 // packing, path selection and the launchers.  No torch, no CPU fallback.
 #include <algorithm>
+#include <atomic>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -37,7 +39,10 @@ long long centre_nnz(int cin, int cout, int zd, int flipmask) {
 
 }  // namespace
 
+int iaf_record_cuda_error(cudaError_t e, const char* what) { return cuda_fail(e, what); }
+
 IafInvKernel iaf_inv = {nullptr, nullptr, nullptr};  // (filled in by iaf_inv.cu)
+IafAdamaxKernel iaf_adamax = {nullptr};             // (filled in by iaf_optim.cu)
 
 struct iaf_plan {
   iaf_desc_t d;
@@ -302,6 +307,35 @@ const char* iaf_strerror(int status) {
 }
 
 const char* iaf_last_cuda_error(void) { return g_cuda_err; }
+
+// The fused Adamax step (iaf_optim.cu): every argument is checked here, before anything is launched.
+static std::atomic<uint64_t> g_adamax_launches{0};
+
+uint64_t iaf_adamax_launch_count(void) { return g_adamax_launches.load(); }
+
+int iaf_adamax_step(int rule, const iaf_adamax_tensor_t* tensors_host, int n_tensors, float* mom1, float* mom_max,
+                    float* avg, double lr, double beta1, double beta2, double avg_decay, float grad_scale,
+                    void* stream) {
+  if (rule != IAF_ADAMAX_TF && rule != IAF_ADAMAX_THEANO) return IAF_ERR_UNSUPPORTED;
+  if (n_tensors < 0 || !std::isfinite(lr) || !std::isfinite(beta1) || !std::isfinite(beta2) ||
+      !std::isfinite(avg_decay) || !std::isfinite(grad_scale))
+    return IAF_ERR_BAD_ARG;
+  if (n_tensors == 0) return IAF_OK;
+  if (!tensors_host || !mom1 || !mom_max || !avg) return IAF_ERR_BAD_ARG;
+  for (int i = 0; i < n_tensors; ++i) {
+    const iaf_adamax_tensor_t& t = tensors_host[i];
+    // 4-byte aligned fp32 pointers; a tensor of at most 2^31 - 1 tiles of 4096 elements (one launch's grid)
+    if (!t.param || t.numel < 1 || t.numel > ((int64_t)0x7fffffff << 12) || t.offset < 0 ||
+        ((uintptr_t)t.param & 3) || ((uintptr_t)t.grad & 3))
+      return IAF_ERR_BAD_ARG;
+  }
+  if (!iaf_adamax.launch) return IAF_ERR_UNSUPPORTED;
+  uint64_t launches = 0;
+  const int st = iaf_adamax.launch(rule, tensors_host, n_tensors, mom1, mom_max, avg, lr, beta1, beta2, avg_decay,
+                                   grad_scale, stream, &launches);
+  g_adamax_launches.fetch_add(launches);
+  return st;
+}
 
 int iaf_plan_create(iaf_plan_t** out, const iaf_desc_t* desc) {
   if (!out || !desc) return IAF_ERR_BAD_ARG;

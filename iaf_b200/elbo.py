@@ -475,6 +475,53 @@ def sharded_bits_per_dim(params, x_uint8, noise, iaf_layer, hps, group=None):
     return loss / (math.log(2.0) * num_pixels * x_uint8.shape[0])
 
 
+def run_train_step(params, x_uint8, opt, noise, objective, loss_per_bpd, sharded=False, group=None):
+    """The step both models' ``train_step`` take: zero the gradients (to None, so a parameter the objective does not
+    reach has no gradient: skipped by the TF rule, a zero gradient for the Theano rule), ``objective(x, noise) ->
+    (obj, bits_per_dim)`` on this rank's rows, ``obj.backward()``, and when sharded the towers' average of the gradients
+    (``allreduce_grads``; tf_train.py:139-147, ``average_grads``), then ``opt.step()``.  Returns the global bits/dim
+    (detached): ``loss_per_bpd`` is one sample's loss at 1 bit/dim, what turns the ranks' bits/dim into a summed loss.
+    ``noise`` covers the global batch; each rank takes its rows."""
+    import torch.distributed as dist
+    from .parallel import allreduce_grads, allreduce_scalars, shard_range
+    sharded = sharded or group is not None
+    B = x_uint8.shape[0]
+    lo, hi = 0, B
+    if sharded and dist.is_initialized():
+        lo, hi = shard_range(B, dist.get_rank(group), dist.get_world_size(group))
+    for p in params.values():
+        p.grad = None
+    obj, bpd = objective(x_uint8[lo:hi], {k: v[lo:hi] for k, v in noise.items()})
+    obj.backward()
+    if sharded:
+        allreduce_grads(params, group)
+        (loss,) = allreduce_scalars([bpd.detach() * (loss_per_bpd * (hi - lo))], group)
+        bpd = loss / (loss_per_bpd * B)
+    opt.step()
+    return bpd.detach()
+
+
+def train_step(params, x_uint8, opt, hps, noise=None, iaf_layer=None, sharded=False, group=None):
+    """One training step of the TF model, as ``tf_train.run`` takes it (tf_train.py:126-147, 211): the gradient of
+    ``obj = sum(kl_obj - log_pxz)`` over the batch (free bits per tower), then ``opt.step()``.  ``params``: leaf tensors
+    with requires_grad (fp32 CUDA for :class:`iaf_b200.optim.Adamax`, ``rule="tf"``); ``opt`` updates them in place.
+    ``iaf_layer``: default ``CudaIAFTrain(params, hps)``, built per call -- pass one to keep its operators across steps.
+    ``noise[(i, j)]``: the posterior's N(0, 1) draw of the global batch (default: torch.randn on the parameters' device).
+    ``sharded=True`` (or a ``group``): this rank is one tower of the reference's ``num_gpus`` and takes its contiguous
+    slice of the batch; the towers' gradients are averaged before the step.  Returns the step's bits/dim (a tensor)."""
+    if iaf_layer is None:
+        iaf_layer = CudaIAFTrain(params, hps)
+    if noise is None:
+        h = params["h_top"]
+        noise = {k: torch.randn(s, device=h.device, dtype=h.dtype) for k, s in _noise_shapes(hps, x_uint8.shape[0]).items()}
+
+    def objective(x, nz):
+        out = forward(params, x, nz, iaf_layer, hps)
+        return out["obj"], out["bits_per_dim"]
+    return run_train_step(params, x_uint8, opt, noise, objective, math.log(2.0) * 3 * hps["image_size"] ** 2, sharded,
+                          group)
+
+
 def sharded_log_likelihood(params, x_uint8, iaf_layer, hps, k, chunk=None, noise=None, seed=0, group=None,
                            estimator=None):
     """Image-sharded importance-sampled bits/dim: every rank runs all k samples of its contiguous slice of the images

@@ -405,6 +405,29 @@ def log_likelihood(w, x_uint8, iaf_layer, hps, k, chunk=None, noise=None, seed=0
     return dict(log_px=log_px, bits_per_dim=-log_px.mean() / (3 * S * S * math.log(2.0)), elbo=mean_w)
 
 
+def train_step(w, x_uint8, opt, hps, noise=None, iaf_layer=None, sharded=False, group=None):
+    """One training step of the Theano model, ``f_train`` (models.py:563-569): the gradient of ``cost.sum()``
+    (optim.py:102) over the batch, then ``opt.step()``.  ``w``: leaf tensors with requires_grad (fp32 CUDA for
+    :class:`iaf_b200.optim.Adamax`, ``rule="theano"``); ``opt`` updates them in place.  ``iaf_layer``: default
+    ``CudaIAFTrain(w, hps)``, built per call -- pass one to keep its operators across steps.  ``noise[(i, j)]``: the
+    N(0, 1) draw of layer (i, j) for the global batch (default: torch.randn on the parameters' device).  ``sharded=True``
+    (or a ``group``): this rank takes its contiguous slice of the batch and the ranks' gradients are averaged before the
+    step, as :func:`iaf_b200.elbo.train_step`.  Returns the step's bits/dim (a tensor)."""
+    from .elbo import run_train_step
+    if iaf_layer is None:
+        iaf_layer = CudaIAFTrain(w, hps)
+    S = hps["image_size"]
+    if noise is None:
+        h, B = w["h_top"], x_uint8.shape[0]
+        noise = {(i, j): torch.randn((B, hps["n_z"], S // 2 ** (i + 1), S // 2 ** (i + 1)), device=h.device, dtype=h.dtype)
+                 for i in range(len(hps["depths"])) for j in range(hps["depths"][i])}
+
+    def objective(x, nz):
+        out = forward(w, x, nz, iaf_layer, hps)
+        return out["cost"].sum(), out["bits_per_dim"]
+    return run_train_step(w, x_uint8, opt, noise, objective, 1.0, sharded, group)
+
+
 def make_params(hps, seed=0, dtype=np.float32):
     """Seeded synthetic parameters under the reference's Theano names and shapes (no checkpoint exists offline)."""
     rng = np.random.RandomState(seed)

@@ -279,6 +279,38 @@ int iaf_multiconv_bwd(iaf_plan_t* plan, const float* z, const float* context, co
                       float* g_context, float* const* g_w, float* const* g_scale,
                       float* const* g_bias, int B, void* stream);
 
+/*
+ * The reference's Adamax update and weight average over a whole parameter set, one fused kernel (iaf_optim.cu).
+ *   IAF_ADAMAX_TF      tf_utils/adamax.py:40-56 with ExponentialMovingAverage (tf_train.py:155-159):
+ *                        v = b1 v + (1 - b1) g;  m = max(b2 m + 1e-8, |g|);  p = p - lr (v / m)
+ *                        avg = avg - (avg - p) (1 - avg_decay)
+ *   IAF_ADAMAX_THEANO  AdaMaxAvg, graphy/misc/optim.py:99-123, called with alpha = -lr (models.py:566-568):
+ *                        mom1 = (1 - b1) mom1 + b1 g;  max = max((1 - b2) max, |g| + 1e-8);  p = p + ((-lr) mom1) / max
+ *                        avg = (1 - avg_decay) p + avg_decay avg
+ * g = grad_scale * grad.  The average reads p's value before the update (Theano's simultaneous update; TF leaves
+ * the order open).  Constants are rounded to fp32 as the reference does: TF computes 1 - b1 in fp32, Theano and the
+ * average's 1 - x in double before rounding.  Every operation is one correctly rounded fp32 operation in the order
+ * above (no FMA contraction), so results are bit-identical to an op-by-op fp32 restatement.
+ * A NULL grad skips the tensor's parameter and moments under the TF rule (apply_gradients with a None gradient) but
+ * still moves its average; under the Theano rule it is a zero gradient (disconnected_inputs='ignore').
+ * State: three fp32 buffers owned by the caller, entry i's slice at [offset, offset + numel): mom1 (TF's v), mom_max
+ * (TF's m) and avg.  Start them at 0, 0 (Theano: 1e-8) and the parameters' values.
+ * Allocates nothing, copies nothing to the device and does not synchronise (capture-safe).  Tables with more than
+ * IAF_ADAMAX_MAX_TENSORS entries go out as further launches of the same kernel.  n_tensors == 0 launches nothing.
+ */
+typedef enum { IAF_ADAMAX_TF = 0, IAF_ADAMAX_THEANO = 1 } iaf_adamax_rule;
+#define IAF_ADAMAX_MAX_TENSORS 800
+typedef struct iaf_adamax_tensor {
+  float* param;       /* numel fp32, 4-byte aligned; any storage offset                               */
+  const float* grad;  /* numel fp32 or NULL                                                          */
+  int64_t numel;      /* >= 1                                                                        */
+  int64_t offset;     /* first element of this tensor's slice of the state buffers, >= 0             */
+} iaf_adamax_tensor_t;
+int iaf_adamax_step(int rule, const iaf_adamax_tensor_t* tensors_host, int n_tensors, float* mom1, float* mom_max,
+                    float* avg, double lr, double beta1, double beta2, double avg_decay, float grad_scale,
+                    void* stream);
+uint64_t iaf_adamax_launch_count(void); /* kernels launched by iaf_adamax_step in this process so far */
+
 /* introspection */
 const char* iaf_strerror(int status);
 const char* iaf_last_cuda_error(void);          /* message of the last failing CUDA call (thread-local) */
