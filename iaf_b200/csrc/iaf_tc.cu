@@ -38,7 +38,9 @@
 #else
 #define TC_SMEM_LIMIT (227 * 1024 - 512)  // opt-in maximum minus the kernels' static shared memory (barriers: < 512 B)
 #endif
-#define TC_ZITEMS 4  // z-window (slot, chunk) items per epilogue thread of the stage kernel
+// the first stage's z window holds at most TC_ZITEMS x 256 = 1024 (slot, chunk) items: n_z up to 48 (its builder warps
+// loop over any count; the limit keeps which stacks run on the tensor cores where it was)
+#define TC_ZITEMS 4
 
 struct IafTcStage {
   const __nv_bfloat16* whi;  // global packed [K/8][N][8], or for SPLIT stages [K/8][2 NS][8] lo and hi (LY_SPLIT_NGW)
@@ -258,10 +260,11 @@ __device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, ui
 // launch that sets tl_enable records (tag, tile or chunk, clock) triples per role, each at the end of a phase of its own
 // warp (other warps of the role may still be in it).  Role 0, lane 0 of MMA warp 0: 15 / 35 the (hidden) / heads MMAs'
 // operands ready, 20 / 40 their MMAs done, 21 / 41 their fragments in the accumulator tile (after waiting for the
-// epilogues to free it).  Role 1, lane 0 of epilogue warp 0: 10 z window built, 25 / 45 (hidden) / heads accumulators
-// ready, 30 (hidden) epilogue done, 50 heads epilogue done (fused), 98 the launch's mode (k = IAF_MODE_*: multiconv,
-// step, layer, logp), 99 kernel end.  Role 2, the producer: 60 / 61 before
-// / after waiting for a ring stage to be released (k = the weight chunk it will refill).
+// epilogues to free it).  Role 1, lane 0 of epilogue warp 0: 25 / 45 (hidden) / heads accumulators ready, 26 + c
+// hidden chunk c written to the buffer (fused), 30 (hidden) epilogue done, 50 heads epilogue done (fused), 98 the
+// launch's mode (k = IAF_MODE_*: multiconv, step, layer, logp), 99 kernel end.  Role 2, the producer: 60 / 61 before
+// / after waiting for a ring stage to be released (k = the weight chunk it will refill).  Role 3, lane 0 of the first
+// window-builder warp: 10 z window built.
 #ifdef IAF_TC_TIMELINE
 #define TL_MAX 96
 __device__ long long g_tl[4][TL_MAX][3];

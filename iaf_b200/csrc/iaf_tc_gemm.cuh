@@ -11,37 +11,48 @@
 //   * five warpgroups with their own jobs: warpgroups 0 and 1 issue the MMAs, warpgroup r for rows [64 r, +64) of the
 //     tile and ALL of the stage's columns (one wgmma m64nNk16 per K-step, tap and product; two per K-step and tap, the
 //     second of twice the width, for spans of at most 64 columns; two of half the width for stages of 129-160 columns;
-//     two passes over K for 161-192), accumulating in registers; warpgroups 2 and 3 build the first stage's z window and
-//     run the epilogues; in warpgroup 4, warp 16 is the producer and warp 17 the reducer.  setmaxnreg moves registers
-//     from warpgroup 4 to the MMA warpgroups;
+//     two passes over K for 161-192), accumulating in registers; warpgroups 2 and 3 run the epilogues; in warpgroup 4,
+//     warp 16 is the producer, warp 17 the reducer and warps 18 and 19 build the first stage's z window.  setmaxnreg
+//     moves registers from warpgroup 4 to the MMA warpgroups;
 //   * the accumulators go through a shared-memory tile [128][N + 4] so that the epilogue keeps one thread per slot
 //     (coalesced global traffic along pixels).  The tile, the z window and the fused kernel's hidden operand buffer
-//     are handed between the MMA and epilogue warpgroups through full / empty mbarrier pairs, so an epilogue runs
-//     while the MMAs of the next tile (or stage) are in flight: the MMA warpgroups' registers are the second buffer;
+//     are handed between the MMA warpgroups and the warps that fill or drain them through full / empty mbarrier pairs,
+//     so an epilogue runs while the MMAs of the next tile (or stage) are in flight: the MMA warpgroups' registers are the
+//     second buffer.  The fused kernel's hidden buffer is handed over per 16-channel chunk, so the heads MMAs of a chunk
+//     run while the hidden epilogue computes the later ones;
 //   * hidden stages write their output operand image back to global memory (16-byte stores), the heads stage applies
 //     the affine update; per-sample sums go through the reducer warp in fixed order.
 #pragma once
 
+#include <type_traits>
+
 #define LY_MMA_WARPS 8                   // warpgroups 0, 1: the MMAs
-#define LY_EPI_WARP0 8                   // warpgroups 2, 3: z window and epilogues
+#define LY_EPI_WARP0 8                   // warpgroups 2, 3: the epilogues
 #define LY_EPI_WARPS 8
 #define LY_ETHREADS (LY_EPI_WARPS * 32)
-#define LY_TMA_WARP 16                   // warpgroup 4: the producer, the reducer and two idle warps
+#define LY_TMA_WARP 16                   // warpgroup 4: the producer, the reducer and two window builders
 #define LY_RED_WARP 17
 #define LY_THREADS 640
 // registers per thread after setmaxnreg.  The launch gives each of the 640 threads 96 (61,440 in all); warpgroup 4
-// returns 48 of them and the MMA warpgroups take 24 more, for up to 80 accumulators (64 x 160 fp32 over 128 threads, or
-// 2 x 64 x 64 when the correction products are summed apart) beside their descriptors and counters.  The epilogue
-// warpgroups keep 96.  ptxas compiles the code after setmaxnreg.inc to the raised count, but each single wgmma must
-// still fit the launch's 96: hence two instructions of half the width for 160 columns (ly_mma_tile).  96 accumulators
-// (a 192-column span) do not fit in 120: stages of 161-192 columns run two passes over K of 96 columns each.
-#define LY_REGS_AUX 48
-#define LY_REGS_MMA 120
+// (producer, reducer, window builders) returns some of them to the MMA warpgroups, which hold up to 80 accumulators
+// (64 x 160 fp32 over 128 threads) or 64 (2 x 64 x 64 when the correction products are summed apart) beside their
+// descriptors and counters; the epilogue warpgroups keep 96.  Stages of 129-160 columns (NGW 5, 80 accumulators): MMA
+// 112, warpgroup 4 64.  Every other instantiation (at most 64 accumulators): MMA 104, warpgroup 4 80, where the reducer
+// and the window builders do not spill (at 48 the layer and logp variants spilled 12-44 B of stores).  Either way
+// 256 x MMA + 128 x aux = 256 x 120 + 128 x 48.  ptxas compiles the code after setmaxnreg.inc to the raised count, but
+// each single wgmma must still fit the launch's 96: hence two instructions of half the width for 160 columns
+// (ly_mma_tile).  96 accumulators (a 192-column span) do not fit: stages of 161-192 columns run two passes over K of
+// 96 columns each.
+__host__ __device__ constexpr int ly_regs_mma(int ngw) { return ngw == 5 ? 112 : 104; }
+__host__ __device__ constexpr int ly_regs_aux(int ngw) { return 48 + 2 * (120 - ly_regs_mma(ngw)); }
 // per-sample partials of one tile (step and multiconv modes): one per (set of column groups g with the same g % 4,
 // quarter of the tile's slots), summed by the reducer warp in that fixed order
 #define LY_PART_SETS 16
 #define LY_KC 5        // K-steps (of 16) per weight chunk
 #define LY_MAX_NB 6
+#define LY_H_CHUNKS 4  // fused: 16-channel chunks of the hidden operand buffer (hidden width <= 32 FZ_NGW = 64)
+#define LY_WIN_WARP0 18  // warpgroup 4's last two warps build the first stage's z window
+#define LY_WIN_WARPS 2
 // Stages whose MMA warpgroup spans at most 32 LY_SPLIT_NGW columns (SPLIT, see ly_mma_tile) sum the correction products
 // apart and keep their weights as one image [K/8][2 NS][8], NS = 32 NGW the span: each K plane holds the lo columns
 // [0, NS), then the hi columns [NS, 2 NS), both halves zero from N on.  Wider stages keep a hi and a lo image [K/8][N][8].
@@ -56,10 +67,11 @@
 enum { LB_BFULL = 0, LB_BEMPTY = LY_MAX_NB, LB_PART = 2 * LY_MAX_NB,
        LB_PART_EMPTY = 2 + 2 * LY_MAX_NB,  // + tile parity: the reducer warp has consumed the partials
        // MMA <-> epilogue handoffs, one phase per use (parity = use & 1): the accumulator tile (written by the MMA warps,
-       // read by the epilogue warps), the z window (written by the epilogue warps, read by the MMA warpgroups) and the
-       // fused kernel's hidden operand buffer (likewise)
-       LB_ACC_FULL = 4 + 2 * LY_MAX_NB, LB_ACC_EMPTY, LB_WIN_FULL, LB_WIN_EMPTY, LB_H_FULL, LB_H_EMPTY,
-       LB_COUNT };
+       // read by the epilogue warps), the z window (written by the builder warps, read by the MMA warpgroups) and the
+       // fused kernel's hidden operand buffer (written by the epilogue warps, read by the MMA warpgroups): full per
+       // 16-channel chunk c, LB_H_FULL + c, so that the heads MMAs of chunk c start once the epilogue has written it
+       LB_ACC_FULL = 4 + 2 * LY_MAX_NB, LB_ACC_EMPTY, LB_WIN_FULL, LB_WIN_EMPTY, LB_H_EMPTY, LB_H_FULL,
+       LB_COUNT = LB_H_FULL + LY_H_CHUNKS };
 
 struct IafLyParams {
   IafTcParams t;               // geometry, pointers, slot decoding (t.st[0] describes THIS stage)
@@ -133,7 +145,8 @@ __device__ __forceinline__ float dg_scale_from_amax(float amax) {
 //   in ring stage g % NB (parity from g / NB), released after its MMAs complete;
 //   otherwise resident: chunk c sits in stage c behind barrier bar0 + c (parity 0).
 //   a_in_stage: the A chunk pair of K-step c rides in the ring stage before the weights; otherwise A is a window at a_addr,
-//   and barrier a_release (if >= 0) is arrived on once the MMAs have read it.
+//   and barrier a_release (if >= 0) is arrived on once the MMAs have read it.  a_full (if >= 0): chunk c of the window
+//   is written while earlier chunks are multiplied, and its MMAs wait on barrier a_full + c (parity a_parity).
 // the two MMA warpgroups converge here before a stage's MMAs: without a barrier between the per-thread mbarrier waits
 // and the accumulator set-up, ptxas treats the wgmma sequence as divergent code and serializes every wgmma
 __device__ __forceinline__ void mma_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(LY_MMA_WARPS * 32) : "memory"); }
@@ -142,7 +155,8 @@ template <int SPG, bool SPLIT>
 __device__ __forceinline__ void ly_mma_tile(float* acc, uint64_t* bars, int N, int col0, int n_chunks, bool ring, int NB,
                                             int gchunk, int bar0, uint32_t b_addr0, uint32_t stage_bytes,
                                             uint32_t b_lo_off, bool a_in_stage, uint32_t a_addr, uint32_t a_plane,
-                                            uint32_t a_lo_off, int Wp, int a_release) {
+                                            uint32_t a_lo_off, int Wp, int a_release, int a_full = -1,
+                                            uint32_t a_parity = 0u) {
   constexpr int NA = 8 * SPG;          // accumulators per thread: 64 x 16 SPG over the 128 threads of the warpgroup
   constexpr int NI = SPG > 8 ? 2 : 1;  // wgmma instructions per product
   constexpr int GI = SPG / NI;         // 16-column groups per instruction
@@ -165,6 +179,7 @@ __device__ __forceinline__ void ly_mma_tile(float* acc, uint64_t* bars, int N, i
   for (int c = 0; c < n_chunks; ++c) {
     const int stg = ring ? (int)((uint32_t)gchunk % (uint32_t)NB) : c;
     mbar_wait(&bars[bar0 + stg], ring ? ((uint32_t)gchunk / (uint32_t)NB) & 1u : 0u);
+    if (a_full >= 0) mbar_wait(&bars[a_full + c], a_parity);
     const uint32_t sbase = b_addr0 + (uint32_t)stg * stage_bytes;
     uint32_t ah0, al0, bbase;
     if (a_in_stage) {
@@ -248,6 +263,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   const int HW = p.HW;
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t bars[LB_COUNT];
+  __shared__ int s_win_next[2];  // first stage: the next unclaimed z-window item of the tiles with parity 0 / 1
   TL_DECL
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -264,6 +280,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   constexpr int NP = NGW > 5 ? 2 : 1;
   constexpr int SPG = 2 * NGW / NP;
   constexpr bool SPLIT = NGW <= LY_SPLIT_NGW;
+  constexpr int REGS_MMA = ly_regs_mma(NGW), REGS_AUX = ly_regs_aux(NGW);
 
   // programmatic dependent launch: everything up to the barrier init overlaps the previous grid
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -281,9 +298,10 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       }
       mbar_init(&bars[LB_ACC_FULL], LY_MMA_WARPS);
       mbar_init(&bars[LB_ACC_EMPTY], LY_EPI_WARPS);
-      mbar_init(&bars[LB_WIN_FULL], LY_EPI_WARPS);
+      mbar_init(&bars[LB_WIN_FULL], LY_WIN_WARPS + LY_EPI_WARPS);
+      s_win_next[0] = s_win_next[1] = 0;
       mbar_init(&bars[LB_WIN_EMPTY], 2);
-      mbar_init(&bars[LB_H_FULL], LY_EPI_WARPS);
+      for (int c = 0; c < LY_H_CHUNKS; ++c) mbar_init(&bars[LB_H_FULL + c], LY_EPI_WARPS);
       mbar_init(&bars[LB_H_EMPTY], 2);
       fence_barrier_init();
     }
@@ -303,8 +321,57 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   if (!epi) asm volatile("griddepcontrol.wait;" ::: "memory");
   __syncthreads();
 
+  // fp32 z (layer mode: post_mean + exp(post_logsd) z) -> the fp16 hi/lo A window of the CTA's i-th tile (first stage).
+  // Items are (chunk of 8 channels, window slot).  The builder warps and, once their hidden epilogue is done, the
+  // epilogue warps claim them 32 K at a time from the tile's counter, so the window is shared by whoever is free; each
+  // lane keeps the loads of its K items in flight.  Then the warp hands its part to the MMAs.
+  auto build_window = [&](int i, auto k_) {
+    constexpr int K = decltype(k_)::value;
+    const int u = (int)blockIdx.x + i * (int)gridDim.x;
+    const int n_items = p.WIN * nchunk;
+#pragma unroll 1
+    for (;;) {
+      int base = 0;
+      if (lane == 0) base = atomicAdd(&s_win_next[i & 1], 32 * K);
+      base = __shfl_sync(0xffffffffu, base, 0);
+      if (base >= n_items) break;
+      float v[K][8];
+#pragma unroll
+      for (int h = 0; h < K; ++h) {
+        const int idx = base + 32 * h + lane;
+        const int ch = fast_div(idx, p.WIN, p.mg_win);
+        const SlotInfo si = decode_slot(p, u * q.TS + idx - ch * p.WIN, HW);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) v[h][e] = 0.f;
+        if (si.valid && idx < n_items) {
+          const size_t g = ((size_t)si.n * p.C + ch * 8) * HW + si.gp;
+#pragma unroll
+          for (int e = 0; e < 8; ++e) v[h][e] = __ldg(p.z + g + (size_t)e * HW);
+          if (MODE == IAF_MODE_LAYER) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+              v[h][e] = fmaf(fast_exp(__ldg(p.post_logsd + g + (size_t)e * HW)), v[h][e],
+                             __ldg(p.post_mean + g + (size_t)e * HW));
+          }
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < K; ++h) {
+        const int idx = base + 32 * h + lane;
+        if (idx < n_items) {
+          const int ch = fast_div(idx, p.WIN, p.mg_win);
+          uint8_t* dst = smem + q.sm_a + ch * a_plane + (idx - ch * p.WIN) * 16;
+          split_store8(v[h], dst, dst + a_lo_off);
+        }
+      }
+    }
+    fence_proxy_async();  // generic-proxy stores -> the wgmma (async proxy) reads of the window
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[LB_WIN_FULL]);
+  };
+
   if (warp >= LY_TMA_WARP) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(LY_REGS_AUX));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS_AUX));
     if (warp == LY_TMA_WARP) {
       // ===================== producer: A windows (operand-image input) and the weight ring =====================
       if (lane == 0 && FUSED) {
@@ -416,11 +483,22 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars[LB_PART_EMPTY + pb]);
       }
+    } else if (warp >= LY_WIN_WARP0 && !q.in_mode) {
+      // ===================== window builders: tile i's z window once the MMAs have read tile i - 1's ================
+      // four items per lane in flight at 80 registers, two at 64
+      for (int i = 0; i < n_my; ++i) {
+        if (i >= 1) mbar_wait(&bars[LB_WIN_EMPTY], (uint32_t)((i - 1) & 1));
+        // every claim on the other counter (tile i - 1's) was made before its window was handed over: reset it for
+        // tile i + 1, whose builders start only after this warp's arrival on tile i's window
+        if (warp == LY_WIN_WARP0 && lane == 0) s_win_next[(i + 1) & 1] = 0;
+        build_window(i, std::integral_constant<int, (REGS_AUX >= 80 ? 4 : 2)>{});
+        if (warp == LY_WIN_WARP0 && lane == 0) TL(3, 10, i);
+      }
     }
-    // warps 18 and 19 have nothing to do: they wait at the closing barrier with their 40 registers
+    // otherwise (operand-image stages, or no per-sample outputs) the warp waits at the closing barrier
   } else if (warp < LY_MMA_WARPS) {
     // ===================== MMA warpgroups: a tile's MMAs run while the epilogue warps finish the previous one =======
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(LY_REGS_MMA));
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_MMA));
     float acc[(SPLIT ? 2 : 1) * 8 * SPG];  // SPLIT: room for the correction sum (ly_mma_tile)
     const bool tl0 = warp == 0 && lane == 0;
     for (int i = 0; i < n_my; ++i) {
@@ -442,13 +520,15 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       if (FUSED) {
         const IafTcStage& St1 = p.st[1];
         const int h_plane = (TC_TILE + p.MIR) * 16;
+        // heads weight chunk c reads hidden channels [16 c, +16): its MMAs start as soon as the epilogue has written
+        // them, while it computes the later chunks
         mbar_wait(&bars[LB_H_FULL], (uint32_t)(i & 1));
         mma_bar_sync();
         if (tl0) TL(0, 35, i);
         ly_mma_tile<SPG, SPLIT>(acc, bars, St1.N, 0, q.n_bchunks1, false, 1, 0, LB_BFULL + q.n_bchunks,
                                 smem_u32(smem + q.sm_b1), (uint32_t)q.b_chunk_bytes1, (uint32_t)(q.b_chunk_bytes1 / 2),
                                 false, smem_u32(smem + q.sm_h), (uint32_t)h_plane, (uint32_t)((St1.cin >> 3) * h_plane),
-                                p.Wp, LB_H_EMPTY);
+                                p.Wp, LB_H_EMPTY, LB_H_FULL, (uint32_t)(i & 1));
         if (tl0) TL(0, 40, i);
         ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St1.N, 0, 2 * i + 1, true, true);
         if (tl0) TL(0, 41, i);
@@ -463,12 +543,12 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     const int sl = qd * 32 + lane;
     float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
     float* s_acc = reinterpret_cast<float*>(smem + q.sm_acc);
-    // this thread's slot row of the accumulator tile, 16 columns from c0, times the columns' inverse weight scales
+    // this thread's slot row of the accumulator tile, 8 (16) columns from c0, times the columns' inverse weight scales
     // (exact: powers of two; wsinv null = unscaled images, the data gradient's)
-    auto acc_ld16 = [&](int c0, uint32_t* r, int pitch, const float* wsinv) {
+    auto acc_ld8 = [&](int c0, uint32_t* r, int pitch, const float* wsinv) {
       const float4* s4 = reinterpret_cast<const float4*>(s_acc + sl * pitch + c0);
 #pragma unroll
-      for (int e4 = 0; e4 < 4; ++e4) {
+      for (int e4 = 0; e4 < 2; ++e4) {
         float4 v4 = s4[e4];
         if (wsinv) {
           const float4 w4 = __ldg(reinterpret_cast<const float4*>(wsinv + c0) + e4);
@@ -478,61 +558,46 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
         r[4 * e4 + 2] = __float_as_uint(v4.z); r[4 * e4 + 3] = __float_as_uint(v4.w);
       }
     };
-    const int h_plane = (TC_TILE + p.MIR) * 16;  // fused: bytes per chunk plane of the hidden operand buffer
-
-    // fp32 z -> fp16 hi/lo A window of this CTA's i-th tile, once the MMAs have read tile i - 1's; handed to the MMAs
-    auto build_window = [&](int i) {
-      if (i >= 1) mbar_wait(&bars[LB_WIN_EMPTY], (uint32_t)((i - 1) & 1));
-      const int u = (int)blockIdx.x + i * (int)gridDim.x;
-#pragma unroll
-      for (int it = 0; it < TC_ZITEMS; ++it) {
-        const int idx = et + it * LY_ETHREADS;
-        if (idx < p.WIN * nchunk) {
-          const int ch = fast_div(idx, p.WIN, p.mg_win);
-          const int s_ = idx - ch * p.WIN;
-          const SlotInfo si = decode_slot(p, u * q.TS + s_, HW);
-          float v[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) v[e] = 0.f;
-          if (si.valid) {
-            const size_t g = ((size_t)si.n * p.C + ch * 8) * HW + si.gp;
-#pragma unroll
-            for (int e = 0; e < 8; ++e) v[e] = __ldg(p.z + g + (size_t)e * HW);
-            if (MODE == IAF_MODE_LAYER) {
-#pragma unroll
-              for (int e = 0; e < 8; ++e)
-                v[e] = fmaf(fast_exp(__ldg(p.post_logsd + g + (size_t)e * HW)), v[e], __ldg(p.post_mean + g + (size_t)e * HW));
-            }
-          }
-          uint8_t* dst = smem + q.sm_a + ch * a_plane + s_ * 16;
-          split_store8(v, dst, dst + a_lo_off);
-        }
-      }
-      fence_proxy_async();  // generic-proxy stores -> the wgmma (async proxy) reads of the window
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[LB_WIN_FULL]);
-      if (ew == 0 && lane == 0) TL(1, 10, i);
+    auto acc_ld16 = [&](int c0, uint32_t* r, int pitch, const float* wsinv) {
+      acc_ld8(c0, r, pitch, wsinv);
+      acc_ld8(c0 + 8, r + 8, pitch, wsinv);
     };
+    const int h_plane = (TC_TILE + p.MIR) * 16;  // fused: bytes per chunk plane of the hidden operand buffer
     // this warp is done reading the accumulator tile
     auto acc_release = [&]() {
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars[LB_ACC_EMPTY]);
     };
 
-    if (!q.in_mode) build_window(0);
+    // the epilogue warps' share of tile i's window (which they start once the MMAs have read tile i - 1's)
+    auto help_window = [&](int i) {
+      if (i >= 1) mbar_wait(&bars[LB_WIN_EMPTY], (uint32_t)((i - 1) & 1));
+      build_window(i, std::integral_constant<int, 2>{});
+      if (ew == 0 && lane == 0) TL(1, 10, i);
+    };
+    if (!q.in_mode) help_window(0);
 
     for (int i = 0; i < n_my; ++i) {
       const int u = (int)blockIdx.x + i * (int)gridDim.x;
-      // per stage: the next tile's window goes to the MMAs before this tile's epilogue, which then runs under them
-      if (!FUSED && !q.in_mode && i + 1 < n_my) build_window(i + 1);
-      // the accumulator tile's uses: one per tile, or (fused) 2i for the hidden stage and 2i + 1 for the heads
-      mbar_wait(&bars[LB_ACC_FULL], FUSED ? 0u : (uint32_t)(i & 1));
-      if (ew == 0 && lane == 0) TL(1, 25, i);
+      // per stage: help with the next tile's window before this tile's epilogue, which then runs under its MMAs
+      if (!FUSED && !q.in_mode && i + 1 < n_my) help_window(i + 1);
       const SlotInfo si_all = decode_slot(p, u * q.TS + sl, HW);
       const bool bx0 = (si_all.x == 0), bxW = (si_all.x == p.W - 1), byH = (si_all.y == p.H - 1);
+      // the accumulator tile's uses: one per tile, or (fused) 2i for the hidden stage and 2i + 1 for the heads.  Each
+      // epilogue issues its first input loads (context, z), which do not depend on the MMAs, before waiting on it
+      auto acc_wait = [&](uint32_t parity, int tag) {
+        mbar_wait(&bars[LB_ACC_FULL], parity);
+        if (ew == 0 && lane == 0) TL(1, tag, i);
+      };
 
-      // hidden stage epilogue: the next operand (global image, or the fused kernel's shared-memory buffer)
-      auto hidden_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch, const SlotInfo si) {
+      // hidden stage epilogue: the next operand (global image, or the fused kernel's shared-memory buffer).  Warp ew
+      // covers slots [32 qd, +32).  Fused: two threads per slot, channels [8 cg, +8) of each 16-channel group, all eight
+      // warps on one group at a time, so that the buffer goes to the heads MMAs chunk by chunk, the first after an
+      // ngroups-th of the epilogue.  Per stage: one thread per slot and 16 channels, groups cg, cg + 2, ...  Every
+      // element is computed the same way under either mapping.
+      constexpr int HC = FUSED ? 8 : 16;  // channels per thread and group
+      auto hidden_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch, const SlotInfo si,
+                            uint32_t acc_parity) {
         auto store_operand = [&](const float* v8, int chunk) {
           if (FUSED) {
             uint8_t* dst = smem + q.sm_h + chunk * h_plane + sl * 16;
@@ -543,35 +608,40 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
           }
         };
           // context of the NEXT column group is fetched while the current one is computed
-          float cxn[16];
+          const int g0 = FUSED ? 0 : cg, gs = FUSED ? 1 : CGS, co = FUSED ? 8 * cg : 0;
+          float cxn[HC];
           auto fetch_ctx = [&](int g) {
             if (q.first && si.valid && g < ngroups) {  // += context   (ar.py:402 / layers.py:163)
-              const float* cp = p.ctx + ((size_t)si.n * St.N + g * 16) * HW + si.gp;
+              const float* cp = p.ctx + ((size_t)si.n * St.N + g * 16 + co) * HW + si.gp;
   #pragma unroll
-              for (int e = 0; e < 16; ++e) cxn[e] = __ldg(cp + (size_t)e * HW);
+              for (int e = 0; e < HC; ++e) cxn[e] = __ldg(cp + (size_t)e * HW);
             } else {
   #pragma unroll
-              for (int e = 0; e < 16; ++e) cxn[e] = 0.f;
+              for (int e = 0; e < HC; ++e) cxn[e] = 0.f;
             }
           };
-          fetch_ctx(cg);
-          for (int g = cg; g < ngroups; g += CGS) {
-            const int c0 = g * 16;
-            float cx[16];
+          fetch_ctx(g0);
+          // fused: refill the buffer once the heads MMAs of tile i - 1 have read it
+          if (FUSED && i >= 1) mbar_wait(&bars[LB_H_EMPTY], (uint32_t)((i - 1) & 1));
+          acc_wait(acc_parity, 25);
+          for (int g = g0; g < ngroups; g += gs) {
+            const int c0 = g * 16 + co;  // this thread's HC columns
+            float cx[HC];
   #pragma unroll
-            for (int e = 0; e < 16; ++e) cx[e] = cxn[e];
-            fetch_ctx(g + CGS);
-            uint32_t r[16];
-            acc_ld16(c0, r, pitch, St.wsinv);
+            for (int e = 0; e < HC; ++e) cx[e] = cxn[e];
+            fetch_ctx(g + gs);
+            uint32_t r[HC];
+            if (HC == 8) acc_ld8(c0, r, pitch, St.wsinv);
+            else acc_ld16(c0, r, pitch, St.wsinv);
             if (q.bwd) {
               // data gradient: acc = (c W)^T g (scaled units); / c (exact: a power of two), x nl'(h), evaluated from the
               // activation itself
               const float sc = si.valid ? dg_scale_from_amax(__ldg(q.amax + si.n)) : 1.0f;
               const float inv = 1.0f / sc;
               const float winv = 1.0f / __ldg(q.wscale);
-              float vb[16];
+              float vb[HC];
   #pragma unroll
-              for (int e = 0; e < 16; ++e) {
+              for (int e = 0; e < HC; ++e) {
                 const float a = __uint_as_float(r[e]) * winv;
                 const float d = (q.bwd == 1) ? dg_nl_grad(cx[e], p.nl) : 1.0f;
                 vb[e] = si.valid ? a * d : 0.f;
@@ -580,21 +650,18 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                 float* hp = St.hid_out + ((size_t)si.n * St.N + c0) * HW + si.gp;
                 if (q.bwd == 2) {
   #pragma unroll
-                  for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] += vb[e] * inv;
+                  for (int e = 0; e < HC; ++e) hp[(size_t)e * HW] += vb[e] * inv;
                 } else {
   #pragma unroll
-                  for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] = vb[e] * inv;
+                  for (int e = 0; e < HC; ++e) hp[(size_t)e * HW] = vb[e] * inv;
                 }
               }
               if (u < p.NT && q.o_hi) {
   #pragma unroll
-                for (int hch = 0; hch < 2; ++hch) {
-                  store_operand(vb + 8 * hch, (c0 >> 3) + hch);
-                }
+                for (int hch = 0; hch < HC / 8; ++hch) store_operand(vb + 8 * hch, (c0 >> 3) + hch);
               }
-              continue;
-            }
-            float v[16];
+            } else {
+            float v[HC];
             {
               // branch-free: bias rows come in as 16-byte vectors, the pad-channel terms (conv.py:77-83: the pad
               // channel is 1 where a tap falls outside the image) are 0/1-weighted FMAs, and an invalid slot
@@ -602,9 +669,9 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
               // a multiply: the zero row of sample n - 1 is computed from row 0 of sample n (every tap shift is
               // forward), and NaN * 0 would carry a non-finite sample n into its neighbour's outputs
               const float4* tb4 = reinterpret_cast<const float4*>(tb + c0);
-              float bsv[16];
+              float bsv[HC];
   #pragma unroll
-              for (int e4 = 0; e4 < 4; ++e4) {
+              for (int e4 = 0; e4 < HC / 4; ++e4) {
                 const float4 t4 = tb4[e4];
                 bsv[4 * e4] = t4.x; bsv[4 * e4 + 1] = t4.y; bsv[4 * e4 + 2] = t4.z; bsv[4 * e4 + 3] = t4.w;
               }
@@ -612,12 +679,12 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                 const float f1 = bxW ? 1.f : 0.f, f2 = (byH || bx0) ? 1.f : 0.f, f3 = byH ? 1.f : 0.f,
                             f4 = (byH || bxW) ? 1.f : 0.f;
   #pragma unroll
-                for (int e = 0; e < 16; ++e)
+                for (int e = 0; e < HC; ++e)
                   bsv[e] += f1 * tb[St.N + c0 + e] + f2 * tb[2 * St.N + c0 + e] + f3 * tb[3 * St.N + c0 + e] +
                             f4 * tb[4 * St.N + c0 + e];
               }
   #pragma unroll
-              for (int e = 0; e < 16; ++e) {
+              for (int e = 0; e < HC; ++e) {
                 const float a = __uint_as_float(r[e]) + bsv[e] + cx[e];
                 float o;
                 if (NLT == IAF_NL_ELU) {
@@ -632,18 +699,24 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             if (St.hid_out && si.valid && sl < q.TO && u < p.NT) {  // training forward: keep the activations for iaf_step_bwd_saved
               float* hp = St.hid_out + ((size_t)si.n * St.N + c0) * HW + si.gp;
   #pragma unroll
-              for (int e = 0; e < 16; ++e) hp[(size_t)e * HW] = v[e];
+              for (int e = 0; e < HC; ++e) hp[(size_t)e * HW] = v[e];
             }
             if (u < p.NT) {
   #pragma unroll
-              for (int hch = 0; hch < 2; ++hch) {
-                store_operand(v + 8 * hch, (c0 >> 3) + hch);
-              }
+              for (int hch = 0; hch < HC / 8; ++hch) store_operand(v + 8 * hch, (c0 >> 3) + hch);
+            }
+            }
+            if (FUSED) {  // chunk g of the buffer (both of its planes, all slots) goes to the heads MMAs
+              fence_proxy_async();  // generic-proxy stores -> the heads' wgmma reads of the buffer
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&bars[LB_H_FULL + g]);
+              if (ew == 0 && lane == 0) TL(1, 26 + g, i);
             }
           }
       };
       // heads epilogue: affine update, per-element and per-sample outputs
-      auto heads_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch, const SlotInfo si) {
+      auto heads_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch, const SlotInfo si,
+                           uint32_t acc_parity, int acc_tag) {
           // ---------------- heads: affine update, per-element and per-sample outputs ----------------
           // layer and logp modes: per-(sample, channel) partials, the 8 channels of a column group apart
           constexpr bool PERCH = (MODE == IAF_MODE_LAYER || MODE == IAF_MODE_LOGP);
@@ -660,18 +733,31 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
           const int n_last = min(p.B - 1, fast_div(tile_s0 + q.TS - 1, p.SPS, p.mg_sps));
           const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
           const int pb = i & 1;
+          // z of the NEXT column group is fetched while the current one is computed, the first before the accumulator
+          // wait
+          float zvn[8];
+          auto fetch_z = [&](int g) {
+            if (si.valid && g < ngroups) {
+              const float* zp = p.z + ((size_t)si.n * p.C + g * 8) * HW + si.gp;
+  #pragma unroll
+              for (int e = 0; e < 8; ++e) zvn[e] = __ldg(zp + (size_t)e * HW);
+            } else {
+  #pragma unroll
+              for (int e = 0; e < 8; ++e) zvn[e] = 0.f;
+            }
+          };
+          fetch_z(cg);
           if (PERCH && (p.persample_out || p.bc_out) && i >= 2)
             mbar_wait(&bars[LB_PART_EMPTY + pb], (uint32_t)(((i >> 1) - 1) & 1));
+          acc_wait(acc_parity, acc_tag);
           for (int g = cg; g < ngroups; g += CGS) {
             const int c0 = g * 16;
             const int ch0 = g * 8;
             float zv[8];
-            size_t gi = 0;
-            if (si.valid) {
-              gi = ((size_t)si.n * p.C + ch0) * HW + si.gp;
   #pragma unroll
-              for (int e = 0; e < 8; ++e) zv[e] = __ldg(p.z + gi + (size_t)e * HW);
-            }
+            for (int e = 0; e < 8; ++e) zv[e] = zvn[e];
+            fetch_z(g + CGS);
+            const size_t gi = si.valid ? ((size_t)si.n * p.C + ch0) * HW + si.gp : 0;
             uint32_t r[16];
             acc_ld16(c0, r, pitch, St.wsinv);
             const bool set_hi = ((g - cg) / CGS) & 1;
@@ -765,27 +851,23 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
 
       const float* tb0 = reinterpret_cast<const float*>(smem + q.sm_bias);
       if (FUSED) {
-        // the hidden epilogue refills the hidden operand buffer once the heads MMAs of tile i - 1 have read it
-        if (i >= 1) mbar_wait(&bars[LB_H_EMPTY], (uint32_t)((i - 1) & 1));
-        hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
-        fence_proxy_async();  // generic-proxy stores -> the heads' wgmma reads of the buffer
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars[LB_H_FULL]);
+        // the hidden epilogue runs under the heads MMAs of its earlier chunks, the heads epilogue under the next tile's
+        // hidden MMAs
+        hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, 0u);
         acc_release();
         if (ew == 0 && lane == 0) TL(1, 30, i);
-        // the next tile's window is built under the heads MMAs, the heads epilogue runs under the next hidden MMAs
-        if (i + 1 < n_my) build_window(i + 1);
-        mbar_wait(&bars[LB_ACC_FULL], 1u);
-        if (ew == 0 && lane == 0) TL(1, 45, i);
+        // under the heads MMAs: the rest of the next tile's window, beside the builder warps
+        if (i + 1 < n_my) help_window(i + 1);
         const IafTcStage& St1 = p.st[1];
         SlotInfo si_out = si_all;
         si_out.valid = si_all.valid && sl < q.TO;
-        heads_epi(St1, reinterpret_cast<const float*>(smem + q.sm_bias1), St1.N >> 4, ly_acc_pitch(St1.N), si_out);
+        heads_epi(St1, reinterpret_cast<const float*>(smem + q.sm_bias1), St1.N >> 4, ly_acc_pitch(St1.N), si_out, 1u,
+                  45);
         acc_release();
         if (ew == 0 && lane == 0) TL(1, 50, i);
       } else {
-        if (!q.is_heads) hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
-        else heads_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all);
+        if (!q.is_heads) hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, (uint32_t)(i & 1));
+        else heads_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, (uint32_t)(i & 1), 25);
         acc_release();
         if (ew == 0 && lane == 0) TL(1, 30, i);
       }

@@ -25,7 +25,8 @@ from bench import make_workload  # noqa: E402
 PHASE = {15: "MMA operands ready", 20: "MMAs done", 21: "acc tile written", 35: "heads operands ready",
          40: "heads MMAs done", 41: "heads acc written", 10: "window built", 25: "acc ready", 30: "(hidden) epilogue done",
          45: "heads acc ready", 50: "heads epilogue done", 99: "end"}
-ROLE = {0: "MMA warpgroups", 1: "epilogue warps"}
+PHASE.update({26 + c: "hidden chunk %d ready" % c for c in range(4)})
+ROLE = {0: "MMA warpgroups", 1: "epilogue warps", 3: "window builders"}
 
 
 def run(name, stage):
@@ -61,10 +62,16 @@ def run(name, stage):
     print("=== %s, stage %s: %d events ===" % (name, "last" if stage is None else stage, len(ev)))
     for t, role, tag, k in ev:
         print("%9d  role%d  %-24s k=%d" % (t, role, PHASE.get(tag, {60: "ring wait", 61: "ring released"}.get(tag, tag)), k))
+    # tile period: from one tile's heads accumulators written to the next's, on the MMA side
+    ends = [t for t, role, tag, _ in ev if role == 0 and tag == 41]
+    if len(ends) > 1:
+        print("--- tile period (MMA side): %s cycles ---" % " ".join(str(b - a) for a, b in zip(ends, ends[1:])))
     # phase cycles per role: its events are phase ends, in order; each phase lasts from the previous event to its own.
     # The two roles run concurrently, so their phases of neighbouring tiles overlap in time (compare the t column).
-    for role in (0, 1):
+    for role in (0, 1, 3):
         w = [e for e in ev if e[1] == role]
+        if not w:
+            continue
         print("--- %s: cycles per phase (lane 0 of its first warp) ---" % ROLE[role])
         for (t0, _, g0, k0), (t1, _, g1, k1) in zip(w, w[1:]):
             print("tile %d  %-24s -> %-24s %7d  (ends at %d)" % (k1 if g1 != 99 else k0, PHASE.get(g0), PHASE.get(g1),
