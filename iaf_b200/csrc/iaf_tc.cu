@@ -260,8 +260,9 @@ __device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, ui
 // launch that sets tl_enable records (tag, tile or chunk, clock) triples per role, each at the end of a phase of its own
 // warp (other warps of the role may still be in it).  Role 0, lane 0 of MMA warp 0: 15 / 35 the (hidden) / heads MMAs'
 // operands ready, 20 / 40 their MMAs done, 21 / 41 their fragments in the accumulator tile (after waiting for the
-// epilogues to free it).  Role 1, lane 0 of epilogue warp 0: 25 / 45 (hidden) / heads accumulators ready, 26 + c
-// hidden chunk c written to the buffer (fused), 30 (hidden) epilogue done, 50 heads epilogue done (fused), 98 the
+// epilogues to free it), 12 the halo block's MMAs done (fused).  Role 1, lane 0 of epilogue warp 0: 25 / 45 (hidden) /
+// heads accumulators ready, 26 + c hidden chunk c written to the buffer (fused), 30 (hidden) epilogue done, 50 heads
+// epilogue done (fused), 13 / 14 the halo block's accumulators ready / epilogue done, 24 carry done (fused), 98 the
 // launch's mode (k = IAF_MODE_*: multiconv, step, layer, logp), 99 kernel end.  Role 2, the producer: 60 / 61 before
 // / after waiting for a ring stage to be released (k = the weight chunk it will refill).  Role 3, lane 0 of the first
 // window-builder warp: 10 z window built.
@@ -530,8 +531,9 @@ static bool ly_layout(const iaf_desc_t* d, IafTcPlan* pl) {
 }
 
 // one-launch layout (after ly_layout filled cin / N / K / MIR / WIN / MAXS): A window, hidden operand buffer (TC_TILE + MIR
-// rows: the heads' shifted windows of the rows past TS read beyond the 128 computed rows; those rows are not stored), both
-// bias tables, the partials, the accumulator tile and both resident weight images
+// rows: the heads' taps read up to MIR rows past the tile's TC_TILE), both bias tables, the partials, the accumulator tile
+// and both resident weight images.  MIR <= TC_TILE / 2: a run's first tile gets its first MIR hidden rows from the first
+// 64 rows of a halo block
 static bool fz_layout(const iaf_desc_t* d, IafTcPlan* q) {
   if (d->n_hidden != 1 || q->N[0] > 32 * FZ_NGW || q->N[1] > 32 * FZ_NGW) return false;
   if (TC_TILE - q->MIR < TC_TILE / 2) return false;
@@ -674,8 +676,7 @@ bool iaf_tc_mode_supported(const IafTcPlan* pl, int mode) {
 static int tc_num_tiles(const IafTcPlan* pl, int B) {
   const int SPS = (pl->d.H + 1) * (pl->d.W + 1);
   if ((long long)B * SPS + TC_TILE >= (1LL << 31)) return 0;
-  const int TS = pl->fused ? TC_TILE - pl->MIR : TC_TILE;  // slots a tile advances (fused: overlapped windows)
-  return (B * SPS + TS - 1) / TS;
+  return (B * SPS + TC_TILE - 1) / TC_TILE;
 }
 
 int iaf_tc_scratch_need(const IafTcPlan* pl, int B) {
@@ -691,7 +692,6 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
   const int NT = tc_num_tiles(pl, B);
   if (NT == 0) return IAF_ERR_UNSUPPORTED;
   const int S = B * SPS;
-  const int TS = pl->fused ? TC_TILE - pl->MIR : TC_TILE;
   if (B > pl->scratch_B || NT > pl->scratch_NT) {
     if (pl->counter) cudaFree(pl->counter);
     if (pl->tilepart) cudaFree(pl->tilepart);
@@ -765,7 +765,6 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
     q.b_chunk_bytes = ly_chunk_bytes(pl->N[0], pl->NS[0]); q.n_bchunks = (pl->K[0] / 16) / LY_KC;
     q.b_chunk_bytes1 = ly_chunk_bytes(pl->N[1], pl->NS[1]); q.n_bchunks1 = (pl->K[1] / 16) / LY_KC;
     q.stage_bytes = q.b_chunk_bytes;
-    q.TS = TS; q.TO = TS;
     q.tl_enable = 1;
     if (!launch(fz_kernel_for(padw, a->mode, elu), q, pl->fz_smem)) return IAF_ERR_CUDA;
     if (n_launches) *n_launches = 1;
@@ -775,7 +774,6 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
     IafLyParams q;
     memset(&q, 0, sizeof(q));
     q.t = p;
-    q.TS = TC_TILE; q.TO = TC_TILE;
     IafTcStage& S_ = q.t.st[0];
     S_.whi = pl->whi[j]; S_.wlo = pl->wlo[j]; S_.bias = pl->bias[j];
     S_.padw = pl->padw[j]; S_.wsinv = pl->wsinv[j];
@@ -1138,7 +1136,6 @@ int iaf_dg_stage(IafDgPlan* pl, int j, const float* w_packed, int in_buf, const 
   q.bwd = hprev ? 1 : 2;
   q.amax = pl->amax;
   q.wscale = pl->wscale + j;
-  q.TS = TC_TILE; q.TO = TC_TILE;
   LyKernel lk = ly_kernel_for(false, IAF_MODE_MULTICONV, d.nl == IAF_NL_ELU, N);
   const int grid = std::min(pl->num_sms, NT);
   lk<<<grid, LY_THREADS, pl->smem[j], stream>>>(q);

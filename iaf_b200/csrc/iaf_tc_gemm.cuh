@@ -91,8 +91,6 @@ struct IafLyParams {
   int tl_enable;               // timeline builds only: this launch flushes its events
   // one-launch step for stacks with one hidden layer (the FUSED instantiation): t.st[0] is the hidden layer, t.st[1] the
   // heads; both weight images are resident, the hidden activations stay in shared memory
-  int TS;                      // slots a tile advances: TC_TILE, or TC_TILE - MIR when fused (overlapped windows)
-  int TO;                      // rows of a tile that produce outputs (TC_TILE, or TS when fused)
   int sm_h;                    // fused: the hidden operand buffer [chunk][TC_TILE + MIR][8] hi, then lo
   int sm_b1, sm_bias1;         // fused: the heads' resident weights and bias table
   int n_bchunks1, b_chunk_bytes1;
@@ -150,6 +148,8 @@ __device__ __forceinline__ float dg_scale_from_amax(float amax) {
 // the two MMA warpgroups converge here before a stage's MMAs: without a barrier between the per-thread mbarrier waits
 // and the accumulator set-up, ptxas treats the wgmma sequence as divergent code and serializes every wgmma
 __device__ __forceinline__ void mma_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(LY_MMA_WARPS * 32) : "memory"); }
+// the epilogue warps alone
+__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 2, %0;" ::"n"(LY_ETHREADS) : "memory"); }
 
 template <int SPG, bool SPLIT>
 __device__ __forceinline__ void ly_mma_tile(float* acc, uint64_t* bars, int N, int col0, int n_chunks, bool ring, int NB,
@@ -255,8 +255,14 @@ __device__ __forceinline__ void ly_acc_store(const float* acc, uint64_t* bars, f
   if (lane == 0) mbar_arrive(&bars[LB_ACC_FULL]);
 }
 
-// NGW: ceil(N / 32); an MMA warpgroup covers the stage's columns as 2 NGW groups of 16.  FUSED: the whole step of a one-hidden-layer stack in one
-// launch (NGW covers both stages), tiles of TS = TC_TILE - MIR output slots whose 128 hidden rows overlap the next tile's.
+// NGW: ceil(N / 32); an MMA warpgroup covers the stage's columns as 2 NGW groups of 16.  Tile t covers slots
+// [TC_TILE t, +TC_TILE) in both kernels.  FUSED: the whole step of a one-hidden-layer stack in one launch (NGW covers
+// both stages).  Each CTA runs one contiguous run of tiles in ascending order.  Row j of the hidden buffer holds slot
+// TC_TILE t + j, j < TC_TILE + MIR, since the heads' taps read up to MIR rows ahead.  A tile's hidden MMAs compute rows
+// [MIR, TC_TILE + MIR) from a z window that starts MIR slots into the tile; rows [0, MIR) are the previous tile's rows
+// [TC_TILE, TC_TILE + MIR), carried to the front once its heads MMAs have released the buffer.  The run's first tile
+// gets them from a halo block: a hidden pass over a z window of its own at the tile's first slot, whose first 64 rows
+// (MIR <= 64, fz_layout) are kept.  A hidden row adds the same products in the same order whichever tile computes it.
 template <bool PADW, int MODE, int NLT, int NGW, bool FUSED>
 __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_constant__ IafLyParams q) {
   const IafTcParams& p = q.t;
@@ -271,8 +277,19 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   const int nchunk = St0.cin >> 3;
   const int a_plane = p.WIN * 16;          // bytes per chunk plane of the A window
   const int a_lo_off = nchunk * a_plane;
-  // tiles of this CTA: u = blockIdx.x + i * gridDim.x
-  const int n_my = (int)((uint32_t)(p.NT - (int)blockIdx.x + (int)gridDim.x - 1) / gridDim.x);
+  // tiles of this CTA, i = 0 .. n_my - 1: fused, the run [t0, t0 + n_my) (which tile covers which slots does not depend
+  // on the grid, only which CTA runs it); per stage, u = blockIdx.x + i * gridDim.x.  Both live in shared memory and
+  // are read where they are used: a register holding them through the whole kernel spilled at the launch's 96
+  __shared__ int s_run[2];
+  const int& t0 = s_run[0];
+  const int& n_my = s_run[1];
+  auto tile_of = [&](int i) { return FUSED ? t0 + i : (int)blockIdx.x + i * (int)gridDim.x; };
+  // z windows, use w: fused, w = 0 is the halo block's (at the run's first slot) and w = i + 1 tile i's (MIR slots into
+  // the tile); per stage, w = i is tile i's
+  constexpr int W0 = FUSED ? 1 : 0;
+  auto win_slot0 = [&](int w) {
+    return FUSED ? (w == 0 ? TC_TILE * t0 : TC_TILE * (t0 + w - 1) + p.MIR) : TC_TILE * tile_of(w);
+  };
   const bool resident = FUSED || q.n_bchunks <= q.NB;
   const bool ring = !resident || q.in_mode;
   // an MMA warpgroup's span: all 32 NGW columns, or for NGW = 6 two passes over K of 96 columns each (the ring streams
@@ -300,6 +317,11 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       mbar_init(&bars[LB_ACC_EMPTY], LY_EPI_WARPS);
       mbar_init(&bars[LB_WIN_FULL], LY_WIN_WARPS + LY_EPI_WARPS);
       s_win_next[0] = s_win_next[1] = 0;
+      // 32-bit products: NT < 2^24 (tc_num_tiles) and the grid is at most the SM count
+      const uint32_t b0 = FUSED ? blockIdx.x * (uint32_t)p.NT / gridDim.x : blockIdx.x;
+      s_run[0] = (int)b0;
+      s_run[1] = FUSED ? (int)((blockIdx.x + 1) * (uint32_t)p.NT / gridDim.x - b0)
+                       : (int)((uint32_t)(p.NT - (int)blockIdx.x + (int)gridDim.x - 1) / gridDim.x);
       mbar_init(&bars[LB_WIN_EMPTY], 2);
       for (int c = 0; c < LY_H_CHUNKS; ++c) mbar_init(&bars[LB_H_FULL + c], LY_EPI_WARPS);
       mbar_init(&bars[LB_H_EMPTY], 2);
@@ -321,18 +343,18 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   if (!epi) asm volatile("griddepcontrol.wait;" ::: "memory");
   __syncthreads();
 
-  // fp32 z (layer mode: post_mean + exp(post_logsd) z) -> the fp16 hi/lo A window of the CTA's i-th tile (first stage).
+  // fp32 z (layer mode: post_mean + exp(post_logsd) z) -> the fp16 hi/lo A window of the CTA's w-th use (first stage).
   // Items are (chunk of 8 channels, window slot).  The builder warps and, once their hidden epilogue is done, the
-  // epilogue warps claim them 32 K at a time from the tile's counter, so the window is shared by whoever is free; each
+  // epilogue warps claim them 32 K at a time from the use's counter, so the window is shared by whoever is free; each
   // lane keeps the loads of its K items in flight.  Then the warp hands its part to the MMAs.
-  auto build_window = [&](int i, auto k_) {
+  auto build_window = [&](int w, auto k_) {
     constexpr int K = decltype(k_)::value;
-    const int u = (int)blockIdx.x + i * (int)gridDim.x;
+    const int s0 = win_slot0(w);
     const int n_items = p.WIN * nchunk;
 #pragma unroll 1
     for (;;) {
       int base = 0;
-      if (lane == 0) base = atomicAdd(&s_win_next[i & 1], 32 * K);
+      if (lane == 0) base = atomicAdd(&s_win_next[w & 1], 32 * K);
       base = __shfl_sync(0xffffffffu, base, 0);
       if (base >= n_items) break;
       float v[K][8];
@@ -340,7 +362,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       for (int h = 0; h < K; ++h) {
         const int idx = base + 32 * h + lane;
         const int ch = fast_div(idx, p.WIN, p.mg_win);
-        const SlotInfo si = decode_slot(p, u * q.TS + idx - ch * p.WIN, HW);
+        const SlotInfo si = decode_slot(p, s0 + idx - ch * p.WIN, HW);
 #pragma unroll
         for (int e = 0; e < 8; ++e) v[h][e] = 0.f;
         if (si.valid && idx < n_items) {
@@ -390,7 +412,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       } else if (lane == 0) {
         int gchunk = 0;
         for (int i = 0; i < n_my; ++i) {
-          const int u = (int)blockIdx.x + i * (int)gridDim.x;
+          const int u = tile_of(i);
           // K order is [K-step within a tap][tap]: weight chunk c and A chunk pair (2c, 2c+1) are consumed together,
           // so both stream through shared memory at the pace of the MMAs
           for (int cp = 0; cp < (ring ? NP : 1) * q.n_bchunks; ++cp) {
@@ -436,11 +458,11 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
       constexpr bool LAY = (MODE == IAF_MODE_LAYER || MODE == IAF_MODE_LOGP);  // per-(sample, channel) partials
       for (int i = 0; i < n_my; ++i) {
-        const int u = (int)blockIdx.x + i * (int)gridDim.x;
+        const int u = tile_of(i);
         const int pb = i & 1;
-        const int tile_s0 = u * q.TS;
+        const int tile_s0 = u * TC_TILE;
         const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
-        const int n_last = min(p.B - 1, fast_div(tile_s0 + q.TS - 1, p.SPS, p.mg_sps));
+        const int n_last = min(p.B - 1, fast_div(tile_s0 + TC_TILE - 1, p.SPS, p.mg_sps));
         const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
         {
               mbar_wait(&bars[LB_PART + pb], (uint32_t)((i >> 1) & 1));
@@ -460,7 +482,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
               for (int k_ = lane; k_ < ns; k_ += 32) {
                 const int n = n_first + k_;
                 const int a = n * p.SPS, bb = a + p.SPS - 1;
-                const int ta = a / q.TS, tbk = bb / q.TS;
+                const int ta = a / TC_TILE, tbk = bb / TC_TILE;
                 const unsigned expected = (unsigned)(tbk - ta + 1);
                 __threadfence();
                 if (atomicAdd(p.counter + n, 1u) == expected - 1u) {
@@ -470,7 +492,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                   for (int c = 0; c < cred; ++c) {
                     float tot = 0.f;
                     for (int tt = ta; tt <= tbk; ++tt) {
-                      const int nf = fast_div(tt * q.TS, p.SPS, p.mg_sps);
+                      const int nf = fast_div(tt * TC_TILE, p.SPS, p.mg_sps);
                       tot += __ldcg(p.tilepart + ((size_t)tt * p.MAXS + (n - nf)) * cred + c);
                     }
                     if (LAY && p.bc_out) p.bc_out[(size_t)n * p.C + c] = tot;
@@ -484,15 +506,15 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
         if (lane == 0) mbar_arrive(&bars[LB_PART_EMPTY + pb]);
       }
     } else if (warp >= LY_WIN_WARP0 && !q.in_mode) {
-      // ===================== window builders: tile i's z window once the MMAs have read tile i - 1's ================
+      // ===================== window builders: window w once the MMAs have read window w - 1 ================
       // four items per lane in flight at 80 registers, two at 64
-      for (int i = 0; i < n_my; ++i) {
-        if (i >= 1) mbar_wait(&bars[LB_WIN_EMPTY], (uint32_t)((i - 1) & 1));
-        // every claim on the other counter (tile i - 1's) was made before its window was handed over: reset it for
-        // tile i + 1, whose builders start only after this warp's arrival on tile i's window
-        if (warp == LY_WIN_WARP0 && lane == 0) s_win_next[(i + 1) & 1] = 0;
-        build_window(i, std::integral_constant<int, (REGS_AUX >= 80 ? 4 : 2)>{});
-        if (warp == LY_WIN_WARP0 && lane == 0) TL(3, 10, i);
+      for (int w = 0; w < n_my + W0; ++w) {
+        if (w >= 1) mbar_wait(&bars[LB_WIN_EMPTY], (uint32_t)((w - 1) & 1));
+        // every claim on the other counter (window w - 1's) was made before that window was handed over: reset it for
+        // window w + 1, whose builders start only after this warp's arrival on window w
+        if (warp == LY_WIN_WARP0 && lane == 0) s_win_next[(w + 1) & 1] = 0;
+        build_window(w, std::integral_constant<int, (REGS_AUX >= 80 ? 4 : 2)>{});
+        if (warp == LY_WIN_WARP0 && lane == 0) TL(3, 10, w);
       }
     }
     // otherwise (operand-image stages, or no per-sample outputs) the warp waits at the closing barrier
@@ -501,8 +523,20 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_MMA));
     float acc[(SPLIT ? 2 : 1) * 8 * SPG];  // SPLIT: room for the correction sum (ly_mma_tile)
     const bool tl0 = warp == 0 && lane == 0;
+    if (FUSED) {
+      // the run's halo block: warpgroup 0's hidden rows [0, 64) of window 0 hold rows [0, MIR) of the run's first tile.
+      // Warpgroup 1 runs the same K-steps on rows nobody reads: a trip count that differs between the warpgroups makes
+      // ptxas serialize every wgmma of the kernel
+      mbar_wait(&bars[LB_WIN_FULL], 0u);
+      mma_bar_sync();
+      ly_mma_tile<SPG, SPLIT>(acc, bars, St0.N, 0, q.n_bchunks, false, 1, 0, LB_BFULL,
+                              smem_u32(smem + q.sm_b), (uint32_t)q.b_chunk_bytes, (uint32_t)(q.b_chunk_bytes / 2), false,
+                              smem_u32(smem + q.sm_a), (uint32_t)a_plane, (uint32_t)a_lo_off, p.Wp, LB_WIN_EMPTY);
+      if (tl0) TL(0, 12, 0);
+      ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St0.N, 0, 0, true, true);
+    }
     for (int i = 0; i < n_my; ++i) {
-      if (!q.in_mode) mbar_wait(&bars[LB_WIN_FULL], (uint32_t)(i & 1));
+      if (!q.in_mode) mbar_wait(&bars[LB_WIN_FULL], (uint32_t)((i + W0) & 1));
       mma_bar_sync();
       if (tl0) TL(0, 15, i);
 #pragma unroll 1
@@ -513,8 +547,8 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                                 (uint32_t)(q.b_chunk_bytes / 2), q.in_mode != 0, smem_u32(smem + q.sm_a), (uint32_t)a_plane,
                                 (uint32_t)a_lo_off, p.Wp, (q.in_mode || ps + 1 < NP) ? -1 : (int)LB_WIN_EMPTY);
         if (tl0 && ps + 1 == NP) TL(0, 20, i);
-        ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St0.N, 16 * SPG * ps, FUSED ? 2 * i : i,
-                          ps == 0, ps + 1 == NP);
+        ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St0.N, 16 * SPG * ps,
+                          FUSED ? 2 * i + 1 : i, ps == 0, ps + 1 == NP);
       }
       if (tl0) TL(0, 21, i);
       if (FUSED) {
@@ -530,7 +564,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                                 false, smem_u32(smem + q.sm_h), (uint32_t)h_plane, (uint32_t)((St1.cin >> 3) * h_plane),
                                 p.Wp, LB_H_EMPTY, LB_H_FULL, (uint32_t)(i & 1));
         if (tl0) TL(0, 40, i);
-        ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St1.N, 0, 2 * i + 1, true, true);
+        ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St1.N, 0, 2 * i + 2, true, true);
         if (tl0) TL(0, 41, i);
       }
     }
@@ -569,22 +603,22 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       if (lane == 0) mbar_arrive(&bars[LB_ACC_EMPTY]);
     };
 
-    // the epilogue warps' share of tile i's window (which they start once the MMAs have read tile i - 1's)
-    auto help_window = [&](int i) {
-      if (i >= 1) mbar_wait(&bars[LB_WIN_EMPTY], (uint32_t)((i - 1) & 1));
-      build_window(i, std::integral_constant<int, 2>{});
-      if (ew == 0 && lane == 0) TL(1, 10, i);
+    // the epilogue warps' share of window w (which they start once the MMAs have read window w - 1)
+    auto help_window = [&](int w) {
+      if (w >= 1) mbar_wait(&bars[LB_WIN_EMPTY], (uint32_t)((w - 1) & 1));
+      build_window(w, std::integral_constant<int, 2>{});
+      if (ew == 0 && lane == 0) TL(1, 10, w);
     };
     if (!q.in_mode) help_window(0);
 
     for (int i = 0; i < n_my; ++i) {
-      const int u = (int)blockIdx.x + i * (int)gridDim.x;
+      const int u = tile_of(i);
       // per stage: help with the next tile's window before this tile's epilogue, which then runs under its MMAs
       if (!FUSED && !q.in_mode && i + 1 < n_my) help_window(i + 1);
-      const SlotInfo si_all = decode_slot(p, u * q.TS + sl, HW);
-      const bool bx0 = (si_all.x == 0), bxW = (si_all.x == p.W - 1), byH = (si_all.y == p.H - 1);
-      // the accumulator tile's uses: one per tile, or (fused) 2i for the hidden stage and 2i + 1 for the heads.  Each
-      // epilogue issues its first input loads (context, z), which do not depend on the MMAs, before waiting on it
+      const SlotInfo si_all = decode_slot(p, u * TC_TILE + sl, HW);
+      // the accumulator tile's uses: one per tile, or (fused) 0 for the run's halo block, then 2i + 1 for the hidden
+      // stage and 2i + 2 for the heads.  Each epilogue issues its first input loads (context, z), which do not depend on
+      // the MMAs, before waiting on it
       auto acc_wait = [&](uint32_t parity, int tag) {
         mbar_wait(&bars[LB_ACC_FULL], parity);
         if (ew == 0 && lane == 0) TL(1, tag, i);
@@ -594,14 +628,22 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       // covers slots [32 qd, +32).  Fused: two threads per slot, channels [8 cg, +8) of each 16-channel group, all eight
       // warps on one group at a time, so that the buffer goes to the heads MMAs chunk by chunk, the first after an
       // ngroups-th of the epilogue.  Per stage: one thread per slot and 16 channels, groups cg, cg + 2, ...  Every
-      // element is computed the same way under either mapping.
+      // element is computed the same way under either mapping.  Fused, the rows go to buffer rows [row0, +TC_TILE);
+      // the halo block's epilogue keeps rows [0, MIR) and hands nothing over (tile 0's chunk handoffs cover its rows).
       constexpr int HC = FUSED ? 8 : 16;  // channels per thread and group
       auto hidden_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch, const SlotInfo si,
-                            uint32_t acc_parity) {
+                            uint32_t acc_parity, const int row0, const bool halo) {
+        const bool bx0 = (si.x == 0), bxW = (si.x == p.W - 1), byH = (si.y == p.H - 1);
+        // store_row: the halo block writes buffer rows [0, MIR) only (its later rows are the first tile's own).
+        // keep_row: every slot's fp32 activations (hid_out) are written once.  The halo block keeps its rows [0, MIR); a
+        // fused tile keeps its last MIR rows, the next tile's first, only when the next tile is in its run (otherwise the
+        // next run's halo block keeps them)
+        const bool store_row = !halo || sl < p.MIR;
+        const bool keep_row = halo ? sl < p.MIR : (!FUSED || sl + p.MIR < TC_TILE || i + 1 < n_my);
         auto store_operand = [&](const float* v8, int chunk) {
           if (FUSED) {
-            uint8_t* dst = smem + q.sm_h + chunk * h_plane + sl * 16;
-            split_store8(v8, dst, dst + (St.N >> 3) * h_plane);
+            uint8_t* dst = smem + q.sm_h + chunk * h_plane + (row0 + sl) * 16;
+            if (store_row) split_store8(v8, dst, dst + (St.N >> 3) * h_plane);
           } else {
             const size_t go = ((size_t)chunk * q.S_pad + (size_t)u * TC_TILE + sl) * 8;
             split_store8(v8, reinterpret_cast<uint8_t*>(q.o_hi + go), reinterpret_cast<uint8_t*>(q.o_lo + go));
@@ -621,9 +663,19 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             }
           };
           fetch_ctx(g0);
-          // fused: refill the buffer once the heads MMAs of tile i - 1 have read it
-          if (FUSED && i >= 1) mbar_wait(&bars[LB_H_EMPTY], (uint32_t)((i - 1) & 1));
-          acc_wait(acc_parity, 25);
+          if (FUSED && !halo && i >= 1) {
+            // fused: refill the buffer once the heads MMAs of tile i - 1 have read it, first carrying its rows
+            // [TC_TILE, TC_TILE + MIR) to the front (every plane), all of them read before any warp overwrites them
+            mbar_wait(&bars[LB_H_EMPTY], (uint32_t)((i - 1) & 1));
+            for (int k = et; k < 2 * (St.N >> 3) * p.MIR; k += LY_ETHREADS) {
+              const int pl = k / p.MIR, rw = k - pl * p.MIR;
+              uint4* rows = reinterpret_cast<uint4*>(smem + q.sm_h + pl * h_plane);
+              rows[rw] = rows[TC_TILE + rw];
+            }
+            epi_bar_sync();
+            if (ew == 0 && lane == 0) TL(1, 24, i);
+          }
+          acc_wait(acc_parity, halo ? 13 : 25);
           for (int g = g0; g < ngroups; g += gs) {
             const int c0 = g * 16 + co;  // this thread's HC columns
             float cx[HC];
@@ -646,7 +698,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                 const float d = (q.bwd == 1) ? dg_nl_grad(cx[e], p.nl) : 1.0f;
                 vb[e] = si.valid ? a * d : 0.f;
               }
-              if (St.hid_out && si.valid && sl < q.TO && u < p.NT) {
+              if (St.hid_out && si.valid && keep_row) {
                 float* hp = St.hid_out + ((size_t)si.n * St.N + c0) * HW + si.gp;
                 if (q.bwd == 2) {
   #pragma unroll
@@ -656,7 +708,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                   for (int e = 0; e < HC; ++e) hp[(size_t)e * HW] = vb[e] * inv;
                 }
               }
-              if (u < p.NT && q.o_hi) {
+              if (q.o_hi) {
   #pragma unroll
                 for (int hch = 0; hch < HC / 8; ++hch) store_operand(vb + 8 * hch, (c0 >> 3) + hch);
               }
@@ -696,17 +748,15 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                 v[e] = si.valid ? o : 0.f;
               }
             }
-            if (St.hid_out && si.valid && sl < q.TO && u < p.NT) {  // training forward: keep the activations for iaf_step_bwd_saved
+            if (St.hid_out && si.valid && keep_row) {  // training forward: keep the activations for iaf_step_bwd_saved
               float* hp = St.hid_out + ((size_t)si.n * St.N + c0) * HW + si.gp;
   #pragma unroll
               for (int e = 0; e < HC; ++e) hp[(size_t)e * HW] = v[e];
             }
-            if (u < p.NT) {
   #pragma unroll
-              for (int hch = 0; hch < HC / 8; ++hch) store_operand(v + 8 * hch, (c0 >> 3) + hch);
+            for (int hch = 0; hch < HC / 8; ++hch) store_operand(v + 8 * hch, (c0 >> 3) + hch);
             }
-            }
-            if (FUSED) {  // chunk g of the buffer (both of its planes, all slots) goes to the heads MMAs
+            if (FUSED && !halo) {  // chunk g of the buffer (both of its planes, all slots) goes to the heads MMAs
               fence_proxy_async();  // generic-proxy stores -> the heads' wgmma reads of the buffer
               __syncwarp();
               if (lane == 0) mbar_arrive(&bars[LB_H_FULL + g]);
@@ -728,9 +778,10 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
           // the current group's set while it is summed), so each partial adds the same terms in the same order as
           // one warp per set would
           float rs0 = 0.f, rs1 = 0.f;
-          const int tile_s0 = u * q.TS;
+          const bool bx0 = (si.x == 0), bxW = (si.x == p.W - 1), byH = (si.y == p.H - 1);
+          const int tile_s0 = u * TC_TILE;
           const int n_first = fast_div(tile_s0, p.SPS, p.mg_sps);
-          const int n_last = min(p.B - 1, fast_div(tile_s0 + q.TS - 1, p.SPS, p.mg_sps));
+          const int n_last = min(p.B - 1, fast_div(tile_s0 + TC_TILE - 1, p.SPS, p.mg_sps));
           const int ns = (tile_s0 < p.S) ? (n_last - n_first + 1) : 0;
           const int pb = i & 1;
           // z of the NEXT column group is fetched while the current one is computed, the first before the accumulator
@@ -851,22 +902,29 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
 
       const float* tb0 = reinterpret_cast<const float*>(smem + q.sm_bias);
       if (FUSED) {
+        if (i == 0) {
+          // the first tile's window (once the halo block's MMAs have read theirs), then the halo block's epilogue under
+          // the first tile's hidden MMAs: rows [0, MIR) of the buffer
+          help_window(1);
+          hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, 0u, 0, true);
+          acc_release();
+          if (ew == 0 && lane == 0) TL(1, 14, i);
+        }
         // the hidden epilogue runs under the heads MMAs of its earlier chunks, the heads epilogue under the next tile's
         // hidden MMAs
-        hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, 0u);
+        hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), decode_slot(p, u * TC_TILE + p.MIR + sl, HW), 1u, p.MIR,
+                   false);
         acc_release();
         if (ew == 0 && lane == 0) TL(1, 30, i);
         // under the heads MMAs: the rest of the next tile's window, beside the builder warps
-        if (i + 1 < n_my) help_window(i + 1);
+        if (i + 1 < n_my) help_window(i + 2);
         const IafTcStage& St1 = p.st[1];
-        SlotInfo si_out = si_all;
-        si_out.valid = si_all.valid && sl < q.TO;
-        heads_epi(St1, reinterpret_cast<const float*>(smem + q.sm_bias1), St1.N >> 4, ly_acc_pitch(St1.N), si_out, 1u,
+        heads_epi(St1, reinterpret_cast<const float*>(smem + q.sm_bias1), St1.N >> 4, ly_acc_pitch(St1.N), si_all, 0u,
                   45);
         acc_release();
         if (ew == 0 && lane == 0) TL(1, 50, i);
       } else {
-        if (!q.is_heads) hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, (uint32_t)(i & 1));
+        if (!q.is_heads) hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, (uint32_t)(i & 1), 0, false);
         else heads_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, (uint32_t)(i & 1), 25);
         acc_release();
         if (ew == 0 && lane == 0) TL(1, 30, i);

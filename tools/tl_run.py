@@ -24,7 +24,9 @@ from bench import make_workload  # noqa: E402
 
 PHASE = {15: "MMA operands ready", 20: "MMAs done", 21: "acc tile written", 35: "heads operands ready",
          40: "heads MMAs done", 41: "heads acc written", 10: "window built", 25: "acc ready", 30: "(hidden) epilogue done",
-         45: "heads acc ready", 50: "heads epilogue done", 99: "end"}
+         45: "heads acc ready", 50: "heads epilogue done", 99: "end",
+         # one launch: the run's halo block (before its first tile) and the carry of each later tile's first MIR rows
+         12: "halo MMAs done", 13: "halo acc ready", 14: "halo epilogue done", 24: "carry done"}
 PHASE.update({26 + c: "hidden chunk %d ready" % c for c in range(4)})
 ROLE = {0: "MMA warpgroups", 1: "epilogue warps", 3: "window builders"}
 
@@ -64,6 +66,12 @@ def run(name, stage):
         print("%9d  role%d  %-24s k=%d" % (t, role, PHASE.get(tag, {60: "ring wait", 61: "ring released"}.get(tag, tag)), k))
     # tile period: from one tile's heads accumulators written to the next's, on the MMA side
     ends = [t for t, role, tag, _ in ev if role == 0 and tag == 41]
+    tiles = [k for _, role, tag, k in ev if role == 1 and tag == 99]
+    if tiles:
+        print("--- CTA 0 ran %d tiles ---" % tiles[0])
+    if ends:
+        # the run's first tile, halo block included: from the first event (the first window) to its heads accumulators
+        print("--- first tile (MMA side, from the first event): %d cycles ---" % (ends[0] - ev[0][0]))
     if len(ends) > 1:
         print("--- tile period (MMA side): %s cycles ---" % " ".join(str(b - a) for a, b in zip(ends, ends[1:])))
     # phase cycles per role: its events are phase ends, in order; each phase lasts from the previous event to its own.
