@@ -71,6 +71,8 @@ SYMBOLS = {
     "iaf_step_inverse_adjoint": (C.c_int, [_P, _P, _P, C.POINTER(_P), _P, _P, _P, _P, C.c_int, _P]),
     "iaf_adamax_step": (C.c_int, [C.c_int, C.POINTER(AdamaxTensor), C.c_int, _P, _P, _P, C.c_double, C.c_double,
                                   C.c_double, C.c_double, C.c_float, _P]),
+    "iaf_eve_step": (C.c_int, [C.POINTER(AdamaxTensor), C.c_int, _P, _P, _P, _P, _P, C.c_double, C.c_double,
+                               C.c_double, C.c_double, C.c_float, _P]),
     "iaf_adamax_launch_count": (C.c_uint64, []),
     "iaf_strerror": (C.c_char_p, [C.c_int]),
     "iaf_last_cuda_error": (C.c_char_p, []),

@@ -42,7 +42,7 @@ long long centre_nnz(int cin, int cout, int zd, int flipmask) {
 int iaf_record_cuda_error(cudaError_t e, const char* what) { return cuda_fail(e, what); }
 
 IafInvKernel iaf_inv = {nullptr, nullptr, nullptr};  // (filled in by iaf_inv.cu)
-IafAdamaxKernel iaf_adamax = {nullptr};             // (filled in by iaf_optim.cu)
+IafAdamaxKernel iaf_adamax = {nullptr, nullptr};    // (filled in by iaf_optim.cu)
 
 struct iaf_plan {
   iaf_desc_t d;
@@ -333,6 +333,32 @@ int iaf_adamax_step(int rule, const iaf_adamax_tensor_t* tensors_host, int n_ten
   uint64_t launches = 0;
   const int st = iaf_adamax.launch(rule, tensors_host, n_tensors, mom1, mom_max, avg, lr, beta1, beta2, avg_decay,
                                    grad_scale, stream, &launches);
+  g_adamax_launches.fetch_add(launches);
+  return st;
+}
+
+// The fused Eve step (iaf_optim.cu), checked the same way, and counted with the Adamax launches.
+int iaf_eve_step(const iaf_adamax_tensor_t* tensors_host, int n_tensors, float* mom1, float* mom_max, float* delta,
+                 float* avg, float* lookahead, double lr, double beta1, double beta2, double beta3, float grad_scale,
+                 void* stream) {
+  if (n_tensors < 0 || !std::isfinite(lr) || !std::isfinite(beta1) || !std::isfinite(beta2) ||
+      !std::isfinite(beta3) || !std::isfinite(grad_scale) || beta1 == 0.0)
+    return IAF_ERR_BAD_ARG;
+  if (n_tensors == 0) return IAF_OK;
+  float* const state[] = {mom1, mom_max, delta, avg, lookahead};
+  if (!tensors_host) return IAF_ERR_BAD_ARG;
+  for (float* s : state)
+    if (!s || ((uintptr_t)s & 3)) return IAF_ERR_BAD_ARG;
+  for (int i = 0; i < n_tensors; ++i) {
+    const iaf_adamax_tensor_t& t = tensors_host[i];
+    if (!t.param || t.numel < 1 || t.numel > ((int64_t)0x7fffffff << 12) || t.offset < 0 ||
+        ((uintptr_t)t.param & 3) || ((uintptr_t)t.grad & 3))
+      return IAF_ERR_BAD_ARG;
+  }
+  if (!iaf_adamax.launch_eve) return IAF_ERR_UNSUPPORTED;
+  uint64_t launches = 0;
+  const int st = iaf_adamax.launch_eve(tensors_host, n_tensors, mom1, mom_max, delta, avg, lookahead, lr, beta1, beta2,
+                                       beta3, grad_scale, stream, &launches);
   g_adamax_launches.fetch_add(launches);
   return st;
 }

@@ -268,12 +268,15 @@ struct IafInvKernel {
   cudaError_t (*launch_adj)(const IafInvAdjParams& p, int B, size_t smem_bytes, cudaStream_t stream);
 };
 extern IafInvKernel iaf_inv;
-// The fused Adamax step's launcher (iaf_optim.cu), registered the same way: without iaf_optim.cu linked in,
-// iaf_adamax_step validates its arguments and then refuses with IAF_ERR_UNSUPPORTED.
+// The fused Adamax and Eve steps' launchers (iaf_optim.cu), registered the same way: without iaf_optim.cu linked in,
+// iaf_adamax_step and iaf_eve_step validate their arguments and then refuse with IAF_ERR_UNSUPPORTED.
 struct IafAdamaxKernel {
   int (*launch)(int rule, const iaf_adamax_tensor_t* tensors_host, int n_tensors, float* mom1, float* mom_max,
                 float* avg, double lr, double beta1, double beta2, double avg_decay, float grad_scale, void* stream,
                 uint64_t* launches);
+  int (*launch_eve)(const iaf_adamax_tensor_t* tensors_host, int n_tensors, float* mom1, float* mom_max, float* delta,
+                    float* avg, float* lookahead, double lr, double beta1, double beta2, double beta3, float grad_scale,
+                    void* stream, uint64_t* launches);
 };
 extern IafAdamaxKernel iaf_adamax;
 // Record a failed CUDA call for iaf_last_cuda_error() and return IAF_ERR_CUDA (iaf_capi.cu).

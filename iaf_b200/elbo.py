@@ -508,7 +508,10 @@ def train_step(params, x_uint8, opt, hps, noise=None, iaf_layer=None, sharded=Fa
     ``iaf_layer``: default ``CudaIAFTrain(params, hps)``, built per call -- pass one to keep its operators across steps.
     ``noise[(i, j)]``: the posterior's N(0, 1) draw of the global batch (default: torch.randn on the parameters' device).
     ``sharded=True`` (or a ``group``): this rank is one tower of the reference's ``num_gpus`` and takes its contiguous
-    slice of the batch; the towers' gradients are averaged before the step.  Returns the step's bits/dim (a tensor)."""
+    slice of the batch; the towers' gradients are averaged before the step.  Returns the step's bits/dim (a tensor).
+    An optimiser with ``lookahead()`` (Eve) is refused: the TF reference has none."""
+    if hasattr(opt, "lookahead"):
+        raise ValueError("elbo.train_step: the TF model trains with Adamax only (Eve is the Theano model's optim='eve')")
     if iaf_layer is None:
         iaf_layer = CudaIAFTrain(params, hps)
     if noise is None:

@@ -406,26 +406,61 @@ def log_likelihood(w, x_uint8, iaf_layer, hps, k, chunk=None, noise=None, seed=0
 
 
 def train_step(w, x_uint8, opt, hps, noise=None, iaf_layer=None, sharded=False, group=None):
-    """One training step of the Theano model, ``f_train`` (models.py:563-569): the gradient of ``cost.sum()``
-    (optim.py:102) over the batch, then ``opt.step()``.  ``w``: leaf tensors with requires_grad (fp32 CUDA for
-    :class:`iaf_b200.optim.Adamax`, ``rule="theano"``); ``opt`` updates them in place.  ``iaf_layer``: default
-    ``CudaIAFTrain(w, hps)``, built per call -- pass one to keep its operators across steps.  ``noise[(i, j)]``: the
-    N(0, 1) draw of layer (i, j) for the global batch (default: torch.randn on the parameters' device).  ``sharded=True``
-    (or a ``group``): this rank takes its contiguous slice of the batch and the ranks' gradients are averaged before the
-    step, as :func:`iaf_b200.elbo.train_step`.  Returns the step's bits/dim (a tensor)."""
+    """One training step of the Theano model, ``f_train`` (models.py:563-573), then ``opt.step()``.  ``w``: leaf tensors
+    (fp32 CUDA for :mod:`iaf_b200.optim`); ``opt`` updates them in place.  ``noise[(i, j)]``: the N(0, 1) draw of layer
+    (i, j) for the global batch (default: torch.randn on the parameters' device).  ``sharded=True`` (or a ``group``):
+    this rank takes its contiguous slice of the batch and the ranks' gradients are averaged before the step, as
+    :func:`iaf_b200.elbo.train_step`.  Returns the step's bits/dim (a tensor).
+
+    * ``optim='adamax'`` (:class:`iaf_b200.optim.Adamax`, ``rule="theano"``): the gradient of ``cost.sum()``
+      (optim.py:102) at ``w``, which must require grad.  ``iaf_layer``: default ``CudaIAFTrain(w, hps)``, built per call
+      -- pass one to keep its operators across steps.
+    * ``optim='eve'`` (an ``opt`` with ``lookahead()``, :class:`iaf_b200.optim.Eve`): the gradient of the global batch's
+      MEAN cost (optim.py:138) at ``opt.lookahead()``, where the forward runs; the bits/dim returned are those at the
+      lookahead, what the reference's ``f_train`` returns.  Sharded, each rank's objective is its cost sum times
+      world / B, so the ranks' average is the global mean for any shard sizes.  ``iaf_layer``: default
+      ``CudaIAFTrain(opt.lookahead(), hps)``; a layer bound to other tensors is refused."""
+    import torch.distributed as dist
     from .elbo import run_train_step
+    lookahead = getattr(opt, "lookahead", None)
+    wf = w if lookahead is None else lookahead()
     if iaf_layer is None:
-        iaf_layer = CudaIAFTrain(w, hps)
-    S = hps["image_size"]
+        iaf_layer = CudaIAFTrain(wf, hps)
+    elif lookahead is not None:
+        bound = getattr(iaf_layer, "w", None)
+        if bound is None or any(bound.get(k) is not v for k, v in wf.items()):
+            raise ValueError("train_step: with Eve the iaf_layer must be bound to opt.lookahead(), where the gradient "
+                             "is taken")
+    S, B = hps["image_size"], x_uint8.shape[0]
     if noise is None:
-        h, B = w["h_top"], x_uint8.shape[0]
+        h = w["h_top"]
         noise = {(i, j): torch.randn((B, hps["n_z"], S // 2 ** (i + 1), S // 2 ** (i + 1)), device=h.device, dtype=h.dtype)
                  for i in range(len(hps["depths"])) for j in range(hps["depths"][i])}
+    world = 1
+    if (sharded or group is not None) and dist.is_initialized():
+        world = dist.get_world_size(group)
 
     def objective(x, nz):
-        out = forward(w, x, nz, iaf_layer, hps)
-        return out["cost"].sum(), out["bits_per_dim"]
-    return run_train_step(w, x_uint8, opt, noise, objective, 1.0, sharded, group)
+        out = forward(wf, x, nz, iaf_layer, hps)
+        obj = out["cost"].sum()
+        if lookahead is not None:
+            obj = obj * (world / B)  # the towers' average of these is the global batch's mean cost
+        return obj, out["bits_per_dim"]
+    return run_train_step(wf, x_uint8, opt, noise, objective, 1.0, sharded, group)
+
+
+def make_optimizer(w, hps):
+    """cvae1's optimiser (models.py:563-573) over ``w``: ``hps.get("optim", "adamax")`` selects
+    ``Adamax(w, rule="theano")`` or ``Eve(w)``; ``alpha``, ``beta1`` and ``beta2`` in ``hps`` (cvae1's argument names;
+    alpha is the learning rate) override the defaults."""
+    from .optim import Adamax, Eve
+    name = hps.get("optim", "adamax")
+    hp = dict(lr=hps.get("alpha"), beta1=hps.get("beta1"), beta2=hps.get("beta2"))
+    if name == "adamax":
+        return Adamax(w, rule="theano", **hp)
+    if name == "eve":
+        return Eve(w, **hp)
+    raise ValueError("make_optimizer: unknown optim %r (the reference has 'adamax' and 'eve')" % (name,))
 
 
 def make_params(hps, seed=0, dtype=np.float32):

@@ -309,7 +309,30 @@ typedef struct iaf_adamax_tensor {
 int iaf_adamax_step(int rule, const iaf_adamax_tensor_t* tensors_host, int n_tensors, float* mom1, float* mom_max,
                     float* avg, double lr, double beta1, double beta2, double avg_decay, float grad_scale,
                     void* stream);
-uint64_t iaf_adamax_launch_count(void); /* kernels launched by iaf_adamax_step in this process so far */
+
+/*
+ * The reference's Eve update and weight average, graphy/misc/optim.py:125-146 called with alpha = -lr
+ * (models.py:570-572), over a whole parameter set in one fused kernel (iaf_optim.cu).  Eve takes the gradient of the
+ * batch's MEAN cost at the lookahead point w' = w + c delta, c = (1 - b1) / b1, not at w.  With g = grad_scale * grad,
+ * grad taken at w', and every right-hand side reading the values from before the step:
+ *     avg = b3 w + (1 - b3) avg;  mom1 = (1 - b1) mom1 + b1 g;  max = max((1 - b2) max, |g| + 1e-8)
+ *     delta = ((-lr) mom1) / max;  w = w + delta;  lookahead = w + c delta   (w and delta after the update)
+ * The kernel writes the next step's lookahead, which is what the reference recomputes from w and delta at its next
+ * call.  Constants are python floats rounded to fp32 as Theano does: each expression (1 - b1, (1 - b1) / b1, ...) in
+ * double, then cast.  Every operation is one correctly rounded fp32 operation in the order above (no FMA contraction),
+ * so results are bit-identical to an op-by-op fp32 restatement.  A NULL grad is a zero gradient
+ * (disconnected_inputs='ignore').  Reference defaults: lr 0.002, b1 0.1, b2 0.001, b3 0.01.
+ * tensors_host[i].param is w and .grad the gradient at w'.  State: five fp32 buffers owned by the caller, entry i's
+ * slice at [offset, offset + numel): mom1, mom_max, delta, avg and lookahead.  Start them at 0, 1e-8, 0, and the
+ * parameters' values for both avg and lookahead.  The previous delta is not read.
+ * beta1 == 0 is refused (c would be infinite).  Allocates nothing, copies nothing to the device and does not
+ * synchronise (capture-safe); tables are chunked into launches as for iaf_adamax_step; n_tensors == 0 launches nothing.
+ */
+int iaf_eve_step(const iaf_adamax_tensor_t* tensors_host, int n_tensors, float* mom1, float* mom_max, float* delta,
+                 float* avg, float* lookahead, double lr, double beta1, double beta2, double beta3, float grad_scale,
+                 void* stream);
+/* kernels launched by iaf_adamax_step and iaf_eve_step in this process so far */
+uint64_t iaf_adamax_launch_count(void);
 
 /* introspection */
 const char* iaf_strerror(int status);
