@@ -25,6 +25,7 @@
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <climits>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -100,6 +101,37 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// CTA clusters (distributed shared memory): the shared::cluster address of `p` in the cluster's CTA `rank`, a 16-byte
+// store there, a proxy fence that covers it, a release arrive on a barrier there, and the acquiring wait that pairs with
+// such an arrive
+__device__ __forceinline__ uint32_t cluster_map(const void* p, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ void st_cluster16(uint32_t addr, const uint4& v) {
+  asm volatile("st.shared::cluster.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
+               : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async_cluster() { asm volatile("fence.proxy.async.shared::cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t addr) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(addr) : "memory");
+}
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "WAIT_%=:\n\t"
+      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
+      "@p bra DONE_%=;\n\t"
+      "bra WAIT_%=;\n\t"
+      "DONE_%=:\n\t}" ::"r"(smem_u32(bar)), "r"(parity)
+      : "memory");
+}
+// every thread of the cluster: the barrier also orders the CTA's own threads, as __syncthreads does.  Not .aligned:
+// the warps reach it from role branches that need not have reconverged
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
@@ -242,7 +274,7 @@ __device__ __forceinline__ float tc_apply_nl(float v, int nl) {
 // Range: |x| >= 65520 becomes inf and that sample's outputs NaN (loud, never silently wrong; invalid slots are zeroed by
 // a select, so the NaN stays inside its sample).  Activations are not scaled: below |x| ~ 2^-3 the lo half is subnormal
 // and x keeps an absolute resolution of about 2^-25 (3e-8) instead of 22 significant bits.
-__device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, uint8_t* lo_ptr) {
+__device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
   uint32_t h[4], l[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -252,35 +284,40 @@ __device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, ui
     h[i] = *reinterpret_cast<const uint32_t*>(&hh);
     l[i] = *reinterpret_cast<const uint32_t*>(&ll);
   }
-  *reinterpret_cast<uint4*>(hi_ptr) = make_uint4(h[0], h[1], h[2], h[3]);
-  *reinterpret_cast<uint4*>(lo_ptr) = make_uint4(l[0], l[1], l[2], l[3]);
+  hi = make_uint4(h[0], h[1], h[2], h[3]);
+  lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+__device__ __forceinline__ void split_store8(const float* v, uint8_t* hi_ptr, uint8_t* lo_ptr) {
+  split8(v, *reinterpret_cast<uint4*>(hi_ptr), *reinterpret_cast<uint4*>(lo_ptr));
 }
 
-// Optional in-kernel timeline (compile with -DIAF_TC_TIMELINE; development aid only, tools/tl_run.py): CTA 0 of the
-// launch that sets tl_enable records (tag, tile or chunk, clock) triples per role, each at the end of a phase of its own
-// warp (other warps of the role may still be in it).  Role 0, lane 0 of MMA warp 0: 15 / 35 the (hidden) / heads MMAs'
-// operands ready, 20 / 40 their MMAs done, 21 / 41 their fragments in the accumulator tile (after waiting for the
-// epilogues to free it), 12 the halo block's MMAs done (fused).  Role 1, lane 0 of epilogue warp 0: 25 / 45 (hidden) /
-// heads accumulators ready, 26 + c hidden chunk c written to the buffer (fused), 30 (hidden) epilogue done, 50 heads
-// epilogue done (fused), 13 / 14 the halo block's accumulators ready / epilogue done, 24 carry done (fused), 98 the
-// launch's mode (k = IAF_MODE_*: multiconv, step, layer, logp), 99 kernel end.  Role 2, the producer: 60 / 61 before
-// / after waiting for a ring stage to be released (k = the weight chunk it will refill).  Role 3, lane 0 of the first
-// window-builder warp: 10 z window built.
+// Optional in-kernel timeline (compile with -DIAF_TC_TIMELINE; development aid only, tools/tl_run.py): one CTA (0
+// unless iaf_tc_timeline_cta chose another) of the launch that sets tl_enable records (tag, tile or chunk, clock)
+// triples per role, each at the end of a phase of its own warp (other warps of the role may still be in it).  Role 0,
+// lane 0 of MMA warp 0: 15 / 35 the (hidden) / heads MMAs' operands ready, 20 / 40 their MMAs done, 21 / 41 their
+// fragments in the accumulator tile (after waiting for the epilogues to free it), 12 the halo block's MMAs done, 36 the
+// halo received from the pair's giver (fused).  Role 1, lane 0 of epilogue warp 0: 25 / 45 (hidden) / heads
+// accumulators ready, 26 + c hidden chunk c written to the buffer (fused), 30 (hidden) epilogue done, 50 heads epilogue
+// done (fused), 13 / 14 the halo block's accumulators ready / epilogue done, 16 the halo sent to the pair's receiver, 24
+// carry done (fused), 98 the launch's mode (k = IAF_MODE_*: multiconv, step, layer, logp), 99 kernel end.  Role 2, the
+// producer: 60 / 61 before / after waiting for a ring stage to be released (k = the weight chunk it will refill).  Role
+// 3, lane 0 of the first window-builder warp: 10 z window built.
 #ifdef IAF_TC_TIMELINE
 #define TL_MAX 96
 __device__ long long g_tl[4][TL_MAX][3];
 __device__ int g_tl_n[4];
+__device__ unsigned g_tl_cta;  // the CTA that records
 // events are staged in shared memory (a global counter would cost an L2 round trip per event)
 #define TL_DECL __shared__ long long s_tl[4][TL_MAX][3]; __shared__ int s_tl_n[4]; if (threadIdx.x < 4) s_tl_n[threadIdx.x] = 0;
 #define TL(role, tag, kk)                                                          \
   do {                                                                             \
-    if (blockIdx.x == 0) {                                                         \
+    if (blockIdx.x == g_tl_cta) {                                                  \
       const int i_ = s_tl_n[role];                                                 \
       if (i_ < TL_MAX) { s_tl[role][i_][0] = (tag); s_tl[role][i_][1] = (kk); s_tl[role][i_][2] = clock64(); s_tl_n[role] = i_ + 1; } \
     }                                                                              \
   } while (0)
 #define TL_FLUSH                                                                   \
-  if (blockIdx.x == 0 && threadIdx.x < 4) {                                        \
+  if (blockIdx.x == g_tl_cta && threadIdx.x < 4) {                                 \
     const int r_ = threadIdx.x;                                                    \
     for (int i_ = 0; i_ < s_tl_n[r_]; ++i_)                                        \
       for (int c_ = 0; c_ < 3; ++c_) g_tl[r_][i_][c_] = s_tl[r_][i_][c_];          \
@@ -431,6 +468,7 @@ struct IafTcPlan {
   bool fused;
   int fz_sm_a, fz_sm_h, fz_sm_bias[2], fz_sm_part, fz_sm_acc, fz_sm_b[2];
   size_t fz_smem;
+  int fz_clusters;           // clusters of two one-launch CTAs the device holds at once (0: none)
   __nv_bfloat16* img[2][2];  // ping-pong operand images: [which][hi|lo]
   int img_S_pad;
   unsigned* counter;
@@ -554,6 +592,23 @@ static bool fz_layout(const iaf_desc_t* d, IafTcPlan* q) {
   return off <= TC_SMEM_LIMIT;
 }
 
+// clusters of two CTAs of the one-launch kernel `k` that the device runs at once (0 if it cannot say)
+static int fz_max_clusters(LyKernel k, size_t smem) {
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(2); cfg.blockDim = dim3(LY_THREADS); cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, k, &cfg) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return 0;
+  }
+  return n;
+}
+
 bool iaf_tc_supported(const iaf_desc_t* d) { return ly_layout(d, nullptr); }
 
 int iaf_tc_plan_create(IafTcPlan** out, const iaf_desc_t* d) {
@@ -583,10 +638,14 @@ int iaf_tc_plan_create(IafTcPlan** out, const iaf_desc_t* d) {
     pl->padw[j] = pl->bias[j] + pl->N[j];
     pl->wsinv[j] = pl->bias[j] + 5 * pl->N[j];
   }
+  pl->fz_clusters = pl->fused ? INT_MAX : 0;
   for (int a = 0; a < 16; ++a) {
     const int md = a >> 2;  // IAF_MODE_MULTICONV .. IAF_MODE_LOGP
     cudaError_t e = cudaSuccess;
-    if (pl->fused) e = iaf_smem_optin(fz_kernel_for(a & 1, md, a & 2));
+    if (pl->fused) {
+      e = iaf_smem_optin(fz_kernel_for(a & 1, md, a & 2));
+      if (e == cudaSuccess) pl->fz_clusters = std::min(pl->fz_clusters, fz_max_clusters(fz_kernel_for(a & 1, md, a & 2), pl->fz_smem));
+    }
     for (int j = 0; j < pl->n_stages && e == cudaSuccess && !pl->fused; ++j) e = iaf_smem_optin(ly_kernel_for(a & 1, md, a & 2, pl->N[j]));
     if (e != cudaSuccess) {
       iaf_tc_plan_destroy(pl);
@@ -663,6 +722,11 @@ extern "C" void iaf_tc_timeline_dump(void) {
   int z[4] = {0, 0, 0, 0};
   cudaMemcpyToSymbol(g_tl_n, z, sizeof(z));
 }
+// the CTA whose timeline the next launches record
+extern "C" void iaf_tc_timeline_cta(int b) {
+  const unsigned u = (unsigned)b;
+  cudaMemcpyToSymbol(g_tl_cta, &u, sizeof(u));
+}
 #endif
 
 bool iaf_tc_mode_supported(const IafTcPlan* pl, int mode) {
@@ -733,17 +797,29 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
   p.mg_sps = (unsigned)((1ULL << 32) / (unsigned)SPS) + 1u;
   p.mg_wp = (unsigned)((1ULL << 32) / (unsigned)p.Wp) + 1u;
   p.mg_win = (unsigned)((1ULL << 32) / (unsigned)p.WIN) + 1u;
-  const int grid = std::min(pl->num_sms, NT);
+  int grid = std::min(pl->num_sms, NT);
   const bool padw = pl->vf.pad_channel, elu = d.nl == IAF_NL_ELU;
+  // the one-launch kernel runs in CTA pairs (fz_run) when the grid, with one CTA more if it is odd and below the SM
+  // cap, is even and the device holds all its clusters at once
+  bool paired = false;
+  if (pl->fused) {
+    const int g2 = grid + (grid & 1);
+    if (g2 <= pl->num_sms && g2 / 2 <= pl->fz_clusters) {
+      grid = g2;
+      paired = true;
+    }
+  }
   auto launch = [&](LyKernel lk, const IafLyParams& q, size_t smem) {
     const char* pe = getenv("IAF_PDL");
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(LY_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
+    cudaLaunchAttribute at[2];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = (pe && pe[0] == '0') ? 0 : 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
+    at[1].id = cudaLaunchAttributeClusterDimension;
+    at[1].val.clusterDim.x = q.paired ? 2 : 1; at[1].val.clusterDim.y = 1; at[1].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = q.paired ? 2 : 1;
     return cudaLaunchKernelEx(&cfg, lk, q) == cudaSuccess;
   };
   if (pl->fused) {
@@ -765,6 +841,7 @@ int iaf_tc_run(IafTcPlan* pl, const IafTcArgs* a, cudaStream_t stream, int* n_la
     q.b_chunk_bytes = ly_chunk_bytes(pl->N[0], pl->NS[0]); q.n_bchunks = (pl->K[0] / 16) / LY_KC;
     q.b_chunk_bytes1 = ly_chunk_bytes(pl->N[1], pl->NS[1]); q.n_bchunks1 = (pl->K[1] / 16) / LY_KC;
     q.stage_bytes = q.b_chunk_bytes;
+    q.paired = paired ? 1 : 0;
     q.tl_enable = 1;
     if (!launch(fz_kernel_for(padw, a->mode, elu), q, pl->fz_smem)) return IAF_ERR_CUDA;
     if (n_launches) *n_launches = 1;

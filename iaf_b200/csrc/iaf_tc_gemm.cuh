@@ -71,7 +71,10 @@ enum { LB_BFULL = 0, LB_BEMPTY = LY_MAX_NB, LB_PART = 2 * LY_MAX_NB,
        // fused kernel's hidden operand buffer (written by the epilogue warps, read by the MMA warpgroups): full per
        // 16-channel chunk c, LB_H_FULL + c, so that the heads MMAs of chunk c start once the epilogue has written it
        LB_ACC_FULL = 4 + 2 * LY_MAX_NB, LB_ACC_EMPTY, LB_WIN_FULL, LB_WIN_EMPTY, LB_H_EMPTY, LB_H_FULL,
-       LB_COUNT = LB_H_FULL + LY_H_CHUNKS };
+       // fused, CTA pairs: the receiver's hidden rows [0, MIR) of its first tile, written and arrived on by the giver's
+       // epilogue warps (fz_run)
+       LB_H_HALO = LB_H_FULL + LY_H_CHUNKS,
+       LB_COUNT };
 
 struct IafLyParams {
   IafTcParams t;               // geometry, pointers, slot decoding (t.st[0] describes THIS stage)
@@ -94,6 +97,7 @@ struct IafLyParams {
   int sm_h;                    // fused: the hidden operand buffer [chunk][TC_TILE + MIR][8] hi, then lo
   int sm_b1, sm_bias1;         // fused: the heads' resident weights and bias table
   int n_bchunks1, b_chunk_bytes1;
+  int paired;                  // fused: launched in clusters of two CTAs that share a halo (fz_run)
   // data-gradient use of a hidden stage (iaf_dg_run): the input image holds the gradient at this layer's output, scaled
   // per sample into fp16 range; weights are the transposed effective weights; t.ctx points at the activations h whose
   // nl' multiplies the result (bwd 1) or is null (bwd 2: gradient at the stack input, ACCUMULATED into hid_out)
@@ -255,14 +259,42 @@ __device__ __forceinline__ void ly_acc_store(const float* acc, uint64_t* bars, f
   if (lane == 0) mbar_arrive(&bars[LB_ACC_FULL]);
 }
 
+// The one-launch kernel's run of tiles for CTA b of a grid of G over NT tiles: `n` tiles from `first`, in descending
+// order if `desc`, and whether the run's first tile computes its halo rows itself (`halo`) or receives them.
+//   unpaired: CTA b runs [floor(b NT / G), floor((b + 1) NT / G)) upwards, each run with a halo block.
+//   paired (clusters of two CTAs, G even): cluster c of G / 2 covers [T0, T2) = [floor(c NT / (G / 2)),
+//   floor((c + 1) NT / (G / 2))), split at T1 = T0 + floor((T2 - T0) / 2).  Rank 0, the giver, runs [T0, T1) downwards
+//   from T1 - 1; rank 1, the receiver, runs [T1, T2) upwards, so the larger half of an odd split goes to the receiver,
+//   which then has no halo block on its critical path.  Both first tiles need the hidden rows of slots [TC_TILE T1,
+//   +MIR): the giver computes them in its halo block and also writes them into the receiver's buffer.  Where two
+//   clusters meet, both runs end and each last tile carries its rows from the tile before it.  A cluster of one tile
+//   has an empty lower run, and its receiver runs as an unpaired CTA.
+// 32-bit products: NT < 2^24 (tc_num_tiles) and G is at most the SM count.
+struct FzRun { int first, n, desc, halo; };
+__host__ __device__ inline FzRun fz_run(int b, int G, int NT, bool paired) {
+  if (!paired) {
+    const int a = (int)((uint32_t)b * (uint32_t)NT / (uint32_t)G), e = (int)((uint32_t)(b + 1) * (uint32_t)NT / (uint32_t)G);
+    return FzRun{a, e - a, 0, 1};
+  }
+  const uint32_t nc = (uint32_t)G / 2u, c = (uint32_t)b / 2u;
+  const int T0 = (int)(c * (uint32_t)NT / nc), T2 = (int)((c + 1u) * (uint32_t)NT / nc);
+  const int T1 = T0 + (T2 - T0) / 2;
+  if (T1 == T0) return (b & 1) ? FzRun{T1, T2 - T1, 0, 1} : FzRun{T0, 0, 0, 0};
+  return (b & 1) ? FzRun{T1, T2 - T1, 0, 0} : FzRun{T1 - 1, T1 - T0, 1, 1};
+}
+
 // NGW: ceil(N / 32); an MMA warpgroup covers the stage's columns as 2 NGW groups of 16.  Tile t covers slots
 // [TC_TILE t, +TC_TILE) in both kernels.  FUSED: the whole step of a one-hidden-layer stack in one launch (NGW covers
-// both stages).  Each CTA runs one contiguous run of tiles in ascending order.  Row j of the hidden buffer holds slot
-// TC_TILE t + j, j < TC_TILE + MIR, since the heads' taps read up to MIR rows ahead.  A tile's hidden MMAs compute rows
-// [MIR, TC_TILE + MIR) from a z window that starts MIR slots into the tile; rows [0, MIR) are the previous tile's rows
-// [TC_TILE, TC_TILE + MIR), carried to the front once its heads MMAs have released the buffer.  The run's first tile
-// gets them from a halo block: a hidden pass over a z window of its own at the tile's first slot, whose first 64 rows
-// (MIR <= 64, fz_layout) are kept.  A hidden row adds the same products in the same order whichever tile computes it.
+// both stages).  Each CTA runs one contiguous run of tiles (fz_run).  Row j of the hidden buffer holds slot
+// TC_TILE t + j, j < TC_TILE + MIR, since the heads' taps read up to MIR rows ahead.  Upwards, a tile's hidden MMAs
+// compute rows [MIR, TC_TILE + MIR) from a z window that starts MIR slots into the tile; rows [0, MIR) are the previous
+// tile's rows [TC_TILE, TC_TILE + MIR), carried to the front once its heads MMAs have released the buffer.  Downwards,
+// a tile computes rows [0, TC_TILE) from a window at its first slot, and rows [TC_TILE, TC_TILE + MIR) are the previous
+// tile's rows [0, MIR), carried to the back.  The run's first tile gets those rows from a halo block: a hidden pass
+// over a z window of its own at the first slot they hold, whose first 64 rows (MIR <= 64, fz_layout) are kept -- or,
+// for a pair's receiver, from its giver's halo block.  Both MMA warpgroups issue the same wgmma sequence either way;
+// the direction changes only window slots and buffer rows.  A hidden row adds the same products in the same order
+// whichever tile computes it.
 template <bool PADW, int MODE, int NLT, int NGW, bool FUSED>
 __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_constant__ IafLyParams q) {
   const IafTcParams& p = q.t;
@@ -277,18 +309,23 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   const int nchunk = St0.cin >> 3;
   const int a_plane = p.WIN * 16;          // bytes per chunk plane of the A window
   const int a_lo_off = nchunk * a_plane;
-  // tiles of this CTA, i = 0 .. n_my - 1: fused, the run [t0, t0 + n_my) (which tile covers which slots does not depend
-  // on the grid, only which CTA runs it); per stage, u = blockIdx.x + i * gridDim.x.  Both live in shared memory and
-  // are read where they are used: a register holding them through the whole kernel spilled at the launch's 96
-  __shared__ int s_run[2];
+  // tiles of this CTA, i = 0 .. n_my - 1: fused, the run of fz_run from t0, up or (desc) down (which tile covers which
+  // slots does not depend on the grid, only which CTA runs it); per stage, u = blockIdx.x + i * gridDim.x.  They live in
+  // shared memory and are read where they are used: a register holding them through the whole kernel spilled at the
+  // launch's 96
+  __shared__ int s_run[4];
   const int& t0 = s_run[0];
   const int& n_my = s_run[1];
-  auto tile_of = [&](int i) { return FUSED ? t0 + i : (int)blockIdx.x + i * (int)gridDim.x; };
-  // z windows, use w: fused, w = 0 is the halo block's (at the run's first slot) and w = i + 1 tile i's (MIR slots into
-  // the tile); per stage, w = i is tile i's
-  constexpr int W0 = FUSED ? 1 : 0;
+  // fused: whether the run goes down, and 1 if it has a halo block, which takes window and accumulator use 0 (per stage,
+  // 0 and 0)
+  auto desc = [&]() { return FUSED ? s_run[2] : 0; };
+  auto W0 = [&]() { return FUSED ? s_run[3] : 0; };
+  auto tile_of = [&](int i) { return FUSED ? (desc() ? t0 - i : t0 + i) : (int)blockIdx.x + i * (int)gridDim.x; };
+  // z windows, use w: fused, w = 0 the halo block's (if any; at the first slot of the rows it keeps) and w = i + W0
+  // tile i's (upwards MIR slots into the tile, downwards at its first slot); per stage, w = i is tile i's
   auto win_slot0 = [&](int w) {
-    return FUSED ? (w == 0 ? TC_TILE * t0 : TC_TILE * (t0 + w - 1) + p.MIR) : TC_TILE * tile_of(w);
+    if (!FUSED) return TC_TILE * tile_of(w);
+    return w < W0() ? TC_TILE * (t0 + desc()) : TC_TILE * tile_of(w - W0()) + (desc() ? 0 : p.MIR);
   };
   const bool resident = FUSED || q.n_bchunks <= q.NB;
   const bool ring = !resident || q.in_mode;
@@ -317,14 +354,17 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       mbar_init(&bars[LB_ACC_EMPTY], LY_EPI_WARPS);
       mbar_init(&bars[LB_WIN_FULL], LY_WIN_WARPS + LY_EPI_WARPS);
       s_win_next[0] = s_win_next[1] = 0;
-      // 32-bit products: NT < 2^24 (tc_num_tiles) and the grid is at most the SM count
-      const uint32_t b0 = FUSED ? blockIdx.x * (uint32_t)p.NT / gridDim.x : blockIdx.x;
-      s_run[0] = (int)b0;
-      s_run[1] = FUSED ? (int)((blockIdx.x + 1) * (uint32_t)p.NT / gridDim.x - b0)
-                       : (int)((uint32_t)(p.NT - (int)blockIdx.x + (int)gridDim.x - 1) / gridDim.x);
+      if (FUSED) {
+        const FzRun r = fz_run((int)blockIdx.x, (int)gridDim.x, p.NT, q.paired != 0);
+        s_run[0] = r.first; s_run[1] = r.n; s_run[2] = r.desc; s_run[3] = r.halo;
+      } else {
+        s_run[0] = (int)blockIdx.x;
+        s_run[1] = (int)((uint32_t)(p.NT - (int)blockIdx.x + (int)gridDim.x - 1) / gridDim.x);
+      }
       mbar_init(&bars[LB_WIN_EMPTY], 2);
       for (int c = 0; c < LY_H_CHUNKS; ++c) mbar_init(&bars[LB_H_FULL + c], LY_EPI_WARPS);
       mbar_init(&bars[LB_H_EMPTY], 2);
+      mbar_init(&bars[LB_H_HALO], LY_EPI_WARPS);  // every epilogue warp of the giver arrives
       fence_barrier_init();
     }
   } else if (epi) {
@@ -341,7 +381,9 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     }
   }
   if (!epi) asm volatile("griddepcontrol.wait;" ::: "memory");
-  __syncthreads();
+  // paired: the barrier also makes each CTA's initialised LB_H_HALO visible to the other before the giver arrives on it
+  if (FUSED && q.paired) cluster_sync();
+  else __syncthreads();
 
   // fp32 z (layer mode: post_mean + exp(post_logsd) z) -> the fp16 hi/lo A window of the CTA's w-th use (first stage).
   // Items are (chunk of 8 channels, window slot).  The builder warps and, once their hidden epilogue is done, the
@@ -398,8 +440,9 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       // ===================== producer: A windows (operand-image input) and the weight ring =====================
       if (lane == 0 && FUSED) {
         // both stages' weights, resident: hidden chunk c behind barrier c, heads chunk c behind barrier n_bchunks + c
+        // (none for an empty run, which must not exit with copies in flight)
         static_assert(!FUSED || SPLIT, "the one-launch kernel's images are [W_lo | W_hi] planes");
-        for (int s = 0; s < 2; ++s) {
+        for (int s = 0; s < (n_my > 0 ? 2 : 0); ++s) {
           const IafTcStage& S = p.st[s];
           const int nb = s ? q.n_bchunks1 : q.n_bchunks, bcb = s ? q.b_chunk_bytes1 : q.b_chunk_bytes;
           uint8_t* base = smem + (s ? q.sm_b1 : q.sm_b);
@@ -508,7 +551,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     } else if (warp >= LY_WIN_WARP0 && !q.in_mode) {
       // ===================== window builders: window w once the MMAs have read window w - 1 ================
       // four items per lane in flight at 80 registers, two at 64
-      for (int w = 0; w < n_my + W0; ++w) {
+      for (int w = 0; w < n_my + W0(); ++w) {
         if (w >= 1) mbar_wait(&bars[LB_WIN_EMPTY], (uint32_t)((w - 1) & 1));
         // every claim on the other counter (window w - 1's) was made before that window was handed over: reset it for
         // window w + 1, whose builders start only after this warp's arrival on window w
@@ -523,10 +566,10 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_MMA));
     float acc[(SPLIT ? 2 : 1) * 8 * SPG];  // SPLIT: room for the correction sum (ly_mma_tile)
     const bool tl0 = warp == 0 && lane == 0;
-    if (FUSED) {
-      // the run's halo block: warpgroup 0's hidden rows [0, 64) of window 0 hold rows [0, MIR) of the run's first tile.
-      // Warpgroup 1 runs the same K-steps on rows nobody reads: a trip count that differs between the warpgroups makes
-      // ptxas serialize every wgmma of the kernel
+    if (FUSED && W0()) {
+      // the run's halo block: warpgroup 0's hidden rows [0, 64) of window 0 hold the MIR halo rows of the run's first
+      // tile.  Warpgroup 1 runs the same K-steps on rows nobody reads: a trip count that differs between the
+      // warpgroups makes ptxas serialize every wgmma of the kernel
       mbar_wait(&bars[LB_WIN_FULL], 0u);
       mma_bar_sync();
       ly_mma_tile<SPG, SPLIT>(acc, bars, St0.N, 0, q.n_bchunks, false, 1, 0, LB_BFULL,
@@ -536,7 +579,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St0.N, 0, 0, true, true);
     }
     for (int i = 0; i < n_my; ++i) {
-      if (!q.in_mode) mbar_wait(&bars[LB_WIN_FULL], (uint32_t)((i + W0) & 1));
+      if (!q.in_mode) mbar_wait(&bars[LB_WIN_FULL], (uint32_t)((i + W0()) & 1));
       mma_bar_sync();
       if (tl0) TL(0, 15, i);
 #pragma unroll 1
@@ -548,12 +591,19 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                                 (uint32_t)a_lo_off, p.Wp, (q.in_mode || ps + 1 < NP) ? -1 : (int)LB_WIN_EMPTY);
         if (tl0 && ps + 1 == NP) TL(0, 20, i);
         ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St0.N, 16 * SPG * ps,
-                          FUSED ? 2 * i + 1 : i, ps == 0, ps + 1 == NP);
+                          FUSED ? 2 * i + W0() : i, ps == 0, ps + 1 == NP);
       }
       if (tl0) TL(0, 21, i);
       if (FUSED) {
         const IafTcStage& St1 = p.st[1];
         const int h_plane = (TC_TILE + p.MIR) * 16;
+        // a pair's receiver: its first tile's rows [0, MIR) come from the giver.  It touches none of them before these
+        // MMAs (its hidden epilogue writes rows [MIR, TC_TILE + MIR), the carry waits for these MMAs), so the giver
+        // needs no "empty" barrier to write them
+        if (!W0() && i == 0) {
+          mbar_wait_cluster(&bars[LB_H_HALO], 0u);
+          if (tl0) TL(0, 36, i);
+        }
         // heads weight chunk c reads hidden channels [16 c, +16): its MMAs start as soon as the epilogue has written
         // them, while it computes the later chunks
         mbar_wait(&bars[LB_H_FULL], (uint32_t)(i & 1));
@@ -564,7 +614,8 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
                                 false, smem_u32(smem + q.sm_h), (uint32_t)h_plane, (uint32_t)((St1.cin >> 3) * h_plane),
                                 p.Wp, LB_H_EMPTY, LB_H_FULL, (uint32_t)(i & 1));
         if (tl0) TL(0, 40, i);
-        ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St1.N, 0, 2 * i + 2, true, true);
+        ly_acc_store<SPG>(acc, bars, reinterpret_cast<float*>(smem + q.sm_acc), St1.N, 0, 2 * i + 1 + W0(), true,
+                          true);
         if (tl0) TL(0, 41, i);
       }
     }
@@ -577,10 +628,10 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     const int sl = qd * 32 + lane;
     float* s_part = reinterpret_cast<float*>(smem + q.sm_part);
     float* s_acc = reinterpret_cast<float*>(smem + q.sm_acc);
-    // this thread's slot row of the accumulator tile, 8 (16) columns from c0, times the columns' inverse weight scales
-    // (exact: powers of two; wsinv null = unscaled images, the data gradient's)
-    auto acc_ld8 = [&](int c0, uint32_t* r, int pitch, const float* wsinv) {
-      const float4* s4 = reinterpret_cast<const float4*>(s_acc + sl * pitch + c0);
+    // slot row `row` of the accumulator tile, 8 (16) columns from c0, times the columns' inverse weight scales (exact:
+    // powers of two; wsinv null = unscaled images, the data gradient's)
+    auto acc_ld8 = [&](int row, int c0, uint32_t* r, int pitch, const float* wsinv) {
+      const float4* s4 = reinterpret_cast<const float4*>(s_acc + row * pitch + c0);
 #pragma unroll
       for (int e4 = 0; e4 < 2; ++e4) {
         float4 v4 = s4[e4];
@@ -592,9 +643,9 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
         r[4 * e4 + 2] = __float_as_uint(v4.z); r[4 * e4 + 3] = __float_as_uint(v4.w);
       }
     };
-    auto acc_ld16 = [&](int c0, uint32_t* r, int pitch, const float* wsinv) {
-      acc_ld8(c0, r, pitch, wsinv);
-      acc_ld8(c0 + 8, r + 8, pitch, wsinv);
+    auto acc_ld16 = [&](int row, int c0, uint32_t* r, int pitch, const float* wsinv) {
+      acc_ld8(row, c0, r, pitch, wsinv);
+      acc_ld8(row, c0 + 8, r + 8, pitch, wsinv);
     };
     const int h_plane = (TC_TILE + p.MIR) * 16;  // fused: bytes per chunk plane of the hidden operand buffer
     // this warp is done reading the accumulator tile
@@ -609,52 +660,76 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
       build_window(w, std::integral_constant<int, 2>{});
       if (ew == 0 && lane == 0) TL(1, 10, w);
     };
-    if (!q.in_mode) help_window(0);
+    if (!q.in_mode && (!FUSED || n_my > 0)) help_window(0);
 
     for (int i = 0; i < n_my; ++i) {
       const int u = tile_of(i);
       // per stage: help with the next tile's window before this tile's epilogue, which then runs under its MMAs
       if (!FUSED && !q.in_mode && i + 1 < n_my) help_window(i + 1);
       const SlotInfo si_all = decode_slot(p, u * TC_TILE + sl, HW);
-      // the accumulator tile's uses: one per tile, or (fused) 0 for the run's halo block, then 2i + 1 for the hidden
-      // stage and 2i + 2 for the heads.  Each epilogue issues its first input loads (context, z), which do not depend on
-      // the MMAs, before waiting on it
+      // the accumulator tile's uses: one per tile, or (fused) 0 for the run's halo block if it has one, then 2i + W0 for
+      // the hidden stage and 2i + 1 + W0 for the heads.  Each epilogue issues its first input loads (context, z), which
+      // do not depend on the MMAs, before waiting on it
       auto acc_wait = [&](uint32_t parity, int tag) {
         mbar_wait(&bars[LB_ACC_FULL], parity);
         if (ew == 0 && lane == 0) TL(1, tag, i);
       };
 
-      // hidden stage epilogue: the next operand (global image, or the fused kernel's shared-memory buffer).  Warp ew
-      // covers slots [32 qd, +32).  Fused: two threads per slot, channels [8 cg, +8) of each 16-channel group, all eight
-      // warps on one group at a time, so that the buffer goes to the heads MMAs chunk by chunk, the first after an
-      // ngroups-th of the epilogue.  Per stage: one thread per slot and 16 channels, groups cg, cg + 2, ...  Every
-      // element is computed the same way under either mapping.  Fused, the rows go to buffer rows [row0, +TC_TILE);
-      // the halo block's epilogue keeps rows [0, MIR) and hands nothing over (tile 0's chunk handoffs cover its rows).
+      // hidden stage epilogue: the next operand (global image, or the fused kernel's shared-memory buffer) for slots
+      // TC_TILE u + row0 + [0, TC_TILE).  Warp ew covers slots [32 qd, +32).  Fused: two threads per slot, channels
+      // [8 cg, +8) of each 16-channel group, all eight warps on one group at a time, so that the buffer goes to the heads
+      // MMAs chunk by chunk, the first after an ngroups-th of the epilogue.  Per stage: one thread per slot and 16
+      // channels, groups cg, cg + 2, ...  The halo block's epilogue covers only its first MIR slots, all eight warps
+      // over them: warp ew takes slots [32 (ew / HWP), +32) and channels [8 (ew % HWP), +8), every 8 HWP, with HWP = 8
+      // warps per 32 slots, or 4 for MIR > 32 -- one 8-channel chunk per thread at c2a, so that its latency is short.
+      // Every element is computed the same way under each mapping.  Fused, the rows go to buffer rows [row0, +TC_TILE);
+      // the halo block's epilogue hands nothing to its own heads MMAs (tile 0's chunk handoffs cover its rows).  A pair's
+      // giver (desc) also writes them to rows [0, MIR) of its receiver's buffer (rank 1 of the cluster, fz_run) and
+      // arrives on the receiver's LB_H_HALO.
       constexpr int HC = FUSED ? 8 : 16;  // channels per thread and group
-      auto hidden_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch, const SlotInfo si,
+      auto hidden_epi = [&](const IafTcStage& St, const float* tb, const int ngroups, const int pitch,
                             uint32_t acc_parity, const int row0, const bool halo) {
+        const int HWP = p.MIR > 32 ? 4 : 8;
+        const int sr = halo ? 32 * (ew / HWP) + lane : sl;  // this thread's slot row
+        const SlotInfo si = decode_slot(p, u * TC_TILE + row0 + sr, HW);
         const bool bx0 = (si.x == 0), bxW = (si.x == p.W - 1), byH = (si.y == p.H - 1);
-        // store_row: the halo block writes buffer rows [0, MIR) only (its later rows are the first tile's own).
-        // keep_row: every slot's fp32 activations (hid_out) are written once.  The halo block keeps its rows [0, MIR); a
-        // fused tile keeps its last MIR rows, the next tile's first, only when the next tile is in its run (otherwise the
-        // next run's halo block keeps them)
-        const bool store_row = !halo || sl < p.MIR;
-        const bool keep_row = halo ? sl < p.MIR : (!FUSED || sl + p.MIR < TC_TILE || i + 1 < n_my);
+        // store_row: the halo block writes MIR buffer rows only (its later rows are the first tile's own).
+        // keep_row: every slot's fp32 activations (hid_out) are written once.  The halo block keeps its MIR rows.  Where
+        // a tile upwards computes its last MIR rows, the next tile's first, it keeps them only when the next tile is in
+        // its run: otherwise they are the first rows of a run that starts there (kept by its halo block, or by its
+        // giver's) or of a run that ends there downwards (kept by its last tile, which keeps all its rows)
+        const bool store_row = !halo || sr < p.MIR;
+        const bool keep_row = halo ? sr < p.MIR : (!FUSED || desc() || sr + p.MIR < TC_TILE || i + 1 < n_my);
+        const bool send = FUSED && halo && desc();
         auto store_operand = [&](const float* v8, int chunk) {
           if (FUSED) {
-            uint8_t* dst = smem + q.sm_h + chunk * h_plane + (row0 + sl) * 16;
-            if (store_row) split_store8(v8, dst, dst + (St.N >> 3) * h_plane);
+            const int lo = (St.N >> 3) * h_plane;
+            uint8_t* dst = smem + q.sm_h + chunk * h_plane + (row0 + sr) * 16;
+            if (store_row) {
+              uint4 vh, vl;
+              split8(v8, vh, vl);
+              *reinterpret_cast<uint4*>(dst) = vh;
+              *reinterpret_cast<uint4*>(dst + lo) = vl;
+              if (send) {
+                const uint32_t r = cluster_map(smem + q.sm_h + chunk * h_plane + sr * 16, 1);
+                st_cluster16(r, vh);
+                st_cluster16(r + lo, vl);
+              }
+            }
           } else {
-            const size_t go = ((size_t)chunk * q.S_pad + (size_t)u * TC_TILE + sl) * 8;
+            const size_t go = ((size_t)chunk * q.S_pad + (size_t)u * TC_TILE + sr) * 8;
             split_store8(v8, reinterpret_cast<uint8_t*>(q.o_hi + go), reinterpret_cast<uint8_t*>(q.o_lo + go));
           }
         };
-          // context of the NEXT column group is fetched while the current one is computed
-          const int g0 = FUSED ? 0 : cg, gs = FUSED ? 1 : CGS, co = FUSED ? 8 * cg : 0;
+          // this thread's HC columns: from c_first, every c_step.  The context of the NEXT ones is fetched while the
+          // current ones are computed
+          const int nc = 16 * ngroups;
+          const int c_first = !FUSED ? 16 * cg : halo ? 8 * (ew % HWP) : 8 * cg;
+          const int c_step = !FUSED ? 16 * CGS : halo ? 8 * HWP : 16;
           float cxn[HC];
-          auto fetch_ctx = [&](int g) {
-            if (q.first && si.valid && g < ngroups) {  // += context   (ar.py:402 / layers.py:163)
-              const float* cp = p.ctx + ((size_t)si.n * St.N + g * 16 + co) * HW + si.gp;
+          auto fetch_ctx = [&](int c0) {
+            if (q.first && si.valid && c0 < nc) {  // += context   (ar.py:402 / layers.py:163)
+              const float* cp = p.ctx + ((size_t)si.n * St.N + c0) * HW + si.gp;
   #pragma unroll
               for (int e = 0; e < HC; ++e) cxn[e] = __ldg(cp + (size_t)e * HW);
             } else {
@@ -662,29 +737,30 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
               for (int e = 0; e < HC; ++e) cxn[e] = 0.f;
             }
           };
-          fetch_ctx(g0);
+          fetch_ctx(c_first);
           if (FUSED && !halo && i >= 1) {
             // fused: refill the buffer once the heads MMAs of tile i - 1 have read it, first carrying its rows
-            // [TC_TILE, TC_TILE + MIR) to the front (every plane), all of them read before any warp overwrites them
+            // [TC_TILE, TC_TILE + MIR) to the front, or downwards its rows [0, MIR) to the back (every plane), all of
+            // them read before any warp overwrites them
             mbar_wait(&bars[LB_H_EMPTY], (uint32_t)((i - 1) & 1));
+            const int from = desc() ? 0 : TC_TILE, to = desc() ? TC_TILE : 0;
             for (int k = et; k < 2 * (St.N >> 3) * p.MIR; k += LY_ETHREADS) {
               const int pl = k / p.MIR, rw = k - pl * p.MIR;
               uint4* rows = reinterpret_cast<uint4*>(smem + q.sm_h + pl * h_plane);
-              rows[rw] = rows[TC_TILE + rw];
+              rows[to + rw] = rows[from + rw];
             }
             epi_bar_sync();
             if (ew == 0 && lane == 0) TL(1, 24, i);
           }
           acc_wait(acc_parity, halo ? 13 : 25);
-          for (int g = g0; g < ngroups; g += gs) {
-            const int c0 = g * 16 + co;  // this thread's HC columns
+          for (int c0 = c_first; c0 < nc; c0 += c_step) {
             float cx[HC];
   #pragma unroll
             for (int e = 0; e < HC; ++e) cx[e] = cxn[e];
-            fetch_ctx(g + gs);
+            fetch_ctx(c0 + c_step);
             uint32_t r[HC];
-            if (HC == 8) acc_ld8(c0, r, pitch, St.wsinv);
-            else acc_ld16(c0, r, pitch, St.wsinv);
+            if (HC == 8) acc_ld8(sr, c0, r, pitch, St.wsinv);
+            else acc_ld16(sr, c0, r, pitch, St.wsinv);
             if (q.bwd) {
               // data gradient: acc = (c W)^T g (scaled units); / c (exact: a power of two), x nl'(h), evaluated from the
               // activation itself
@@ -756,12 +832,18 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
   #pragma unroll
             for (int hch = 0; hch < HC / 8; ++hch) store_operand(v + 8 * hch, (c0 >> 3) + hch);
             }
-            if (FUSED && !halo) {  // chunk g of the buffer (both of its planes, all slots) goes to the heads MMAs
+            if (FUSED && !halo) {  // chunk c0 / 16 of the buffer (both of its planes, all slots) goes to the heads MMAs
               fence_proxy_async();  // generic-proxy stores -> the heads' wgmma reads of the buffer
               __syncwarp();
-              if (lane == 0) mbar_arrive(&bars[LB_H_FULL + g]);
-              if (ew == 0 && lane == 0) TL(1, 26 + g, i);
+              if (lane == 0) mbar_arrive(&bars[LB_H_FULL + (c0 >> 4)]);
+              if (ew == 0 && lane == 0) TL(1, 26 + (c0 >> 4), i);
             }
+          }
+          if (send) {  // the receiver's rows are written: its heads MMAs (async proxy) may read them
+            fence_proxy_async_cluster();
+            __syncwarp();
+            if (lane == 0) mbar_arrive_cluster(cluster_map(&bars[LB_H_HALO], 1));
+            if (ew == 0 && lane == 0) TL(1, 16, i);
           }
       };
       // heads epilogue: affine update, per-element and per-sample outputs
@@ -810,7 +892,7 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
             fetch_z(g + CGS);
             const size_t gi = si.valid ? ((size_t)si.n * p.C + ch0) * HW + si.gp : 0;
             uint32_t r[16];
-            acc_ld16(c0, r, pitch, St.wsinv);
+            acc_ld16(sl, c0, r, pitch, St.wsinv);
             const bool set_hi = ((g - cg) / CGS) & 1;
             if (PERCH) {
   #pragma unroll
@@ -902,29 +984,30 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
 
       const float* tb0 = reinterpret_cast<const float*>(smem + q.sm_bias);
       if (FUSED) {
-        if (i == 0) {
-          // the first tile's window (once the halo block's MMAs have read theirs), then the halo block's epilogue under
-          // the first tile's hidden MMAs: rows [0, MIR) of the buffer
-          help_window(1);
-          hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, 0u, 0, true);
+        if (i == 0 && W0()) {
+          // the first tile's window (once the halo block's MMAs have read theirs) and the halo block's epilogue under
+          // the first tile's hidden MMAs: buffer rows [0, MIR) upwards, [TC_TILE, TC_TILE + MIR) downwards.  A giver
+          // hands its halo over first, since its receiver's first heads MMAs wait for it
+          if (!desc()) help_window(1);
+          hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), 0u, desc() ? TC_TILE : 0, true);
           acc_release();
           if (ew == 0 && lane == 0) TL(1, 14, i);
+          if (desc()) help_window(1);
         }
         // the hidden epilogue runs under the heads MMAs of its earlier chunks, the heads epilogue under the next tile's
-        // hidden MMAs
-        hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), decode_slot(p, u * TC_TILE + p.MIR + sl, HW), 1u, p.MIR,
-                   false);
+        // hidden MMAs.  Buffer rows [MIR, TC_TILE + MIR) upwards, [0, TC_TILE) downwards
+        hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), (uint32_t)W0(), desc() ? 0 : p.MIR, false);
         acc_release();
         if (ew == 0 && lane == 0) TL(1, 30, i);
         // under the heads MMAs: the rest of the next tile's window, beside the builder warps
-        if (i + 1 < n_my) help_window(i + 2);
+        if (i + 1 < n_my) help_window(i + 1 + W0());
         const IafTcStage& St1 = p.st[1];
-        heads_epi(St1, reinterpret_cast<const float*>(smem + q.sm_bias1), St1.N >> 4, ly_acc_pitch(St1.N), si_all, 0u,
-                  45);
+        heads_epi(St1, reinterpret_cast<const float*>(smem + q.sm_bias1), St1.N >> 4, ly_acc_pitch(St1.N), si_all,
+                  (uint32_t)(1 - W0()), 45);
         acc_release();
         if (ew == 0 && lane == 0) TL(1, 50, i);
       } else {
-        if (!q.is_heads) hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, (uint32_t)(i & 1), 0, false);
+        if (!q.is_heads) hidden_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), (uint32_t)(i & 1), 0, false);
         else heads_epi(St0, tb0, St0.N >> 4, ly_acc_pitch(St0.N), si_all, (uint32_t)(i & 1), 25);
         acc_release();
         if (ew == 0 && lane == 0) TL(1, 30, i);
@@ -932,7 +1015,9 @@ __global__ void __launch_bounds__(LY_THREADS, 1) iaf_ly_kernel(const __grid_cons
     }
   }
 
-  __syncthreads();
+  // paired: neither CTA of the cluster exits while the other may still write to or arrive on its shared memory
+  if (FUSED && q.paired) cluster_sync();
+  else __syncthreads();
   if (q.tl_enable) {
     if (tid == 0) TL(1, 98, MODE);
     if (tid == 0) TL(1, 99, n_my);

@@ -2,10 +2,13 @@
 source is newer), run one IAF step of a bench.py workload and print the in-kernel timeline of CTA 0 (see TL() in
 iaf_b200/csrc/iaf_tc.cu), then the cycles of every phase per tile and the producer's ring waits.
 
-    python tools/tl_run.py [workload] [stage]
+    python tools/tl_run.py [workload] [stage] [--cta B]
 
 stage: which launch of a per-stage step records (IAF_TL_STAGE; default the last).  A one-launch step always records.
+--cta: the CTA that records (default 0).  In a one-launch step of CTA pairs, an odd B is a receiver and an even B a
+giver; at c2a on 132 SMs, CTA 3 is a receiver of 5 tiles.
 """
+import argparse
 import ctypes
 import io
 import os
@@ -26,21 +29,24 @@ PHASE = {15: "MMA operands ready", 20: "MMAs done", 21: "acc tile written", 35: 
          40: "heads MMAs done", 41: "heads acc written", 10: "window built", 25: "acc ready", 30: "(hidden) epilogue done",
          45: "heads acc ready", 50: "heads epilogue done", 99: "end",
          # one launch: the run's halo block (before its first tile) and the carry of each later tile's first MIR rows
-         12: "halo MMAs done", 13: "halo acc ready", 14: "halo epilogue done", 24: "carry done"}
+         12: "halo MMAs done", 13: "halo acc ready", 14: "halo epilogue done", 24: "carry done",
+         # CTA pairs: the giver's halo rows written to its receiver, and received there before its first heads MMAs
+         16: "halo sent", 36: "halo received"}
 PHASE.update({26 + c: "hidden chunk %d ready" % c for c in range(4)})
 ROLE = {0: "MMA warpgroups", 1: "epilogue warps", 3: "window builders"}
 
 
-def run(name, stage):
+def run(name, stage, cta):
     if stage is not None:
         os.environ["IAF_TL_STAGE"] = str(stage)
     dev = torch.device("cuda:0")
     op, layers, sets = make_workload(name, dev, 2)
     s = sets[0]
+    lib = ctypes.CDLL(B.LIB)
+    lib.iaf_tc_timeline_cta(cta)
     for _ in range(3):
         op.step(s["z"], s["ctx"])
     torch.cuda.synchronize()
-    lib = ctypes.CDLL(B.LIB)
     lib.iaf_tc_timeline_dump()  # discard warm-up events
     op.step(s["z"], s["ctx"])
     torch.cuda.synchronize()
@@ -61,16 +67,17 @@ def run(name, stage):
             d = dict(x.split("=") for x in line.split()[1:])
             ev.append((int(d["t"]), int(d["role"]), int(d["tag"]), int(d["k"])))
     ev.sort()
-    print("=== %s, stage %s: %d events ===" % (name, "last" if stage is None else stage, len(ev)))
+    print("=== %s, stage %s, CTA %d: %d events ===" % (name, "last" if stage is None else stage, cta, len(ev)))
     for t, role, tag, k in ev:
         print("%9d  role%d  %-24s k=%d" % (t, role, PHASE.get(tag, {60: "ring wait", 61: "ring released"}.get(tag, tag)), k))
     # tile period: from one tile's heads accumulators written to the next's, on the MMA side
     ends = [t for t, role, tag, _ in ev if role == 0 and tag == 41]
     tiles = [k for _, role, tag, k in ev if role == 1 and tag == 99]
     if tiles:
-        print("--- CTA 0 ran %d tiles ---" % tiles[0])
+        print("--- CTA %d ran %d tiles ---" % (cta, tiles[0]))
     if ends:
-        # the run's first tile, halo block included: from the first event (the first window) to its heads accumulators
+        # the run's first tile, halo block (if any) included: from the first event (the first window) to its heads
+        # accumulators
         print("--- first tile (MMA side, from the first event): %d cycles ---" % (ends[0] - ev[0][0]))
     if len(ends) > 1:
         print("--- tile period (MMA side): %s cycles ---" % " ".join(str(b - a) for a, b in zip(ends, ends[1:])))
@@ -91,5 +98,9 @@ def run(name, stage):
 
 
 if __name__ == "__main__":
-    name = sys.argv[1] if len(sys.argv) > 1 else "c2a"
-    run(name, int(sys.argv[2]) if len(sys.argv) > 2 else None)
+    ap = argparse.ArgumentParser()
+    ap.add_argument("workload", nargs="?", default="c2a")
+    ap.add_argument("stage", nargs="?", type=int, default=None)
+    ap.add_argument("--cta", type=int, default=0)
+    a = ap.parse_args()
+    run(a.workload, a.stage, a.cta)
